@@ -308,51 +308,73 @@ __global__ void __launch_bounds__(256) k_shade_miss(DevScene sc, DevConfig cfg, 
     if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&ctr->misses, (unsigned long long)n); atomicAdd(&ctr->shade_invocations, (unsigned long long)n); }
 }
 
-// SH/RayGen.slang:92-113 for a path that was shaded at a hit: contribution (luminance clamp unless Depth == 1, Q3), throughput update, Russian
-// roulette (Q4), loop condition.  Returns whether the path continues; a finished path is folded into its sample slot (:116-128).
-__device__ __forceinline__ bool path_epilogue(const DevConfig &cfg, float3 emitted, float4 b4, uint32_t newDepth, int channel, float4 thr4, float4 r4, Rng &rng,
-                                              float3 &thr, float3 &rad, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
-    thr = f3(thr4); rad = f3(r4);
-    float3 contribution = emitted * thr;
-    if (newDepth != 1u) {                                                   // Q3
-        const float lum = dot(contribution, f3(0.212671f, 0.715160f, 0.072169f));
-        const float scale = cfg.MaxLuminance / fmaxf(lum, cfg.MaxLuminance);
-        contribution = contribution * scale;
-    }
-    rad = rad + contribution;
-    thr = thr * (f3(b4) / b4.w);
+// SH/RayGen.slang:92-113 for a path that was shaded at a hit, in two parts: path_roulette (throughput update, Russian roulette (Q4), loop
+// condition) does not depend on the NEE terms, so the fused bounce kernel decides a path's next segment before its shadow queries are traced;
+// path_radiance (contribution, luminance clamp unless Depth == 1 (Q3), radiance; a finished path is folded into its sample slot, :116-128)
+// runs once they are joined.  k_connect calls both in sequence.
+// The join and every product / sum of the epilogue are written with explicitly rounded operations, in the form k_connect compiled to when
+// its inputs came from memory: a value that stays in registers (the fused kernels) must not be contracted into an FMA that the unfused
+// pipeline, whose NEE terms and BxDF pass through HBM, cannot form.  Fused and unfused images are then bit-identical.
+__device__ __forceinline__ float3 add_rn(float3 a, float3 b) { return f3(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z)); }
+__device__ __forceinline__ float3 mul_rn(float3 a, float3 b) { return f3(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y), __fmul_rn(a.z, b.z)); }
+__device__ __forceinline__ float3 nee_join(float3 emitted, float3 c) { return add_rn(emitted, c); }   // payload.Emitted += NEE term (sky, then light)
+__device__ __forceinline__ bool path_roulette(const DevConfig &cfg, float4 b4, uint32_t newDepth, float4 thr4, Rng &rng, float3 &thr) {
+    thr = mul_rn(f3(thr4), f3(b4) / b4.w);
     float p = fmaxf(thr.x, fmaxf(thr.y, thr.z));
     p = fminf(p, 1.0f);
     const float u = rng.next();                                             // Q4
     bool alive = !(p < u);
     if (alive) thr = thr / p;
-    alive = alive && (newDepth < cfg.MaxDepth);                             // loop condition :66
+    return alive && (newDepth < cfg.MaxDepth);                              // loop condition :66
+}
+__device__ __forceinline__ float3 path_radiance(const DevConfig &cfg, float3 emitted, uint32_t newDepth, int channel, float4 thr4, float4 r4, bool alive, uint32_t rng_state,
+                                                float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
+    float3 contribution = mul_rn(emitted, f3(thr4));
+    if (newDepth != 1u) {                                                   // Q3: dot(contribution, luminance weights)
+        const float lum = __fmaf_rn(contribution.z, 0.072169f, __fmaf_rn(contribution.x, 0.212671f, __fmul_rn(contribution.y, 0.715160f)));
+        const float scale = cfg.MaxLuminance / fmaxf(lum, cfg.MaxLuminance);
+        contribution = mul_rn(contribution, f3(scale));
+    }
+    const float3 rad = add_rn(f3(r4), contribution);
     if (!alive) {                                                           // path finished: :116-128 (+ carry RNG for SampleCount > 1)
         const uint32_t slot = __float_as_uint(r4.w);
         const bool ok = !isinf(rad.x) && !isinf(rad.y) && !isinf(rad.z) && !isnan(rad.x) && !isnan(rad.y) && !isnan(rad.z);
         float4 acc = sample_buf[slot];
         if (ok) add_path_light(acc, rad, channel);
         sample_buf[slot] = acc;
-        rng_carry[slot] = rng.s;
+        rng_carry[slot] = rng_state;
     }
-    return alive;
+    return rad;
 }
 
 // ------------------------------------------------------------------------------------------------
 // k_shade_hit<CLASS, VOL, FUSE> : SH/ClosestHit.slang:20-378 for the hit queue of one material class.
 //   FUSE == 0  writes the new ray + payload in place and <= 2 NEE shadow requests; k_connect (or k_shadow_dyn + k_connect) finishes the bounce.
-//   FUSE >= 1  "k_bounce" for scenes whose BVH is staged in shared memory (no volumes): each NEE request is traced the moment it is built
-//              (one copy of the any-hit traversal inside the rolled NEE loop), then SH/RayGen.slang:92-113 runs in the same thread and the
-//              survivor is written compacted to the other PathState buffer -- no request / payload round trip through HBM, no k_connect.
-//   FUSE == 2  additionally traces the survivor's NEXT segment (the next bounce's k_extend) and appends it to the next bounce's miss / class
-//              queues: one kernel per (bounce, class), 80 B read + 84 B written per continuing path.
+//   FUSE == 1  for scenes whose BVH is staged in shared memory (no volumes): each NEE request is traced the moment it is built (one copy of
+//              the any-hit traversal inside the rolled NEE loop), then SH/RayGen.slang:92-113 runs in the same thread and the survivor is
+//              written compacted to the other PathState buffer -- no request / payload round trip through HBM, no k_connect.
+//   FUSE == 2  the bounce kernel of shared-memory scenes (the default there): one kernel per (bounce, class) that also traces the survivor's
+//              NEXT segment (the next bounce's k_extend) and appends it to the next bounce's miss / class queues.  A warp iteration (32 queue
+//              entries) runs in three phases:
+//                shade     up to the NEE requests, which are written to the warp's ray list in shared memory instead of being traced;
+//                roulette  path_roulette decides the path's fate (shadow queries consume no random numbers when this kernel runs: no
+//                          volumes, no atmosphere), a survivor appends its next segment to the same list;
+//                trace     the warp traces the list densely, one entry per lane and round (one copy of the traversal, query kind chosen
+//                          per ray), then each owner joins its visible NEE terms, finishes or compacts its path and queues the next segment.
+//              Per continuing path: 80 B read + 84 B written.
 // ------------------------------------------------------------------------------------------------
 #ifndef SHADE_MIN_BLOCKS
 #define SHADE_MIN_BLOCKS 5
 #endif
-#ifndef BOUNCE_MIN_BLOCKS
-#define BOUNCE_MIN_BLOCKS 5
+#ifndef BOUNCE_MIN_BLOCKS                                                   // 4 x 128 threads: 128 registers, no spills (at 5 the 96-register cap spills 84-140 B)
+#define BOUNCE_MIN_BLOCKS 4
 #endif
+// Ray list of k_shade_hit<., ., 2> (dynamic shared memory after the stacks and the BVH): per warp up to 3 rays per lane -- sky, light,
+// next segment.  Entry e = two float4: [2e] origin + tmax, [2e+1] direction + target word (0xFFFFFFFF: sky, RAY_NEXT: the next segment's
+// closest-hit query, otherwise the sampled light triangle).  The traversal writes its hit record (t, u, v, gid) over [2e].
+constexpr uint32_t RAY_LIST_PER_WARP = 96;
+constexpr size_t RAY_LIST_BYTES_PER_WARP = (size_t)RAY_LIST_PER_WARP * 2 * sizeof(float4);
+constexpr uint32_t RAY_NEXT = 0xFFFFFFFEu;
 // BIG: 512-thread CTAs, one per SM -- for BVHs of 64..~170 KiB, which fit shared memory only once per SM (config 4's glass scene: 108 KiB).
 template <uint32_t CLASS, bool VOL, int FUSE, bool BIG = false>   // VOL: the scene has AABB volumes (volumes.cuh) -- volume events in the hit queue are skipped, NEE terms get the transmittance
 __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_BLOCKS : SHADE_MIN_BLOCKS)) k_shade_hit(DevScene sc, DevConfig cfg, PathState ps, PathState dst, ShadeOut so,
@@ -362,10 +384,18 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
     constexpr uint32_t LOBES = class_lobes(CLASS);
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
+    __shared__ uint32_t list_count[FUSE == 2 ? (BIG ? 16 : 4) : 1];           // entries in each warp's ray list
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
     const int stride = blockDim.x;
     BvhView bv;
     if (FUSE) bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
+    float4 *list = nullptr; uint32_t *list_n = nullptr;
+    if (FUSE == 2) {
+        list = reinterpret_cast<float4 *>(smem + (size_t)max_stack * blockDim.x * sizeof(int) + sc.bvh_bytes) + (threadIdx.x >> 5) * (2u * RAY_LIST_PER_WARP);
+        list_n = list_count + (threadIdx.x >> 5);
+        if ((threadIdx.x & 31u) == 0u) *list_n = 0u;
+        __syncwarp();
+    }
     const uint32_t n = ctrl[CTRL_Q + 8u * parity + 1u + CLASS];
     const uint32_t *__restrict__ q_hit = q.hit + (size_t)CLASS * q.cap;
     uint32_t *qc_next = ctrl + CTRL_Q + 8u * (parity ^ 1u);
@@ -381,6 +411,7 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
     if (j < n) { i_nx = q_hit[j]; h4_nx = hit_in[i_nx]; }
     const uint32_t n_loop = FUSE ? ((n + 31u) & ~31u) : n;                  // fused: warps stay converged for the compaction collectives
     for (; j < n_loop; j += jstep) {
+        if (FUSE == 2) __syncwarp();                                        // the previous iteration's list reads and counter reset are done
         const bool valid = j < n;
         // ---- results of the shading part, consumed by the fused tail
         bool shaded = false;                                                // this lane holds a path whose bounce must be finished (fused)
@@ -388,6 +419,8 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
         float4 b4 = zero4; uint32_t newDflags = 0u; Rng rng; rng.s = 0u;
         bool entered = false;
         const DevMaterial *cmp = nullptr;
+        uint32_t ents = 0xFFFFFFu;                                          // FUSE == 2: list entries of this lane's sky / light / next-segment rays (8 bits each, 0xFF: none)
+        float3 c_sky = f3(0.0f), c_lit = f3(0.0f);                          // FUSE == 2: their NEE terms, joined once the visibility is known
         const uint32_t i = i_nx;
         if (valid) do {
             const float4 h4 = h4_nx;
@@ -517,7 +550,8 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                 const bool contributes = need && e.PDF > 0.0f;
                 if (contributes || (k == 0 && (cfg.EnableAtmosphere || (VOL && sc.n_grids)) && cfg.EnableSkyMIS)) {   // grid volumes: same reason (:332-333)
                     const float3 c = contributes ? (((e.BxDF * 1.0f) * f3(lv)) / lv.w) * power_heuristic(lv.w, e.PDF) : f3(0.0f);
-                    const float3 ro = (k == 0) ? sf.WorldPos + sf.Normal * 1e-5f : sf.WorldPos + toW * 1e-2f;   // :139, :171
+                    // :139, :171 -- rounded like the unfused kernel, which stores the origin (product and sum apart, whatever the kernel around it)
+                    const float3 ro = add_rn(sf.WorldPos, (k == 0) ? mul_rn(sf.Normal, f3(1e-5f)) : mul_rn(toW, f3(1e-2f)));
                     if (FUSE) {
                         //   sky   (SH/ClosestHit.slang:139 + :326-358): any hit in (1e-4, 1e6) occludes;
                         //   light (:171-176 + :360-372): the closest hit must be the sampled triangle.  Equivalent occlusion form: the ray hits
@@ -533,10 +567,16 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                             tmax = tL; tmax_test = __uint_as_float(__float_as_uint(tL) + 1u);
                         }
                         n_shadow++;
-                        if (go) {
+                        if (go && FUSE == 2) {                                  // queued; traced with the warp's other rays after the roulette
+                            const uint32_t e = atomicAdd(list_n, 1u);
+                            list[2u * e] = make_float4(ro.x, ro.y, ro.z, tmax);
+                            list[2u * e + 1u] = make_float4(toW.x, toW.y, toW.z, __uint_as_float(k == 0 ? 0xFFFFFFFFu : lgid));
+                            ents = (ents & ~(0xFFu << (8 * k))) | (e << (8 * k));
+                            if (k == 0) c_sky = c; else c_lit = c;
+                        } else if (go) {
                             HitRec hs;
                             const bool occluded = bvh_trace<true, true, false, true, true>(bv, ro, toW, 0.0001f, tmax, hs, stack, stride, max_stack, nullptr, nullptr, lgid, tmax_test);
-                            if (!occluded) emitted = emitted + c;
+                            if (!occluded) emitted = nee_join(emitted, c);
                         }
                     } else {
                         float4 *const po = (k == 0) ? so.sky_o : so.lit_o, *const pd = (k == 0) ? so.sky_d : so.lit_d, *const pc = (k == 0) ? so.sky_c : so.lit_c;
@@ -586,18 +626,44 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
         if (FUSE) {
             // ---- SH/RayGen.slang:92-113, then (FUSE == 2) the next segment's TraceRay, then compaction into the other PathState buffer
             bool alive = false;
-            float4 r4 = zero4; float3 thr = f3(0.0f), rad = f3(0.0f);
+            float4 thr4 = zero4, r4 = zero4; float3 thr = f3(0.0f), rad = f3(0.0f);
             if (shaded) {
-                const float4 thr4 = ps.thr_depth[i]; r4 = ps.rad_slot[i];
-                alive = path_epilogue(cfg, emitted, b4, newDflags & DEPTH_MASK, dflags_channel(newDflags), thr4, r4, rng, thr, rad, sample_buf, rng_carry);
+                thr4 = ps.thr_depth[i]; r4 = ps.rad_slot[i];
+                alive = path_roulette(cfg, b4, newDflags & DEPTH_MASK, thr4, rng, thr);
             }
-            uint32_t code = Q_NONE; HitRec h; h.t = 0.0f; h.u = 0.0f; h.v = 0.0f; h.gid = 0xFFFFFFFFu;
-            if (FUSE == 2 && alive) {
-                const float3 rd2 = normalize_ray(newD);                     // SH/RayGen.slang:70-72 of the next loop iteration
-                const bool hit = bvh_trace<true, false, false, false, true>(bv, newO, rd2, 0.01f, 100000.0f, h, stack, stride, max_stack);
-                code = hit ? hit_code(sc, h.gid) : 0u;
-                n_ext++;
+            uint32_t code = Q_NONE; float4 h4 = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0xFFFFFFFFu));
+            if (FUSE == 2) {
+                if (alive) {                                                // SH/RayGen.slang:70-72 of the next loop iteration, queued
+                    const uint32_t e = atomicAdd(list_n, 1u);
+                    list[2u * e] = make_float4(newO.x, newO.y, newO.z, 100000.0f);
+                    list[2u * e + 1u] = make_float4(newD.x, newD.y, newD.z, __uint_as_float(RAY_NEXT));
+                    ents = (ents & 0x00FFFFu) | (e << 16);
+                    n_ext++;
+                }
+                __syncwarp();
+                // trace the warp's list densely: round r hands entry 32 r + lane to this lane
+                const uint32_t n_rays = *list_n;
+                for (uint32_t e = lane; e < n_rays; e += 32u) {
+                    const float4 a = list[2u * e], b = list[2u * e + 1u];
+                    const uint32_t target = __float_as_uint(b.w);
+                    const bool shadow = target != RAY_NEXT;
+                    HitRec h;
+                    bvh_trace<true, false, false, false, true, true>(bv, f3(a), shadow ? f3(b) : normalize_ray(f3(b)), shadow ? 0.0001f : 0.01f, a.w, h, stack, stride, max_stack,
+                                                                       nullptr, nullptr, target, target == 0xFFFFFFFFu ? a.w : -1.0f, shadow);
+                    list[2u * e] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
+                }
+                __syncwarp();
+                if (lane == 0u) *list_n = 0u;                               // ordered before the next iteration's appends by the __syncwarp there
+                // join in the reference's order: e0, then the sky term, then the light term, each iff its ray came out unoccluded
+                const uint32_t e_sky = ents & 0xFFu, e_lit = (ents >> 8) & 0xFFu, e_ext = ents >> 16;
+                if (e_sky != 0xFFu && __float_as_uint(list[2u * e_sky].w) == 0xFFFFFFFFu) emitted = nee_join(emitted, c_sky);
+                if (e_lit != 0xFFu && __float_as_uint(list[2u * e_lit].w) == 0xFFFFFFFFu) emitted = nee_join(emitted, c_lit);
+                if (alive) {
+                    h4 = list[2u * e_ext];
+                    code = __float_as_uint(h4.w) != 0xFFFFFFFFu ? hit_code(sc, __float_as_uint(h4.w)) : 0u;
+                }
             }
+            if (shaded) rad = path_radiance(cfg, emitted, newDflags & DEPTH_MASK, dflags_channel(newDflags), thr4, r4, alive, rng.s, sample_buf, rng_carry);
             const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alive);
             if (ballot) {
                 uint32_t base = 0;
@@ -618,7 +684,7 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                         } else { mv = ps.medium[i]; mg = ps.medium_g[i]; }
                         dst.medium[k] = mv; dst.medium_g[k] = mg;
                     }
-                    if (FUSE == 2) hit_out[k] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
+                    if (FUSE == 2) hit_out[k] = h4;
                 }
                 if (FUSE == 2) queue_append(code, k, qc_next, q_next, lane);
             }
@@ -715,11 +781,11 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
             //         the closest-hit query) -- bounded by tL and free to stop at the first occluder.
             if (TRACE) n_shadow += (pending & 1u) + (pending >> 1);
             if (!TRACE) {                                                   // surviving bits = unoccluded requests, joined in the reference's order
-                if (pending & 1u) emitted = emitted + (walks ? sky_term(f3(so.sky_c[i]), f3(so.sky_d[i])) : f3(so.sky_c[i]));
+                if (pending & 1u) emitted = WALKS ? emitted + (walks ? sky_term(f3(so.sky_c[i]), f3(so.sky_d[i])) : f3(so.sky_c[i])) : nee_join(emitted, f3(so.sky_c[i]));
                 if (pending & 2u) {
                     float3 c = f3(so.lit_c[i]);
                     if (het) c = c * volumes_transmittance_walk(sc, rng, f3(o4), f3(so.lit_d[i]), litDepth);
-                    emitted = emitted + c;
+                    emitted = WALKS ? emitted + c : nee_join(emitted, c);
                 }
                 pending = 0u;
             }
@@ -728,7 +794,7 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
             if (pending & 1u) {
                 HitRec h;
                 const bool occluded = bvh_trace<SMEM, true, false, false, true>(bv, f3(so4), f3(sd4), 0.0001f, 1000000.0f, h, stack, stride, max_stack);
-                if (!occluded) emitted = emitted + (walks ? sky_term(f3(so.sky_c[i]), f3(sd4)) : f3(so.sky_c[i]));
+                if (!occluded) emitted = WALKS ? emitted + (walks ? sky_term(f3(so.sky_c[i]), f3(sd4)) : f3(so.sky_c[i])) : nee_join(emitted, f3(so.sky_c[i]));
             }
             if (pending & 2u) {
                 const float4 lo4 = so.lit_o[i], ld4_ = so.lit_d[i];
@@ -742,7 +808,7 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
                     if (!occluded) {
                         float3 c = f3(so.lit_c[i]);
                         if (het) c = c * volumes_transmittance_walk(sc, rng, f3(o4), f3(ld4_), litDepth);
-                        emitted = emitted + c;
+                        emitted = WALKS ? emitted + c : nee_join(emitted, c);   // (the walks' products may contract into the join: WALKS keeps its form)
                     }
                 }
             }
@@ -750,7 +816,8 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
             const float4 thr4 = src.thr_depth[i]; r4 = src.rad_slot[i];
             if (!walks) { o4 = src.org_pdf[i]; d4 = src.dir_rng[i]; rng.s = __float_as_uint(d4.w); }
             const float4 b4 = so.bxdf_pdf[i];
-            alive = path_epilogue(cfg, emitted, b4, newDepth, channel, thr4, r4, rng, thr, rad, sample_buf, rng_carry);
+            alive = path_roulette(cfg, b4, newDepth, thr4, rng, thr);
+            rad = path_radiance(cfg, emitted, newDepth, channel, thr4, r4, alive, rng.s, sample_buf, rng_carry);
         }
         // ---- warp ballot + prefix-sum compaction of the live paths
         const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alive);
@@ -1250,6 +1317,10 @@ static constexpr size_t DYN_RING_BYTES_HOST = 8 * 128 * sizeof(uint32_t);
 static size_t trace_smem_bytes(const DevScene &sc, int max_stack, int threads, bool smem) {
     return (size_t)max_stack * threads * sizeof(int) + (smem ? sc.bvh_bytes : 0);
 }
+// k_shade_hit<., ., 2>: stacks + BVH + one ray list per warp
+static size_t bounce_smem_bytes(const DevScene &sc, int max_stack, int threads) {
+    return trace_smem_bytes(sc, max_stack, threads, true) + (size_t)(threads / 32) * RAY_LIST_BYTES_PER_WARP;
+}
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) applies to the CURRENT device only, and the C-ABI lets one process drive several GPUs
 // (b200pt_create(device, ..)): the opt-in is tracked per device ordinal.
@@ -1299,7 +1370,7 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     // Big mode runs the one-ray-per-thread kernels over the shared-memory BVH at 8-16 warps per SM with divergent LDS; the dynamic-fetch kernels
     // over L2 are the default there -> big mode is OPT-IN (B200PT_SMEM_BIG=1).
     bool fits_big = false;
-    if (const char *e = getenv("B200PT_SMEM_BIG")) { if (atoi(e) == 1) fits_big = aligned && !fits_small && (size_t)sc.bvh_bytes + (size_t)lc->max_stack * 512u * sizeof(int) <= 226u * 1024u; }
+    if (const char *e = getenv("B200PT_SMEM_BIG")) { if (atoi(e) == 1) fits_big = aligned && !fits_small && bounce_smem_bytes(sc, lc->max_stack, 512) <= 226u * 1024u; }
     lc->bvh_in_smem = fits_small || fits_big;
     lc->big = fits_big;
     lc->extend_threads = fits_big ? 512 : 256;
@@ -1323,11 +1394,12 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
         lc->dyn_stack = need < cap ? need : cap;
         if (need - lc->dyn_stack > DYN_SPILL) lc->wide = false, lc->dyn_stack = lc->max_stack;   // deeper than shared column + overflow array: BVH2
     }
-    // fused bounce kernel (k_shade_hit<., ., 2>): scenes whose BVH is staged in shared memory and walked one ray per thread.  B200PT_FUSE=0|1|2 overrides
-    // (0: k_shade_hit + k_connect, 1: NEE queries and the path epilogue fused, k_extend separate, 2: next segment's TraceRay fused as well).
-    // The traffic the fused kernels save is not what bounds the Cornell box, while their shadow / extend traversals run inside half-empty warps of a
-    // 65 KB kernel, so k_extend + k_shade_hit + k_connect stay the default and the fused kernels an opt-in.
-    lc->fuse = 0;
+    // fused bounce kernel (k_shade_hit<., ., 2>): the default for scenes whose BVH is staged in shared memory and walked one ray per thread.  It keeps
+    // the NEE requests, the payload and the next segment's origin on chip (~170 B of HBM traffic per shaded hit instead of ~450 B) and traces a warp's
+    // shadow and extension rays together from a shared-memory list, so no traversal runs in a half-empty warp.  Cornell box, H100 SXM at 700 W: see
+    // DESIGN.md section 8.  B200PT_FUSE=0|1|2 overrides (0: k_extend + k_shade_hit + k_connect, 1: NEE queries and the path epilogue fused,
+    // k_extend separate, 2: the default).
+    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? 2 : 0;
     if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if (v >= 0 && v <= 2 && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = (lc->big && v == 1) ? 2 : v; }
     // BVH4 treelet in shared memory (bvh_dynfetch.cuh): the first n_top4 nodes (breadth-first order = the top levels).  B200PT_TOP_KB sizes it (0 = off).
     lc->n_top4 = 0;
@@ -1362,8 +1434,8 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     if (occ_sh < 1) occ_sh = 1;
     lc->grid_shadow = sms * occ_sh;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_shade_hit<MC_GENERAL, false, 0>, 128, 0);
-    if (lc->big) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2, true>, 512, trace_smem_bytes(sc, lc->max_stack, 512, true));
-    else if (lc->bvh_in_smem) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2>, 128, trace_smem_bytes(sc, lc->max_stack, 128, true));
+    if (lc->big) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2, true>, 512, bounce_smem_bytes(sc, lc->max_stack, 512));
+    else if (lc->bvh_in_smem) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2>, 128, bounce_smem_bytes(sc, lc->max_stack, 128));
     if (occ_e < 1) occ_e = 1; if (occ_c < 1) occ_c = 1; if (occ_s < 1) occ_s = 1; if (occ_b < 1) occ_b = 1;
     lc->grid_extend = sms * occ_e; lc->grid_connect = sms * occ_c;
     { int occ_t = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, lc->bvh_in_smem ? k_trace_rays<true> : k_trace_rays<false>, 256, sh256); lc->grid_trace = sms * (occ_t < 1 ? 1 : occ_t); }
@@ -1416,7 +1488,7 @@ int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, 
     set_attrs_for_current_device();
     int launched = 1;
     k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, fuse == 2 ? 1u : 0u, q.miss, sample_buf, rng_carry, ctr);
-    const size_t shb = trace_smem_bytes(sc, lc.max_stack, lc.big ? 512 : 128, true);
+    const size_t shb = fuse == 2 ? bounce_smem_bytes(sc, lc.max_stack, lc.big ? 512 : 128) : trace_smem_bytes(sc, lc.max_stack, 128, true);
 #define B200PT_SHADE(C) do { if (class_mask & (1u << C)) { launched++;                                                                                              \
         if (fuse == 2 && lc.big) k_shade_hit<C, false, 2, true><<<lc.grid_bounce, 512, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr); \
         else if (fuse == 2) k_shade_hit<C, false, 2><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr);      \
