@@ -15,9 +15,8 @@ def run(name, W, H, frames, depth, **kw):
     T.post_process_rows(8, min(H, 24)); T.get_ldr_rows(8, min(H, 24))
     print(name, kw.get("Volumes") is not None, os.environ.get("B200PT_FUSE"), os.environ.get("B200PT_TRAV"), "ok", float(img[..., :3].mean()))
 
-run("cornell_box", 64, 36, 2, 6)                                   # BVH in shared memory (TMA), flat traversal, uniform class
+run("cornell_box", 64, 36, 2, 6)                                   # BVH in shared memory (TMA), flat traversal, uniform class, fused bounce kernel
 os.environ["B200PT_FLAT_MAX"] = "0"; run("cornell_box", 48, 32, 1, 4); del os.environ["B200PT_FLAT_MAX"]      # BVH2 stack traversal in shared memory
-os.environ["B200PT_FUSE"] = "2"; run("cornell_box", 48, 32, 2, 5); del os.environ["B200PT_FUSE"]              # fused bounce kernel
 run("cornell_box", 48, 32, 1, 5, Volumes=[FOG])                     # k_volume_decide / k_shade_volume
 run("cornell_box", 48, 32, 2, 5, EnableAtmosphere=1, SkyRotationAltitude=-30.0)                       # atmosphere: sun NEE, delta tracking, transmittance walks
 run("cornell_box", 40, 30, 1, 5, EnableAtmosphere=1, SkyRotationAltitude=-20.0, Volumes=[FOG])        # atmosphere + homogeneous volume
@@ -30,6 +29,4 @@ run("cornell_box", 40, 30, 1, 5, Volumes=[FOG, _het()])                         
 run("cornell_box", 40, 30, 1, 5, EnableAtmosphere=1, SkyRotationAltitude=-20.0, Volumes=[_het()])    # ... under the atmosphere
 run("cornell_box_glass", 48, 48, 2, 8)                              # dynamic-fetch BVH2 kernels, class queues (glass / diffuse)
 os.environ["B200PT_WIDE"] = "1"; run("viking_room", 48, 48, 1, 4); del os.environ["B200PT_WIDE"]              # BVH4 + textures
-os.environ["B200PT_SORT"] = "1"; os.environ["B200PT_TOP_KB"] = "16"; os.environ["B200PT_WIDE"] = "1"
-run("viking_room", 32, 32, 1, 3)                                    # ray sort + treelet staging (opt-in paths)
 print("sanitize_small done")

@@ -118,19 +118,10 @@ __device__ __forceinline__ int dyn_sel4(float4 ch, uint32_t key) {
     const uint32_t k = key & 3u;
     return __float_as_int(k == 0u ? ch.x : (k == 1u ? ch.y : (k == 2u ? ch.z : ch.w)));
 }
-// Treelet staging: the BVH4 is emitted breadth-first (bvh4_collapse_host), so its first n_top nodes are the top levels every ray walks through.
-// Each CTA copies them into shared memory with TMA bulk copies (stage_top_smem); a node index below n_top is read from there (generic loads:
-// one instruction serves lanes that are in the treelet and lanes that are below it), the rest comes from L2 through L1 as before.
 template <bool FMA_SLABS>
-__device__ __forceinline__ void dyn_node4_step(const float4 *nodes4, const float4 *top, int n_top, DynRay &r, uint32_t s_step, uint32_t s_limit, int *spill) {
-    float4 LX, LY, LZ, HX, HY, HZ, CH;
-    if (n_top > 0) {
-        const float4 *np = (r.cur < n_top ? top : nodes4) + (size_t)r.cur * 8;
-        LX = np[0]; LY = np[1]; LZ = np[2]; HX = np[3]; HY = np[4]; HZ = np[5]; CH = np[6];
-    } else {
-        const float4 *np = nodes4 + (size_t)r.cur * 8;
-        LX = __ldg(np); LY = __ldg(np + 1); LZ = __ldg(np + 2); HX = __ldg(np + 3); HY = __ldg(np + 4); HZ = __ldg(np + 5); CH = __ldg(np + 6);
-    }
+__device__ __forceinline__ void dyn_node4_step(const float4 *nodes4, DynRay &r, uint32_t s_step, uint32_t s_limit, int *spill) {
+    const float4 *np = nodes4 + (size_t)r.cur * 8;
+    const float4 LX = __ldg(np), LY = __ldg(np + 1), LZ = __ldg(np + 2), HX = __ldg(np + 3), HY = __ldg(np + 4), HZ = __ldg(np + 5), CH = __ldg(np + 6);
     uint32_t k0 = dyn_child_key<FMA_SLABS>(r, LX.x, LY.x, LZ.x, HX.x, HY.x, HZ.x, 0u);
     uint32_t k1 = dyn_child_key<FMA_SLABS>(r, LX.y, LY.y, LZ.y, HX.y, HY.y, HZ.y, 1u);
     uint32_t k2 = dyn_child_key<FMA_SLABS>(r, LX.z, LY.z, LZ.z, HX.z, HY.z, HZ.z, 2u);

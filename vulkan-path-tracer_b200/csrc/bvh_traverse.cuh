@@ -55,17 +55,6 @@ __device__ __forceinline__ BvhView stage_bvh_smem(const DevScene &sc, unsigned c
     v.root = sc.root; v.n_flat = sc.n_flat;
     return v;
 }
-// Stage `bytes` (multiple of 16) of read-only data into shared memory: same TMA bulk-copy + mbarrier protocol, used for the BVH4 treelet.
-__device__ __forceinline__ void stage_bytes_smem(unsigned char *dst, const void *src_gmem, uint32_t bytes, uint64_t *bar) {
-    if (threadIdx.x == 0) { mbar_init(bar, 1); }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, bytes);
-        const unsigned char *src = reinterpret_cast<const unsigned char *>(src_gmem);
-        for (uint32_t off = 0; off < bytes; off += 32768u) tma_bulk_g2s(dst + off, src + off, min(32768u, bytes - off), bar);
-    }
-    mbar_wait(bar, 0);
-}
 __device__ __forceinline__ BvhView global_bvh(const DevScene &sc) {
     BvhView v; v.nodes = reinterpret_cast<const float4 *>(sc.nodes); v.tris = reinterpret_cast<const float4 *>(sc.tris); v.root = sc.root; v.n_flat = 0u; return v;
 }

@@ -136,7 +136,6 @@ struct DevScene {
     uint32_t n_emissive, envW, envH, n_tris, n_nodes, n_nodes4;
     int32_t root;            // child-style reference of the root
     uint32_t bvh_bytes;      // nodes+tris size if they are contiguous and small enough to stage in smem, else 0
-    float sort_lo[3], sort_scale[3];   // ray-sort grid: cell = (origin - sort_lo) * sort_scale, 32 cells per axis over the scene box
     uint32_t n_flat;         // != 0: the scene has so few triangle slots that shared-memory traversals test them all in order, no hierarchy (bvh_traverse.cuh)
 };
 

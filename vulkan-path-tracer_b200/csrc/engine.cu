@@ -174,15 +174,7 @@ void Engine::upload_scene() {
         if (const char *e = getenv("B200PT_FLAT_MAX")) { const int v = atoi(e); if (v >= 0 && v <= 64) flat_max = (uint32_t)v; }
         ds_.n_flat = (bvh_.n_tris <= flat_max) ? bvh_.n_tris : 0u;
     }
-    for (int k = 0; k < 3; k++) {                                           // ray-sort grid over the scene box (k_ray_sort_keys)
-        const float ext = bvh_.scene_bounds[3 + k] - bvh_.scene_bounds[k];
-        ds_.sort_lo[k] = bvh_.scene_bounds[k]; ds_.sort_scale[k] = ext > 0.0f ? 32.0f / ext : 0.0f;
-    }
     int q = query_launch_cfg(ds_, bvh_.max_depth, bvh_.depth4, &lc_);
-    // Rays sorted by (origin cell, direction octant) before k_extend_dyn: incoherent traversal is bound by node visits per ray rather than by cache
-    // misses, while the sort and the scattered state reads it causes add work.  OPT-IN: B200PT_SORT=1.
-    sort_rays_ = false;
-    if (const char *e = getenv("B200PT_SORT")) sort_rays_ = atoi(e) != 0 && lc_.trav_dyn;
     if (q != 0) throw CudaError{ B200PT_ERR_CUDA, "query_launch_cfg failed" };
 }
 
@@ -462,11 +454,10 @@ void Engine::free_wave() {
         dfree(B.sample_buf); dfree(B.rng_carry); dfree(B.q_hit[0]); dfree(B.q_hit[1]); dfree(B.q_miss[0]); dfree(B.q_miss[1]);
         B.cap = 0;
     }
-    dfree(d_sort_key_rank_); dfree(d_sort_hist_); dfree(d_sort_offs_); dfree(d_order_);
     wave_cap_ = 0;
 }
 void Engine::ensure_wave(size_t cap, int contexts) {
-    bool ok = cap <= wave_cap_ && (!sort_rays_ || d_order_ != nullptr);
+    bool ok = cap <= wave_cap_;
     for (int c = 0; c < contexts; c++) ok = ok && wb_[c].cap >= cap;
     if (ok) return;
     sync_all();
@@ -481,11 +472,6 @@ void Engine::ensure_wave(size_t cap, int contexts) {
         CK(cudaMalloc(&B.rng_carry, cap * sizeof(uint32_t)));
         for (int i = 0; i < 2; i++) { CK(cudaMalloc(&B.q_hit[i], (size_t)MC_COUNT * cap * sizeof(uint32_t))); CK(cudaMalloc(&B.q_miss[i], cap * sizeof(uint32_t))); }   // one hit queue per material class, ping-pong for the fused bounce kernel
         B.cap = cap;
-    }
-    if (sort_rays_) {                                                        // opt-in ray sort (B200PT_SORT=1, single context): 12 B per path + two bin tables
-        CK(cudaMalloc(&d_sort_key_rank_, cap * sizeof(uint2))); CK(cudaMalloc(&d_order_, cap * sizeof(uint32_t)));
-        CK(cudaMalloc(&d_sort_hist_, SORT_BINS * sizeof(uint32_t))); CK(cudaMalloc(&d_sort_offs_, SORT_BINS * sizeof(uint32_t)));
-        CK(cudaMemsetAsync(d_sort_hist_, 0, SORT_BINS * sizeof(uint32_t), stream_));
     }
     wave_cap_ = cap;
 }
@@ -535,8 +521,8 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     // the image afterwards (get_hdr, post_process, set_hdr, checkpoints, ...) first makes the caller's stream wait for the resolves (join_waves); the next call's
     // resolves in turn wait for what the caller enqueued on the image in between (image_free_ev_).  So consecutive path_trace calls -- the steps of a multi-GPU
     // run, each followed by an NCCL gather of the bands -- overlap as well: the gather of step k runs beside the first bounces of step k + 1.
-    // B200PT_OVERLAP=0 runs one wave at a time on the caller's stream (also used while profiling per-kernel times and with the opt-in ray sort).
-    bool overlap = !profiling_ && !sort_rays_;
+    // B200PT_OVERLAP=0 runs one wave at a time on the caller's stream (also used while profiling per-kernel times).
+    bool overlap = !profiling_;
     if (const char *e = getenv("B200PT_OVERLAP")) { if (atoi(e) == 0) overlap = false; }
     uint32_t F = cfg_.FramesInFlight;
     if (F == 0) {
@@ -612,9 +598,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     const uint32_t par = k & 1u;
                     const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
                     if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
-                    const bool sorted = sort_rays_ && d_order_ != nullptr && k >= 1;   // camera rays are pixel-coherent already
-                    if (sorted) { launch_ray_sort(lc_, ds_, pst[cur], B.counts, par, d_sort_key_rank_, d_sort_hist_, d_sort_offs_, d_order_, st); launches += 3; }
-                    if (fuse != 2 || k == 0) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, sorted ? d_order_ : nullptr, st); launches++; } mark(1);
+                    if (fuse != 2 || k == 0) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
                     launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
                                              fuse, cmask, st); mark(2);
                     if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
@@ -801,20 +785,11 @@ void Engine::post_process_rows(uint32_t y0, uint32_t y1) {
             D[i][0] = std::min(U[i][0], clampr(2 * D[i + 1][0] - 2, i)); D[i][1] = std::max(U[i][1], clampr(2 * D[i + 1][1] + 1, i));
         }
         auto rows_of = [&](const int r[2], int out[2]) { out[0] = r[0]; out[1] = r[1] + 1; };
-        // the small end of the chain inside one cluster launch (k_bloom_small): OPT-IN, whole image only
-        uint32_t ls = mips;
-        if (whole) if (const char *e = getenv("B200PT_POST_SMALL")) { if (atoi(e) == 1) for (uint32_t i = 2; i < mips; i++) if ((uint64_t)mip_wh_[2 * (i - 1)] * mip_wh_[2 * (i - 1) + 1] <= 160u * 1024u) { ls = i; break; } }
-        if (mips > 16) ls = mips;
         int r[2];
         rows_of(D[1], r);
         launch_bloom_down_first(d_image_, W_, H_, d_mips_[1], mip_wh_[2], mip_wh_[3], p, stream_, whole ? nullptr : r);                               // :200-226, i == 0 and i == 1
-        for (uint32_t i = 2; i < ls; i++) { rows_of(D[i], r); launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_, whole ? nullptr : r); }
-        if (ls < mips) {
-            SmallMips sm{}; sm.first = (int)ls; sm.last = (int)mips - 1;
-            for (uint32_t i = ls - 1; i < mips; i++) { sm.mip[i] = d_mips_[i]; sm.w[i] = (int)mip_wh_[2 * i]; sm.h[i] = (int)mip_wh_[2 * i + 1]; }
-            launch_bloom_small(sm, p, stream_);
-        }
-        for (uint32_t i = ls - 1; i > 1; i--) { rows_of(U[i - 1], r); launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_, whole ? nullptr : r); }   // :229-235
+        for (uint32_t i = 2; i < mips; i++) { rows_of(D[i], r); launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_, whole ? nullptr : r); }
+        for (uint32_t i = mips - 1; i > 1; i--) { rows_of(U[i - 1], r); launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_, whole ? nullptr : r); }   // :229-235
         r[0] = (int)y0; r[1] = (int)y1;
         launch_bloom_final(d_image_, d_mips_[1], mip_wh_[2], mip_wh_[3], d_ldr_, (keep_bloom_ && whole) ? d_mips_[0] : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
         bloom_valid_ = keep_bloom_ && whole;

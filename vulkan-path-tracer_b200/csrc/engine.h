@@ -145,8 +145,6 @@ private:
     void sync_all();                                // the caller's stream AND the internal wave streams are idle
     void join_waves();                              // work enqueued on the caller's stream from here on sees every launched wave resolved into the image
     WaveCounters *d_ctr_ = nullptr;
-    uint2 *d_sort_key_rank_ = nullptr; uint32_t *d_sort_hist_ = nullptr, *d_sort_offs_ = nullptr, *d_order_ = nullptr;   // ray sort of incoherent bounces (launch_ray_sort)
-    bool sort_rays_ = false;
     b200pt_counters last_{};
 };
 

@@ -19,7 +19,6 @@ struct LaunchCfg {
     int dyn_stack;      // shared-memory stack entries per thread of the dynamic-fetch kernels (BVH4: overflow goes to local memory)
     bool big;           // bvh_in_smem with a BVH > 64 KiB: one 512-thread CTA per SM for k_extend and the fused bounce kernels
     int extend_threads; // CTA size of k_extend (256, big: 512)
-    int n_top4;         // BVH4 nodes (top levels, breadth-first prefix) staged into shared memory by the dynamic-fetch kernels
     int fuse;           // 0: k_shade_hit + k_connect; 1: NEE queries + path epilogue inside k_shade_hit; 2: + the next segment's TraceRay (one kernel per bounce and class)
     int grid_bounce;    // persistent grid of the fused k_shade_hit instantiations (BVH + stacks in shared memory)
 };
@@ -28,12 +27,7 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
 void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st);
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
-                   WaveCounters *ctr, bool primary, const uint32_t *order, cudaStream_t st);
-// Ray sort for the dynamic-fetch traversal of incoherent bounces: order[0..n) = the live paths of parity `parity` sorted by (origin cell, direction octant).
-// key_rank: n x uint2 scratch, hist / offs: SORT_BINS words each (hist must be zero on entry and is zero again on exit).
-constexpr uint32_t SORT_BINS = 1u << 18;
-void launch_ray_sort(const LaunchCfg &lc, const DevScene &sc, PathState ps, const uint32_t *ctrl, uint32_t parity, uint2 *key_rank, uint32_t *hist, uint32_t *offs,
-                     uint32_t *order, cudaStream_t st);
+                   WaveCounters *ctr, bool primary, cudaStream_t st);
 // k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.
 // fuse != 0: the bounce is finished inside k_shade_hit (dst, q_next, hit_out are written), launch_connect is not called.
 int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in, float4 *hit_out,
@@ -53,8 +47,7 @@ void launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, cons
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
 struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;
                     Bvh4Node *nodes4; uint32_t n_nodes4; int depth4;
-                    float *h_ref_box; uint32_t n_prims;
-                    float scene_bounds[6]; };                              // lo.xyz, hi.xyz of all triangles (world space)                 // host copy of the per-slot reference boxes (only when asked for), triangle count
+                    float *h_ref_box; uint32_t n_prims; };                  // host copy of the per-slot reference boxes (only when asked for), triangle count
 // Builds into ONE contiguous allocation [nodes | tris] (so small scenes can be staged to smem with one bulk copy).
 // Returns cudaError_t as int.
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
@@ -85,9 +78,6 @@ void launch_bloom_down(const float4 *src, uint32_t sw, uint32_t sh, float4 *dst,
 // fused chain: threshold folded into the first down pass (mip 0 is never written) and [last up pass + threshold + tonemap] in one kernel
 void launch_bloom_down_first(const float4 *hdr, uint32_t W, uint32_t H, float4 *mip1, uint32_t dw, uint32_t dh, PostParams p, cudaStream_t st, const int *rows = nullptr);
 void launch_bloom_final(const float4 *hdr, const float4 *mip1, uint32_t mw, uint32_t mh, uchar4 *ldr, float4 *mip0_out, uint32_t W, uint32_t H, PostParams p, cudaStream_t st, const int *rows = nullptr);
-// passes first..last of the chain (down first..last, then up last..first) in one cluster launch; mip[i] / w[i] / h[i] for i in [first-1, last]
-struct SmallMips { float4 *mip[16]; int w[16], h[16]; int first, last; };
-void launch_bloom_small(const SmallMips &m, PostParams p, cudaStream_t st);
 void launch_bloom_up(const float4 *src, uint32_t sw, uint32_t sh, float4 *dst, uint32_t dw, uint32_t dh, PostParams p, cudaStream_t st, const int *rows = nullptr);
 void launch_tonemap(const float4 *hdr, const float4 *bloom0, uchar4 *ldr, uint32_t W, uint32_t H, PostParams p, cudaStream_t st);
 void launch_prepare_materials(DevMaterial *mats, uint32_t first, uint32_t count, cudaStream_t st);   // fills DevMaterial::pre0..pre3

@@ -933,7 +933,6 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
         out->h_ref_box = static_cast<float *>(malloc((size_t)n * 6 * sizeof(float)));
         if (out->h_ref_box) LBVH_CHECK(cudaMemcpy(out->h_ref_box, leaf_box, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
     }
-    LBVH_CHECK(cudaMemcpy(out->scene_bounds, bounds, 6 * sizeof(float), cudaMemcpyDeviceToHost));   // world-space box of the scene (ray-sort grid, engine.cu)
     cudaFree(tmp); cudaFree(aabb); cudaFree(bounds); cudaFree(ksplit); cudaFree(ref_off);
     cudaFree(ref_box); cudaFree(ref_tri); cudaFree(leaf_box); cudaFree(node_box);
     cudaFree(keys); cudaFree(vals); cudaFree(keys2); cudaFree(vals2); cudaFree(hist);

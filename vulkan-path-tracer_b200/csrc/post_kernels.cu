@@ -4,7 +4,6 @@
 // 16-B coalesced accesses; the 16 taps of the down/up filters hit L1/L2 (each source texel is read by 4 neighbours).
 #include "shading.cuh"
 #include "kernels.h"
-#include <cooperative_groups.h>
 
 namespace b200pt {
 
@@ -205,58 +204,6 @@ __global__ void __launch_bounds__(256) k_bloom_final(const float4 *__restrict__ 
     ldr[(size_t)y * W + x] = tonemap_px(f3(tile_h[cy][cx]), bloom_blend(tile[ly0][lx0], tile[ly0][lx1], tile[ly1][lx0], tile[ly1][lx1], t.ax, t.ay), p.Exposure, p.Gamma);
     if (mip0_out) mip0_out[(size_t)y * W + x] = tile[cy][cx];
 }
-
-// The small end of the mip chain in ONE launch: every down pass first..last followed by every up pass last..first (PostProcessor.cpp:200-235
-// for those i).  At 3840x2160 mips 4..9 hold 32 K .. 32 pixels: twelve launches of 4-6 us each (ncu) for ~3 MB of traffic.  Here one
-// thread-block cluster of 8 CTAs x 1024 threads walks the passes with a hardware cluster barrier between them; the data stays in L2
-// (loads / stores bypass the non-coherent L1: ld.global.cg / st.global.cg), the arithmetic is that of k_bloom_down / k_bloom_up to the bit.
-constexpr int SMALL_CLUSTER = 8;
-__global__ void __cluster_dims__(SMALL_CLUSTER, 1, 1) __launch_bounds__(1024) k_bloom_small(SmallMips m, PostParams p) {
-    namespace cg = cooperative_groups;
-    cg::cluster_group cl = cg::this_cluster();
-    const int nthr = SMALL_CLUSTER * 1024, t0 = (int)cl.block_rank() * 1024 + (int)threadIdx.x;
-    for (int i = m.first; i <= m.last; i++) {                               // BloomDownSample.slang:46-64
-        const float4 *src = m.mip[i - 1]; float4 *dst = m.mip[i];
-        const int sw = m.w[i - 1], sh = m.h[i - 1], dw = m.w[i], dh = m.h[i];
-        for (int k = t0; k < dw * dh; k += nthr) {
-            const int x = k % dw, y = k / dw;
-            float3 acc = f3(0.0f);
-            #pragma unroll
-            for (int a = -2; a < 2; a++) {
-                #pragma unroll
-                for (int b = -2; b < 2; b++) {
-                    const int sx = clampi(x * 2 + a, 0, sw - 1), sy = clampi(y * 2 + b, 0, sh - 1);
-                    const float4 s4 = __ldcg(src + (size_t)sy * sw + sx);
-                    acc.x = __fadd_rn(acc.x, s4.x); acc.y = __fadd_rn(acc.y, s4.y); acc.z = __fadd_rn(acc.z, s4.z);
-                }
-            }
-            __stcg(dst + k, make_float4(bloom_scale(acc.x, p.BloomStrength), bloom_scale(acc.y, p.BloomStrength), bloom_scale(acc.z, p.BloomStrength), 1.0f));
-        }
-        cl.sync();
-    }
-    for (int i = m.last; i >= m.first; i--) {                               // BloomUpSample.slang:21-48, added to the finer mip in place
-        const float4 *src = m.mip[i]; float4 *dst = m.mip[i - 1];
-        const int sw = m.w[i], sh = m.h[i], dw = m.w[i - 1], dh = m.h[i - 1];
-        for (int k = t0; k < dw * dh; k += nthr) {
-            const int x = k % dw, y = k / dw;
-            float3 acc = f3(0.0f);
-            #pragma unroll
-            for (int a = -2; a < 2; a++) {
-                #pragma unroll
-                for (int b = -2; b < 2; b++) {
-                    const int sx = clampi(x / 2 + a + 1, 0, sw - 1), sy = clampi(y / 2 + b + 1, 0, sh - 1);
-                    const float4 s4 = __ldcg(src + (size_t)sy * sw + sx);
-                    acc.x = __fadd_rn(acc.x, s4.x); acc.y = __fadd_rn(acc.y, s4.y); acc.z = __fadd_rn(acc.z, s4.z);
-                }
-            }
-            const float4 cur = __ldcg(dst + k);
-            __stcg(dst + k, make_float4(__fadd_rn(bloom_scale(acc.x, p.BloomStrength), cur.x), __fadd_rn(bloom_scale(acc.y, p.BloomStrength), cur.y),
-                                        __fadd_rn(bloom_scale(acc.z, p.BloomStrength), cur.z), 1.0f));
-        }
-        if (i > m.first) cl.sync();
-    }
-}
-void launch_bloom_small(const SmallMips &m, PostParams p, cudaStream_t st) { k_bloom_small<<<SMALL_CLUSTER, 1024, 0, st>>>(m, p); }
 
 // SH/RayGen.slang:130-137 as a stand-alone pass: fold one frame's radiance image into the accumulation image with the running-mean rule
 // lerp(prev, new, 1 / (FrameCount + 1)) -- the "HDR accumulate" stage of BASELINE config 5 (inside PathTrace the same rule runs in k_resolve).

@@ -720,14 +720,6 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
     const uint32_t lane = threadIdx.x & 31u;
     uint32_t n_shadow = 0;
     const uint32_t n_round = (n + 31u) & ~31u;                              // keep warps converged for the ballots
-#ifdef B200PT_CONNECT_PREFETCH
-    // The queue entry of this thread's NEXT path is fetched one iteration ahead and its request header pulled towards L2; the words of the CURRENT path that
-    // are only read after the shadow queries (state, contributions) are pulled towards L2 before the traversals start.
-    const uint32_t jstep = gridDim.x * blockDim.x;
-    uint32_t i_nx = 0;
-    { const uint32_t j0 = blockIdx.x * blockDim.x + threadIdx.x; if (j0 < n) i_nx = hit_entry(q, span, j0); }
-#define B200PT_PF(p) asm volatile("prefetch.global.L2 [%0];" ::"l"(p))
-#endif
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n_round; j += gridDim.x * blockDim.x) {
         const bool active = j < n;
         bool alive = false;
@@ -735,17 +727,8 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
         float3 thr = f3(0.0f), rad = f3(0.0f);
         uint32_t i = 0;
         if (active) {
-#ifdef B200PT_CONNECT_PREFETCH
-            i = i_nx;
-            const float4 e4 = so.e0[i];
-            if (j + jstep < n) { i_nx = hit_entry(q, span, j + jstep); B200PT_PF(so.e0 + i_nx); }
-            B200PT_PF(src.thr_depth + i); B200PT_PF(src.rad_slot + i); B200PT_PF(src.org_pdf + i); B200PT_PF(src.dir_rng + i); B200PT_PF(so.bxdf_pdf + i);
-            if (__float_as_uint(e4.w) & (1u << 29)) { B200PT_PF(so.sky_c + i); }
-            if (__float_as_uint(e4.w) & (1u << 30)) { B200PT_PF(so.lit_o + i); B200PT_PF(so.lit_d + i); B200PT_PF(so.lit_c + i); }
-#else
             i = hit_entry(q, span, j);
             const float4 e4 = so.e0[i];
-#endif
             uint32_t pending = (__float_as_uint(e4.w) >> 29) & 3u;         // bit 0: sky request, bit 1: light request (k_shade_hit)
             newDflags = __float_as_uint(e4.w) & 0x9FFFFFFFu;
             const uint32_t newDepth = newDflags & DEPTH_MASK;
@@ -846,16 +829,14 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
 // ------------------------------------------------------------------------------------------------
 template <bool SMEM, bool PRIMARY, bool WIDE>   // WIDE: BVH4 nodes (sc.nodes4) instead of the BVH2
 __global__ void __launch_bounds__(256) k_extend_dyn(DevScene sc, PathState ps, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl, uint32_t parity,
-                                                     Queues q, int max_stack, int thresh, int n_top, const uint32_t *__restrict__ order, WaveCounters *ctr) {
+                                                     Queues q, int max_stack, int thresh, WaveCounters *ctr) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
     stack[0] = DYN_DONE;
     BvhView bv;
-    const float4 *top = reinterpret_cast<const float4 *>(smem + (size_t)(max_stack + 1) * blockDim.x * sizeof(int));   // BVH4 treelet (WIDE, n_top > 0)
     if (SMEM) bv = stage_bvh_smem(sc, smem + (size_t)(max_stack + 1) * blockDim.x * sizeof(int), &bar);
     else bv = global_bvh(sc);
-    if (WIDE && n_top > 0) stage_bytes_smem(smem + (size_t)(max_stack + 1) * blockDim.x * sizeof(int), sc.nodes4, (uint32_t)n_top * (uint32_t)sizeof(Bvh4Node), &bar);
     const uint32_t n = ctrl[parity];
     if (blockIdx.x == 0 && threadIdx.x == 0) {                              // counters of the NEXT bounce (last used two bounces ago)
         ctrl_reset_parity(ctrl, parity ^ 1u);
@@ -884,7 +865,7 @@ __global__ void __launch_bounds__(256) k_extend_dyn(DevScene sc, PathState ps, f
         if (need) {
             const uint32_t idx = pool.take(need, lane, fetch);
             if (fin) {
-                i = (order != nullptr && idx != DYN_NONE) ? order[idx] : idx;   // sorted bounce: the pool hands out positions of the sorted list (k_ray_sort_*)
+                i = idx;
                 const uint32_t pre = (i != DYN_NONE && sc.pre_pass) ? __float_as_uint(hit_out[i].w) : 0u;
                 if (pre == VOLUME_EVENT) {
                     r.gid = VOLUME_EVENT;                                   // scattered inside a volume / the atmosphere (k_volume_decide): queued as a hit at the next commit, record kept
@@ -904,7 +885,7 @@ __global__ void __launch_bounds__(256) k_extend_dyn(DevScene sc, PathState ps, f
         }
         const int thr_now = pool.empty() ? 1 : thresh;
         do {
-            if (WIDE) { while (r.cur >= 0) dyn_node4_step<!PRIMARY>(nodes4, top, n_top, r, s_step, s_limit, spill); }
+            if (WIDE) { while (r.cur >= 0) dyn_node4_step<!PRIMARY>(nodes4, r, s_step, s_limit, spill); }
             else { while (r.cur >= 0) dyn_node_step<SMEM, !PRIMARY>(bv, r, s_step, s_limit); }
             __syncwarp();
             while (r.cur < 0 && r.cur != DYN_DONE) dyn_leaf_step<SMEM, false, WIDE>(bv, r, s_step, spill);
@@ -913,57 +894,12 @@ __global__ void __launch_bounds__(256) k_extend_dyn(DevScene sc, PathState ps, f
     }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Ray sort (scenes traversed out of L2): after the first bounce the live list is in compaction order -- neighbouring lanes hold unrelated rays,
-// every warp of k_extend_dyn touches 32 different parts of a 40 MB BVH.  A counting sort of the path INDICES by an 18-bit key (15-bit Morton
-// code of the origin's cell in a 32^3 grid over the scene box | direction octant) costs three light passes (~0.3 ms per 16 M paths) and hands
-// k_extend_dyn spatially coherent rays; the hit queues it fills inherit the order, so k_shadow_dyn's origins are coherent too.  The path state
-// itself is not moved.  Order inside a bin is whatever the atomics return: paths are independent, the image does not depend on it.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t morton_spread5(uint32_t v) {           // 5 bits -> every third bit
-    v = (v | (v << 8)) & 0x0000100Fu; v = (v | (v << 4)) & 0x000010C3u; v = (v | (v << 2)) & 0x00001249u; return v;
-}
-__global__ void __launch_bounds__(256) k_ray_sort_keys(DevScene sc, PathState ps, const uint32_t *__restrict__ ctrl, uint32_t parity,
-                                                        uint2 *__restrict__ key_rank, uint32_t *__restrict__ hist) {
-    const uint32_t n = ctrl[parity];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const float4 o4 = ps.org_pdf[i], d4 = ps.dir_rng[i];
-        const int cx = min(31, max(0, (int)((o4.x - sc.sort_lo[0]) * sc.sort_scale[0])));
-        const int cy = min(31, max(0, (int)((o4.y - sc.sort_lo[1]) * sc.sort_scale[1])));
-        const int cz = min(31, max(0, (int)((o4.z - sc.sort_lo[2]) * sc.sort_scale[2])));
-        const uint32_t cell = morton_spread5((uint32_t)cx) | (morton_spread5((uint32_t)cy) << 1) | (morton_spread5((uint32_t)cz) << 2);
-        const uint32_t oct = (d4.x < 0.0f ? 1u : 0u) | (d4.y < 0.0f ? 2u : 0u) | (d4.z < 0.0f ? 4u : 0u);
-        const uint32_t key = (cell << 3) | oct;
-        key_rank[i] = make_uint2(key, atomicAdd(hist + key, 1u));
-    }
-}
-__global__ void __launch_bounds__(1024) k_ray_sort_scan(uint32_t *__restrict__ hist, uint32_t *__restrict__ offs) {   // one block: exclusive scan of SORT_BINS counts, hist cleared
-    __shared__ uint32_t part[1024];
-    constexpr uint32_t PER = SORT_BINS / 1024u;
-    const uint32_t t = threadIdx.x, b0 = t * PER;
-    uint32_t sum = 0;
-    for (uint32_t k = 0; k < PER; k++) sum += hist[b0 + k];
-    part[t] = sum;
-    __syncthreads();
-    for (uint32_t o = 1; o < 1024u; o <<= 1) { const uint32_t v = t >= o ? part[t - o] : 0u; __syncthreads(); part[t] += v; __syncthreads(); }
-    uint32_t run = part[t] - sum;
-    for (uint32_t k = 0; k < PER; k++) { const uint32_t c = hist[b0 + k]; offs[b0 + k] = run; run += c; hist[b0 + k] = 0u; }
-}
-__global__ void __launch_bounds__(256) k_ray_sort_scatter(const uint32_t *__restrict__ ctrl, uint32_t parity, const uint2 *__restrict__ key_rank,
-                                                           const uint32_t *__restrict__ offs, uint32_t *__restrict__ order) {
-    const uint32_t n = ctrl[parity];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint2 kr = key_rank[i];
-        order[__ldg(offs + kr.x) + kr.y] = i;
-    }
-}
-
 // Shadow requests of the hit queues, compacted per warp: ring entry = (path index << 1) | kind (0 sky, 1 light).
 // An occluded ray clears its request bit in e0.w (bit 29 sky, bit 30 light); k_connect<.., false> joins the surviving requests.
 constexpr size_t DYN_RING_BYTES = 8 * 128 * sizeof(uint32_t);              // per-CTA request rings of k_shadow_dyn (dynamic shared memory, after the stacks)
 template <bool SMEM, bool WIDE>
 __global__ void __launch_bounds__(256, 4) k_shadow_dyn(DevScene sc, ShadeOut so, uint32_t *__restrict__ ctrl, uint32_t parity,
-                                                     Queues q, int max_stack, int thresh, int n_top, WaveCounters *ctr) {
+                                                     Queues q, int max_stack, int thresh, WaveCounters *ctr) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
@@ -971,10 +907,8 @@ __global__ void __launch_bounds__(256, 4) k_shadow_dyn(DevScene sc, ShadeOut so,
     const size_t stack_bytes = (size_t)(max_stack + 1) * blockDim.x * sizeof(int);
     uint32_t *ring_all = reinterpret_cast<uint32_t *>(smem + stack_bytes);  // 128 entries per warp
     BvhView bv;
-    const float4 *top = reinterpret_cast<const float4 *>(smem + stack_bytes + DYN_RING_BYTES);   // BVH4 treelet (WIDE, n_top > 0)
     if (SMEM) bv = stage_bvh_smem(sc, smem + stack_bytes + DYN_RING_BYTES, &bar);
     else bv = global_bvh(sc);
-    if (WIDE && n_top > 0) stage_bytes_smem(smem + stack_bytes + DYN_RING_BYTES, sc.nodes4, (uint32_t)n_top * (uint32_t)sizeof(Bvh4Node), &bar);
     const HitSpan span = hit_span(ctrl, parity);
     const uint32_t n = span.n;                                              // total hit-queue length of this bounce
     uint32_t *fetch = ctrl + 10u + parity;
@@ -1039,7 +973,7 @@ __global__ void __launch_bounds__(256, 4) k_shadow_dyn(DevScene sc, ShadeOut so,
         if (act == 0u) { if (tail == head && pool.empty()) break; else continue; }
         const int thr_now = (tail == head && pool.empty()) ? 1 : thresh;
         do {
-            if (WIDE) { while (r.cur >= 0) dyn_node4_step<true>(nodes4, top, n_top, r, s_step, s_limit, spill); }
+            if (WIDE) { while (r.cur >= 0) dyn_node4_step<true>(nodes4, r, s_step, s_limit, spill); }
             else { while (r.cur >= 0) dyn_node_step<SMEM, true>(bv, r, s_step, s_limit); }
             __syncwarp();
             while (r.cur < 0 && r.cur != DYN_DONE) {
@@ -1401,16 +1335,7 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     // k_extend separate, 2: the default).
     lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? 2 : 0;
     if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if (v >= 0 && v <= 2 && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = (lc->big && v == 1) ? 2 : v; }
-    // BVH4 treelet in shared memory (bvh_dynfetch.cuh): the first n_top4 nodes (breadth-first order = the top levels).  B200PT_TOP_KB sizes it (0 = off).
-    lc->n_top4 = 0;
-    if (lc->wide) {
-        // The generic loads that serve treelet and L2 lanes in one instruction cost more than the L1 hits they replace, and the footprint costs occupancy -> OPT-IN.
-        int kb = 0;
-        if (const char *e = getenv("B200PT_TOP_KB")) { const int v = atoi(e); if (v >= 0 && v <= 160) kb = v; }
-        const uint32_t want = (uint32_t)kb * 1024u / (uint32_t)sizeof(Bvh4Node);
-        lc->n_top4 = (int)(want < sc.n_nodes4 ? want : sc.n_nodes4);
-    }
-    const size_t sh_dyn = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, lc->bvh_in_smem) + (size_t)lc->n_top4 * sizeof(Bvh4Node);
+    const size_t sh_dyn = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, lc->bvh_in_smem);
     int occ_e = 0, occ_c = 0, occ_s = 0, occ_sh = 0, occ_b = 0;
     if (lc->trav_dyn) {
         if (lc->wide) {
@@ -1443,8 +1368,8 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     lc->grid_bounce = sms * occ_b;
     lc->grid_light = sms * 8;
     if (getenv("B200PT_DEBUG"))
-        fprintf(stderr, "[b200pt] launch cfg: bvh depth %d (bvh4 %d) max_stack %d dyn_stack %d bvh_bytes %u smem %d dyn %d wide %d (treelet %d nodes) thresh %d fuse %d big %d | CTAs/SM extend %d connect %d shadow %d shade %d bounce %d\n",
-                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)lc->bvh_in_smem, (int)lc->trav_dyn, (int)lc->wide, lc->n_top4, lc->dyn_thresh, lc->fuse, (int)lc->big, occ_e, occ_c, occ_sh, occ_s, occ_b);
+        fprintf(stderr, "[b200pt] launch cfg: bvh depth %d (bvh4 %d) max_stack %d dyn_stack %d bvh_bytes %u smem %d dyn %d wide %d thresh %d fuse %d big %d | CTAs/SM extend %d connect %d shadow %d shade %d bounce %d\n",
+                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)lc->bvh_in_smem, (int)lc->trav_dyn, (int)lc->wide, lc->dyn_thresh, lc->fuse, (int)lc->big, occ_e, occ_c, occ_sh, occ_s, occ_b);
     return 0;
 }
 
@@ -1452,19 +1377,13 @@ void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch 
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st) {
     k_raygen<<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr);
 }
-void launch_ray_sort(const LaunchCfg &lc, const DevScene &sc, PathState ps, const uint32_t *ctrl, uint32_t parity, uint2 *key_rank, uint32_t *hist, uint32_t *offs,
-                     uint32_t *order, cudaStream_t st) {
-    k_ray_sort_keys<<<lc.grid_light, 256, 0, st>>>(sc, ps, ctrl, parity, key_rank, hist);
-    k_ray_sort_scan<<<1, 1024, 0, st>>>(hist, offs);
-    k_ray_sort_scatter<<<lc.grid_light, 256, 0, st>>>(ctrl, parity, key_rank, offs, order);
-}
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
-                   WaveCounters *ctr, bool primary, const uint32_t *order, cudaStream_t st) {
+                   WaveCounters *ctr, bool primary, cudaStream_t st) {
     set_attrs_for_current_device();
     const bool smem = lc.bvh_in_smem;
     if (lc.trav_dyn) {
-        const size_t sh = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem) + (size_t)lc.n_top4 * sizeof(Bvh4Node);
-#define B200PT_EXT_DYN(S, P, W) k_extend_dyn<S, P, W><<<lc.grid_extend, 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, lc.n_top4, order, ctr)
+        const size_t sh = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem);
+#define B200PT_EXT_DYN(S, P, W) k_extend_dyn<S, P, W><<<lc.grid_extend, 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr)
         if (lc.wide) { if (primary) B200PT_EXT_DYN(false, true, true); else B200PT_EXT_DYN(false, false, true); }
         else if (smem) { if (primary) B200PT_EXT_DYN(true, true, false); else B200PT_EXT_DYN(true, false, false); }
         else { if (primary) B200PT_EXT_DYN(false, true, false); else B200PT_EXT_DYN(false, false, false); }
@@ -1514,8 +1433,8 @@ void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cf
     const bool smem = lc.bvh_in_smem;
     const bool walks = cfg.EnableAtmosphere != 0u || sc.n_grids != 0u;      // k_connect<.., WALKS>
     if (lc.trav_dyn) {                                                      // shadow rays in their own dynamic-fetch kernel, then the join without tracing
-        const size_t shd = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem) + DYN_RING_BYTES_HOST + (size_t)lc.n_top4 * sizeof(Bvh4Node);
-#define B200PT_SH_DYN(S, W) k_shadow_dyn<S, W><<<lc.grid_shadow, 256, shd, st>>>(sc, so, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, lc.n_top4, ctr)
+        const size_t shd = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem) + DYN_RING_BYTES_HOST;
+#define B200PT_SH_DYN(S, W) k_shadow_dyn<S, W><<<lc.grid_shadow, 256, shd, st>>>(sc, so, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr)
         if (lc.wide) B200PT_SH_DYN(false, true); else if (smem) B200PT_SH_DYN(true, false); else B200PT_SH_DYN(false, false);
 #undef B200PT_SH_DYN
         if (walks) k_connect<false, false, true><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr);
