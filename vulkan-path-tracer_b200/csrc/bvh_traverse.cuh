@@ -90,16 +90,19 @@ __device__ __forceinline__ float slab_rcp(float d) { return 1.0f / (fabsf(d) < 1
 // the early-outs do skip work (k_extend 13.8 -> 12.7 ms).  Both forms evaluate u, v and t with the SAME operations and roundings: identical results.
 // 1 / det is the raw reciprocal approximation (MUFU.RCP, 1 ulp) in the default build -- the same precision class as the 2-ulp division it replaces
 // (Makefile: -prec-div=false), without the denormal / overflow rescaling around it; PRECISE=1 keeps the IEEE division.
+__device__ __forceinline__ float det_rcp(float det) {
+#ifdef B200PT_PRECISE
+    return 1.0f / det;
+#else
+    return __fdividef(1.0f, det);
+#endif
+}
 template <bool EARLY = false>
 __device__ __forceinline__ bool tri_test(float3 v0, float3 e1, float3 e2, float3 o, float3 d, float tmin, float tmax, float &t, float &u, float &v) {
     const float3 p = cross_fma(d, e2);
     const float det = dot_fma(e1, p);
     if (EARLY && det == 0.0f) return false;
-#ifdef B200PT_PRECISE
-    const float inv = 1.0f / det;
-#else
-    const float inv = __fdividef(1.0f, det);
-#endif
+    const float inv = det_rcp(det);
     const float3 tv = f3(__fsub_rn(o.x, v0.x), __fsub_rn(o.y, v0.y), __fsub_rn(o.z, v0.z));
     u = __fmul_rn(dot_fma(tv, p), inv);
     if (EARLY && !(u >= 0.0f && u <= 1.0f)) return false;
@@ -206,6 +209,45 @@ __device__ __forceinline__ bool bvh_trace(const BvhView &b, float3 o, float3 d, 
         if (s_top == s_base) break;
         s_top -= s_step;
         asm volatile("ld.shared.b32 %0, [%1];" : "=r"(cur) : "r"(s_top) : "memory");
+    }
+    if (!found) h.t = -1.0f;
+    return found;
+}
+
+// Flat closest-hit walk of rays that all start at ONE origin O (pinhole camera rays, k_camera).  The parts of tri_test that depend only on O
+// and the triangle -- tv = O - v0, q = tv x e1 and t's numerator e2 . q -- are computed once per CTA into a table; the per-ray rest and the
+// tie rule are tri_test<true> / bvh_trace's flat walk operation for operation (all explicitly rounded), so the hits are bit-identical.
+// Entry of slot s: [4s] e1 + gid, [4s+1] e2 + e2 . q, [4s+2] tv + q.x, [4s+3] q.y, q.z.
+constexpr uint32_t FLAT_FIXED_MAX = 64;                                     // B200PT_FLAT_MAX's upper limit
+__device__ __forceinline__ void flat_fixed_entry(const BvhView &b, uint32_t slot, float3 O, float4 *tab) {
+    const float4 *tp = b.tris + (size_t)slot * 3;
+    const float4 ta = tp[0], tb = tp[1], tc = tp[2];
+    const float3 tv = f3(__fsub_rn(O.x, ta.x), __fsub_rn(O.y, ta.y), __fsub_rn(O.z, ta.z));
+    const float3 q = cross_fma(tv, f3(tb));
+    tab[4 * slot] = make_float4(tb.x, tb.y, tb.z, ta.w);
+    tab[4 * slot + 1] = make_float4(tc.x, tc.y, tc.z, dot_fma(f3(tc), q));
+    tab[4 * slot + 2] = make_float4(tv.x, tv.y, tv.z, q.x);
+    tab[4 * slot + 3] = make_float4(q.y, q.z, 0.0f, 0.0f);
+}
+__device__ __forceinline__ bool flat_fixed_trace(const float4 *tab, uint32_t n, float3 d, float tmin, float tmax, HitRec &h) {
+    h.slot = 0xFFFFFFFFu; h.gid = 0xFFFFFFFFu; h.t = tmax; h.u = 0.0f; h.v = 0.0f;
+    uint32_t best_gid = 0xFFFFFFFFu;
+    bool found = false;
+    for (uint32_t s = 0; s < n; s++) {
+        const float4 a = tab[4 * s], b = tab[4 * s + 1], c = tab[4 * s + 2];
+        const float3 p = cross_fma(d, f3(b));
+        const float det = dot_fma(f3(a), p);
+        if (det == 0.0f) continue;
+        const float inv = det_rcp(det);
+        const float u = __fmul_rn(dot_fma(f3(c), p), inv);
+        if (!(u >= 0.0f && u <= 1.0f)) continue;
+        const float4 e = tab[4 * s + 3];
+        const float v = __fmul_rn(dot_fma(d, f3(c.w, e.x, e.y)), inv);
+        if (!(v >= 0.0f && __fadd_rn(u, v) <= 1.0f)) continue;
+        const float t = __fmul_rn(b.w, inv);
+        if (!(t > tmin && t < tmax)) continue;
+        const uint32_t gid = __float_as_uint(a.w);
+        if (!found || t < h.t || (t == h.t && gid < best_gid)) { found = true; h.t = t; h.u = u; h.v = v; h.slot = s; h.gid = gid; best_gid = gid; }
     }
     if (!found) h.t = -1.0f;
     return found;

@@ -556,6 +556,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     // Fused bounce kernels (LaunchCfg::fuse) need the BVH in shared memory and no volumes; they ping-pong the queues and the hit records
     // (the kernel that consumes bounce k's queue fills bounce k+1's), the unfused pipeline uses buffer 0 only.
     const int fuse = pre ? 0 : lc_.fuse;
+    const bool camera = lc_.camera && !pre;                   // k_camera: camera rays generated and traced in one kernel (bounce 0's k_extend is skipped)
     const uint32_t cmask = pre ? (class_mask_ | (1u << MC_GENERAL)) : class_mask_;   // volume / atmosphere events ride in the general queue
     const uint32_t qcap = (uint32_t)wave_cap_;
     const int qsel[2] = { 0, fuse == 2 ? 1 : 0 };
@@ -587,7 +588,10 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
         if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
         float4 *const hitb[2] = { B.so.hit, fuse == 2 ? B.so.bxdf_pdf : B.so.hit };
         for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
-            launch_raygen(lc_, dc, B.d_disp, nd, P, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st);
+            if (camera) {
+                const Queues q0{ B.q_miss[0], B.q_hit[0], qcap };
+                CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, P, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, hitb[0], B.counts, q0, d_ctr_, st));
+            } else launch_raygen(lc_, dc, B.d_disp, nd, P, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st);
             launches++; mark(0);
             int cur = 0; uint32_t k = 0;
             for (;;) {
@@ -598,7 +602,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     const uint32_t par = k & 1u;
                     const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
                     if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
-                    if (fuse != 2 || k == 0) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
+                    if ((fuse != 2 || k == 0) && !(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
                     launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
                                              fuse, cmask, st); mark(2);
                     if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);

@@ -21,11 +21,17 @@ struct LaunchCfg {
     int extend_threads; // CTA size of k_extend (256, big: 512)
     int fuse;           // 0: k_shade_hit + k_connect; 1: NEE queries + path epilogue inside k_shade_hit; 2: + the next segment's TraceRay (one kernel per bounce and class)
     int grid_bounce;    // persistent grid of the fused k_shade_hit instantiations (BVH + stacks in shared memory)
+    bool camera;        // camera rays generated and traced by k_camera (shared-memory BVH, one ray per thread) when the call has no pre-pass
+    int grid_camera;    // persistent grid of k_camera (extend_threads per CTA)
 };
 
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc);
 void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st);
+// launch_raygen + the camera rays' launch_extend in one kernel (LaunchCfg::camera, no pre-pass): clears the control block on `st`, writes the
+// path state, the hit records (hit_out) and the parity-0 queues.  Returns cudaError_t as int.
+int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st);
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st);
 // k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.

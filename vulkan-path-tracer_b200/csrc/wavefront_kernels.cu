@@ -4,6 +4,7 @@
 // closest-hit / miss inline (SH/RayGen.slang:9-160).  Here the same estimator is a wavefront:
 //
 //   k_raygen   camera sample + payload init                    SH/RayGen.slang:12-63
+//              (k_camera: the same + the camera rays' k_extend in one kernel, shared-memory scenes without a pre-pass)
 //   per bounce:
 //     k_extend   closest-hit traversal of the live paths       SH/RayGen.slang:68-72,90 (TraceRay)
 //                + sort into the miss queue and one hit queue per MATERIAL CLASS (lobe set)
@@ -13,8 +14,9 @@
 //     k_connect  shadow rays, payload.Emitted assembly,        SH/ClosestHit.slang:139,171-176,326-372
 //                luminance clamp, throughput, Russian          SH/RayGen.slang:92-113
 //                roulette, ballot/prefix-sum compaction
-//   scenes whose BVH is staged in shared memory by TMA run the bounce as ONE kernel per class (k_shade_hit<CLASS, ., 2>):
-//   shading + both NEE shadow queries + roulette + the next segment's closest-hit query + queue append.
+//   scenes whose BVH is staged in shared memory by TMA fuse the shadow queries and the roulette into k_shade_hit<CLASS, ., 1> (default), or
+//   run the bounce as ONE kernel per class (k_shade_hit<CLASS, ., 2>): shading + both NEE shadow queries + roulette + the next segment's
+//   closest-hit query + queue append.
 //   k_resolve  NaN/Inf rejection + running mean                SH/RayGen.slang:116-159
 //
 // Every path owns one sample slot, so radiance accumulation needs no atomics and is deterministic.
@@ -39,17 +41,23 @@ __host__ __device__ inline uint32_t part_global_row(uint32_t local_row, uint32_t
 
 // control block (device memory, u32): device_types.h (CTRL_Q)
 
+// camera position before the depth-of-field offset (SH/RayGen.slang:41): the origin of every camera ray when DepthOfFieldStrength == 0
+__device__ __forceinline__ float3 camera_eye(const DevConfig &cfg) {
+    const float *VI = cfg.VI;
+    return f3(VI[0] * 0.0f + VI[4] * 0.0f + VI[8] * 0.0f + VI[12] * 1.0f,
+              VI[1] * 0.0f + VI[5] * 0.0f + VI[9] * 0.0f + VI[13] * 1.0f,
+              VI[2] * 0.0f + VI[6] * 0.0f + VI[10] * 0.0f + VI[14] * 1.0f);
+}
+
 // ------------------------------------------------------------------------------------------------
-// k_raygen
+// camera_path : camera sample + payload init of path j of a wave (k_raygen, k_camera); returns the camera ray
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
-                                                 uint32_t first_sample, const uint32_t *__restrict__ rng_carry,
-                                                 PathState ps, float4 *__restrict__ sample_buf, uint32_t *__restrict__ ctrl,
-                                                 WaveCounters *ctr) {
-    const uint32_t n = n_disp * P;
+__device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispatch *__restrict__ disp, uint32_t P, uint32_t first_sample,
+                                            const uint32_t *__restrict__ rng_carry, const PathState &ps, float4 *__restrict__ sample_buf,
+                                            uint32_t j, float3 &ray_o, float3 &ray_d) {
     const uint32_t S = cfg.ScreenSplitCount;
     const uint32_t LW = (cfg.W + S - 1) / S;
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    {
         const uint32_t b = j / P, p = j - b * P;
         const DevDispatch dd = disp[b];
         uint32_t x, y;
@@ -70,9 +78,7 @@ __global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch
         const float pcx = (float)x + 0.5f + jx, pcy = (float)y + 0.5f + jy;
         const float dx = (pcx / (float)cfg.W) * 2.0f - 1.0f, dy = (pcy / (float)cfg.H) * 2.0f - 1.0f;
         const float *VI = cfg.VI, *PI = cfg.PI;
-        float3 origin = f3(VI[0] * 0.0f + VI[4] * 0.0f + VI[8] * 0.0f + VI[12] * 1.0f,
-                           VI[1] * 0.0f + VI[5] * 0.0f + VI[9] * 0.0f + VI[13] * 1.0f,
-                           VI[2] * 0.0f + VI[6] * 0.0f + VI[10] * 0.0f + VI[14] * 1.0f);
+        float3 origin = camera_eye(cfg);
         float3 target = f3(PI[0] * dx + PI[4] * dy + PI[8] * 1.0f + PI[12] * 1.0f,
                            PI[1] * dx + PI[5] * dy + PI[9] * 1.0f + PI[13] * 1.0f,
                            PI[2] * dx + PI[6] * dy + PI[10] * 1.0f + PI[14] * 1.0f);
@@ -89,6 +95,21 @@ __global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch
         ps.thr_depth[j] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(inside ? 0u : PT_MAX_DEPTH));
         ps.rad_slot[j] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(j));
         if (ps.vol_depth) ps.vol_depth[j] = 0u;                             // payload.VolumeDepth = 0 (SH/RayGen.slang:61)
+        ray_o = origin; ray_d = direction;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_raygen (pipelines without k_camera: volumes / atmosphere pre-pass, BVH outside shared memory, B200PT_CAMERA=0)
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
+                                                 uint32_t first_sample, const uint32_t *__restrict__ rng_carry,
+                                                 PathState ps, float4 *__restrict__ sample_buf, uint32_t *__restrict__ ctrl,
+                                                 WaveCounters *ctr) {
+    const uint32_t n = n_disp * P;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        float3 o, d;
+        camera_path(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, j, o, d);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { for (uint32_t w = 0; w < CTRL_WORDS; w++) ctrl[w] = 0; ctrl[0] = n; atomicAdd(&ctr->paths, (unsigned long long)n); }
 }
@@ -133,111 +154,64 @@ __device__ __forceinline__ void queue_append(uint32_t code, uint32_t entry, uint
 // k_extend : closest hit for every live path; sorts the live list into the miss queue and one hit queue per material class
 //            (material-sorted shading: every k_shade_hit<CLASS> warp runs one lobe set, converged)
 // ------------------------------------------------------------------------------------------------
-template <bool SMEM, bool PRIMARY>   // PRIMARY: camera rays (origin anywhere) -> exact slab arithmetic; later bounces start on scene surfaces -> FMA slabs
-__global__ void __launch_bounds__(512) k_extend(DevScene sc, PathState ps, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl, uint32_t parity,
-                                                 Queues q, int max_stack, WaveCounters *ctr) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t bar;
-    int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
-    const int stride = blockDim.x;
-    BvhView bv;
-    if (SMEM) bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
-    else bv = global_bvh(sc);
-    const uint32_t n = ctrl[parity];
-    if (blockIdx.x == 0 && threadIdx.x == 0) ctrl_reset_parity(ctrl, parity ^ 1u);   // counters of the NEXT bounce (last used two bounces ago)
-    uint32_t *qc = ctrl + CTRL_Q + 8u * parity;
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t lt = (1u << lane) - 1u;
-    // Queue append without block barriers and with few atomics (ncu round 1: returning per-warp atomics on hot addresses were
-    // 51 % of this kernel's stalls; the block-level scan that replaced them left 2.9 warps/issue parked on __syncthreads).
-    // A block owns SEGMENTS of K*256 consecutive paths (grid-stride over segments); in iteration `it` its 8 warps cover 256
-    // consecutive paths (neighbouring pixels -> shared BVH nodes in L1), each warp traces its K rays without ever waiting for the
-    // others.  Every lane keeps the queue codes of its K rays (3 bits each), lane `it` keeps the per-queue counts of iteration `it`
-    // (6 bits x 5 queues, one redux), then ONE atomic instruction per warp (lanes 0..4, one address each) reserves room in all five
-    // queues for all K iterations.  K adapts to the live count so small waves still fill the GPU.
-    const uint32_t K = min(8u, max(1u, n / (gridDim.x * blockDim.x * 2u)));
-    const uint32_t seg_paths = K * blockDim.x, n_seg = (n + seg_paths - 1u) / seg_paths;
-    // Scenes whose materials all fall into ONE class (and have no volumes) need no per-hit class lookup and only two queues: lane `it` keeps the
-    // hit / miss ballots of iteration `it`, one 64-bit atomic reserves room in both (the miss count and the class's hit count are not adjacent
-    // words, so two lanes issue one 32-bit atomic each in the same instruction).
-    const bool uniform = sc.uniform_class != 0xFFu && sc.pre_pass == 0u;
-    if (uniform) {
-        uint32_t *const q_hit_u = q.hit + (size_t)sc.uniform_class * q.cap;
-        for (uint32_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
-            const uint32_t base_i = seg * seg_paths + (threadIdx.x & ~31u);
-            uint32_t my_bh = 0, my_bm = 0, ch = 0, cm = 0;
-            uint32_t i = base_i + lane;
-            float4 o4 = make_float4(0, 0, 0, 0), d4 = o4;
-            if (i < n) { o4 = ps.org_pdf[i]; d4 = ps.dir_rng[i]; }
-            for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
-                if (base_i + it * blockDim.x >= n) break;                           // warp-uniform
-                const bool active = i < n;
-                bool hit = false;
-                float4 o4n = make_float4(0, 0, 0, 0), d4n = o4n;
-                if (it + 1u < K && i + blockDim.x < n) { o4n = ps.org_pdf[i + blockDim.x]; d4n = ps.dir_rng[i + blockDim.x]; }
-                if (active) {
-                    const float3 rd = normalize_ray(f3(d4));                    // SH/RayGen.slang:70
-                    HitRec h;
-                    hit = bvh_trace<SMEM, false, false, false, !PRIMARY>(bv, f3(o4), rd, 0.01f, 100000.0f, h, stack, stride, max_stack);   // :71-72
-                    hit_out[i] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
-                }
-                o4 = o4n; d4 = d4n;
-                const uint32_t bh = __ballot_sync(0xFFFFFFFFu, hit), bm = __ballot_sync(0xFFFFFFFFu, active && !hit);
-                if (lane == it) { my_bh = bh; my_bm = bm; }
-                ch += (uint32_t)__popc(bh); cm += (uint32_t)__popc(bm);
-            }
-            uint32_t base = 0u;
-            if (lane == 0u && cm) base = atomicAdd(qc, cm);
-            else if (lane == 1u && ch) base = atomicAdd(qc + 1u + sc.uniform_class, ch);
-            uint32_t om = __shfl_sync(0xFFFFFFFFu, base, 0), oh = __shfl_sync(0xFFFFFFFFu, base, 1);
-            i = base_i + lane;
-            for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
-                const uint32_t bh = __shfl_sync(0xFFFFFFFFu, my_bh, (int)it), bm = __shfl_sync(0xFFFFFFFFu, my_bm, (int)it);
-                if ((bh >> lane) & 1u) q_hit_u[oh + __popc(bh & lt)] = i;
-                else if ((bm >> lane) & 1u) q.miss[om + __popc(bm & lt)] = i;
-                oh += (uint32_t)__popc(bh); om += (uint32_t)__popc(bm);
-            }
+// Queue append without block barriers and with few atomics (ncu round 1: returning per-warp atomics on hot addresses were
+// 51 % of this kernel's stalls; the block-level scan that replaced them left 2.9 warps/issue parked on __syncthreads).
+// A block owns SEGMENTS of K*blockDim consecutive paths (grid-stride over segments); in iteration `it` its warps cover blockDim
+// consecutive paths (neighbouring pixels -> shared BVH nodes in L1), each warp traces its K rays without ever waiting for the
+// others.  A tally keeps the warp's queue codes of the K iterations, then ONE atomic instruction per warp reserves room in every
+// queue for all K iterations.  K adapts to the live count so small waves still fill the GPU.  (k_extend, k_camera)
+//
+// UniformTally: scenes whose materials all fall into ONE class (and have no volumes) need no per-hit class lookup and only two queues: lane
+// `it` keeps the hit / miss ballots of iteration `it`, one atomic instruction reserves room in both (the miss count and the class's hit count
+// are not adjacent words, so two lanes issue one 32-bit atomic each in the same instruction).
+// Neither tally keeps running totals across the traversals: lanes 0..K-1 hold every iteration's ballots / counts, and the flush sums them.
+struct UniformTally {
+    uint32_t my_bh = 0u, my_bm = 0u;
+    __device__ __forceinline__ void add(uint32_t it, uint32_t lane, bool active, bool hit) {
+        const uint32_t bh = __ballot_sync(0xFFFFFFFFu, hit), bm = __ballot_sync(0xFFFFFFFFu, active && !hit);
+        if (lane == it) { my_bh = bh; my_bm = bm; }
+    }
+    // the entry of iteration `it` is path i0 + lane + it * step
+    __device__ __forceinline__ void flush(uint32_t K, uint32_t i0, uint32_t step, uint32_t lane, uint32_t *qc, uint32_t cls, const Queues &q) const {
+        uint32_t *const q_hit_u = q.hit + (size_t)cls * q.cap;
+        const uint32_t lt = (1u << lane) - 1u;
+        const uint32_t ch = __reduce_add_sync(0xFFFFFFFFu, (uint32_t)__popc(my_bh)), cm = __reduce_add_sync(0xFFFFFFFFu, (uint32_t)__popc(my_bm));
+        uint32_t base = 0u;
+        if (lane == 0u && cm) base = atomicAdd(qc, cm);
+        else if (lane == 1u && ch) base = atomicAdd(qc + 1u + cls, ch);
+        uint32_t om = __shfl_sync(0xFFFFFFFFu, base, 0), oh = __shfl_sync(0xFFFFFFFFu, base, 1);
+        uint32_t i = i0 + lane;
+        for (uint32_t it = 0; it < K; it++, i += step) {
+            const uint32_t bh = __shfl_sync(0xFFFFFFFFu, my_bh, (int)it), bm = __shfl_sync(0xFFFFFFFFu, my_bm, (int)it);
+            if ((bh >> lane) & 1u) q_hit_u[oh + __popc(bh & lt)] = i;
+            else if ((bm >> lane) & 1u) q.miss[om + __popc(bm & lt)] = i;
+            oh += (uint32_t)__popc(bh); om += (uint32_t)__popc(bm);
         }
-    } else
-    for (uint32_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
-        const uint32_t base_i = seg * seg_paths + (threadIdx.x & ~31u);     // first path of this warp in iteration 0
-        uint32_t codes = 0u, my_cnts = 0u, totA = 0u, totB = 0u;            // totA: queues 0..2, totB: queues 3..4 (10-bit fields, <= 256 each)
-        uint32_t i = base_i + lane;
-        float4 o4 = make_float4(0, 0, 0, 0), d4 = o4;
-        if (i < n) { o4 = ps.org_pdf[i]; d4 = ps.dir_rng[i]; }
-        for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
-            if (base_i + it * blockDim.x >= n) { codes |= Q_NONE << (3u * it); continue; }   // warp-uniform
-            const bool active = i < n;
-            uint32_t code = Q_NONE;
-            float4 o4n = make_float4(0, 0, 0, 0), d4n = o4n;
-            if (it + 1u < K && i + blockDim.x < n) { o4n = ps.org_pdf[i + blockDim.x]; d4n = ps.dir_rng[i + blockDim.x]; }   // software pipelining of the state loads
-            const uint32_t pre = (active && sc.pre_pass) ? __float_as_uint(hit_out[i].w) : 0u;   // k_volume_decide's verdict on this segment
-            if (pre == VOLUME_EVENT) {
-                code = 1u + MC_GENERAL;                                     // scattered inside a volume / the atmosphere: no TraceRay, SH/RayGen.slang:86-90
-            } else if (pre == DEAD_EVENT) {
-                code = Q_NONE;                                              // finished in k_volume_decide (below the planet surface): nothing to queue
-            } else if (active) {
-                const float3 rd = normalize_ray(f3(d4));                    // SH/RayGen.slang:70
-                HitRec h;
-                const bool hit = bvh_trace<SMEM, false, false, false, !PRIMARY>(bv, f3(o4), rd, 0.01f, 100000.0f, h, stack, stride, max_stack);   // :71-72
-                hit_out[i] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
-                code = hit ? hit_code(sc, h.gid) : 0u;
-            }
-            o4 = o4n; d4 = d4n;
-            const uint32_t cn = __reduce_add_sync(0xFFFFFFFFu, code != Q_NONE ? 1u << (6u * code) : 0u);
-            codes |= code << (3u * it);
-            if (lane == it) my_cnts = cn;
-            totA += (cn & 63u) | (((cn >> 6) & 63u) << 10) | (((cn >> 12) & 63u) << 20);
-            totB += ((cn >> 18) & 63u) | (((cn >> 24) & 63u) << 10);
-        }
+    }
+};
+// ClassTally: every lane keeps the queue codes of its K rays (3 bits each), lane `it` keeps the per-queue counts of iteration `it` (6 bits x 5
+// queues, one redux), lanes 0..4 reserve room in one queue each.
+struct ClassTally {
+    uint32_t codes = 0u, my_cnts = 0u;
+    __device__ __forceinline__ void skip(uint32_t it) { codes |= Q_NONE << (3u * it); }
+    __device__ __forceinline__ void add(uint32_t it, uint32_t lane, uint32_t code) {
+        const uint32_t cn = __reduce_add_sync(0xFFFFFFFFu, code != Q_NONE ? 1u << (6u * code) : 0u);
+        codes |= code << (3u * it);
+        if (lane == it) my_cnts = cn;
+    }
+    __device__ __forceinline__ void flush(uint32_t K, uint32_t i0, uint32_t step, uint32_t lane, uint32_t *qc, const Queues &q) const {
+        const uint32_t lt = (1u << lane) - 1u;
+        const uint32_t cn = my_cnts;                                        // totA: queues 0..2, totB: queues 3..4 (10-bit fields, <= 256 each)
+        const uint32_t totA = __reduce_add_sync(0xFFFFFFFFu, (cn & 63u) | (((cn >> 6) & 63u) << 10) | (((cn >> 12) & 63u) << 20));
+        const uint32_t totB = __reduce_add_sync(0xFFFFFFFFu, ((cn >> 18) & 63u) | (((cn >> 24) & 63u) << 10));
         uint32_t base = 0u;
         {
             const uint32_t mytot = lane < 3u ? (totA >> (10u * lane)) & 1023u : (lane < 5u ? (totB >> (10u * (lane - 3u))) & 1023u : 0u);
             if (mytot) base = atomicAdd(qc + lane, mytot);
         }
         uint32_t runA = 0u, runB = 0u;
-        i = base_i + lane;
-        for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
+        uint32_t i = i0 + lane;
+        for (uint32_t it = 0; it < K; it++, i += step) {
             const uint32_t code = (codes >> (3u * it)) & 7u;
             const uint32_t cn = __shfl_sync(0xFFFFFFFFu, my_cnts, (int)it);
             const uint32_t peers = __match_any_sync(0xFFFFFFFFu, code);
@@ -251,7 +225,131 @@ __global__ void __launch_bounds__(512) k_extend(DevScene sc, PathState ps, float
             runB += ((cn >> 18) & 63u) | (((cn >> 24) & 63u) << 10);
         }
     }
+};
+
+// The shared-memory instantiations of k_extend are held to 80 registers, so that 3 CTAs of 256 threads share an SM: 24 warps hide the flat
+// loop's broadcast LDS -> dependent FMA chains, where 16 did not.  The bound is stated as a 768-thread maximum (65536 / 768 -> 80 registers)
+// because big mode launches the same instantiations with one 512-thread CTA per SM.
+constexpr int EXTEND_SMEM_MAX_THREADS = 768;
+// PRIMARY: camera rays (origin anywhere) -> exact slab arithmetic; later bounces start on scene surfaces -> FMA slabs.
+// UNIFORM: one material class and no pre-pass (sc.uniform_class, UniformTally); otherwise ClassTally and k_volume_decide's verdicts.
+template <bool SMEM, bool PRIMARY, bool UNIFORM>
+__global__ void __launch_bounds__(SMEM ? EXTEND_SMEM_MAX_THREADS : 512) k_extend(DevScene sc, PathState ps, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl,
+                                                                                  uint32_t parity, Queues q, int max_stack, WaveCounters *ctr) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ uint64_t bar;
+    int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
+    const int stride = blockDim.x;
+    BvhView bv;
+    if (SMEM) bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
+    else bv = global_bvh(sc);
+    const uint32_t n = ctrl[parity];
+    if (blockIdx.x == 0 && threadIdx.x == 0) ctrl_reset_parity(ctrl, parity ^ 1u);   // counters of the NEXT bounce (last used two bounces ago)
+    uint32_t *qc = ctrl + CTRL_Q + 8u * parity;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t K = min(8u, max(1u, n / (gridDim.x * blockDim.x * 2u)));
+    const uint32_t seg_paths = K * blockDim.x, n_seg = (n + seg_paths - 1u) / seg_paths;
+    for (uint32_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
+        const uint32_t base_i = seg * seg_paths + (threadIdx.x & ~31u);     // first path of this warp in iteration 0
+        UniformTally ut; ClassTally ct;
+        uint32_t i = base_i + lane;
+        float4 o4 = make_float4(0, 0, 0, 0), d4 = o4;
+        if (i < n) { o4 = ps.org_pdf[i]; d4 = ps.dir_rng[i]; }
+        for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
+            if (base_i + it * blockDim.x >= n) { if (!UNIFORM) ct.skip(it); continue; }   // warp-uniform
+            const bool active = i < n;
+            bool hit = false;
+            uint32_t code = Q_NONE;
+            float4 o4n = make_float4(0, 0, 0, 0), d4n = o4n;
+            if (it + 1u < K && i + blockDim.x < n) { o4n = ps.org_pdf[i + blockDim.x]; d4n = ps.dir_rng[i + blockDim.x]; }   // software pipelining of the state loads
+            const uint32_t pre = (!UNIFORM && active && sc.pre_pass) ? __float_as_uint(hit_out[i].w) : 0u;   // k_volume_decide's verdict on this segment
+            if (!UNIFORM && pre == VOLUME_EVENT) {
+                code = 1u + MC_GENERAL;                                     // scattered inside a volume / the atmosphere: no TraceRay, SH/RayGen.slang:86-90
+            } else if (!UNIFORM && pre == DEAD_EVENT) {
+                code = Q_NONE;                                              // finished in k_volume_decide (below the planet surface): nothing to queue
+            } else if (active) {
+                const float3 rd = normalize_ray(f3(d4));                    // SH/RayGen.slang:70
+                HitRec h;
+                hit = bvh_trace<SMEM, false, false, false, !PRIMARY>(bv, f3(o4), rd, 0.01f, 100000.0f, h, stack, stride, max_stack);   // :71-72
+                hit_out[i] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
+                if (!UNIFORM) code = hit ? hit_code(sc, h.gid) : 0u;
+            }
+            o4 = o4n; d4 = d4n;
+            if (UNIFORM) ut.add(it, lane, active, hit); else ct.add(it, lane, code);
+        }
+        if (UNIFORM) ut.flush(K, base_i, blockDim.x, lane, qc, sc.uniform_class, q); else ct.flush(K, base_i, blockDim.x, lane, qc, q);
+    }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&ctr->extend_rays, (unsigned long long)n);
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_camera : k_raygen and the camera rays' k_extend in one kernel, for scenes whose BVH is staged in shared memory and walked one ray per
+//            thread, without a pre-pass (no volumes, no atmosphere).  Each path's state is written for the shading kernels as k_raygen writes
+//            it, but the ray is traced from registers instead of being read back: the closest-hit query of k_extend<true, true, .>
+//            (normalize_ray, exact slabs, tmin 0.01, tmax 1e5).  The hit record goes to hit_out, the path to the queues of parity 0.
+//            The control block is cleared on the stream before the launch (launch_camera): the appends of other CTAs may run before
+//            block 0 does.
+// ------------------------------------------------------------------------------------------------
+// 64 registers: 4 CTAs of 256 threads per SM (big mode: 2 of 512).
+template <bool UNIFORM>
+__global__ void __launch_bounds__(512, 2) k_camera(DevScene sc, DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
+                                                   uint32_t first_sample, const uint32_t *__restrict__ rng_carry, PathState ps,
+                                                   float4 *__restrict__ sample_buf, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl,
+                                                   Queues q, int max_stack, WaveCounters *ctr) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ uint64_t bar;
+    int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
+    const int stride = blockDim.x;
+    const BvhView bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
+    // Flat scenes: the origin-only part of every triangle test, for rays from the camera position (flat_fixed_trace).  A warp uses the table
+    // only when all its rays start bit for bit there (always without depth of field); otherwise it walks the scene like k_extend.
+    __shared__ float4 fixed_tab[4 * FLAT_FIXED_MAX];
+    __shared__ float4 fixed_eye;
+    const bool fixed = bv.n_flat != 0u && bv.n_flat <= FLAT_FIXED_MAX;
+    if (fixed) {
+        const float3 eye = camera_eye(cfg);
+        for (uint32_t s = threadIdx.x; s < bv.n_flat; s += blockDim.x) flat_fixed_entry(bv, s, eye, fixed_tab);
+        if (threadIdx.x == 0) fixed_eye = make_float4(eye.x, eye.y, eye.z, 0.0f);
+        __syncthreads();
+    }
+    const uint32_t n = n_disp * P;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {                              // nothing in this launch reads ctrl[0]: the first k_shade_* kernels do
+        ctrl[0] = n;
+        atomicAdd(&ctr->paths, (unsigned long long)n); atomicAdd(&ctr->extend_rays, (unsigned long long)n);
+    }
+    uint32_t *qc = ctrl + CTRL_Q;                                           // queues of parity 0
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t K = min(8u, max(1u, n / (gridDim.x * blockDim.x * 2u)));
+    // the segments of k_extend, walked by the warp's first path (one loop register fewer: 64 registers without spilling)
+    const uint32_t seg_paths = K * blockDim.x;
+    for (uint32_t base_i = blockIdx.x * seg_paths + (threadIdx.x & ~31u); base_i < n; base_i += gridDim.x * seg_paths) {
+        UniformTally ut; ClassTally ct;
+        uint32_t i = base_i + lane;
+        for (uint32_t it = 0; it < K; it++, i += blockDim.x) {
+            if (base_i + it * blockDim.x >= n) { if (!UNIFORM) ct.skip(it); continue; }   // warp-uniform
+            const bool active = i < n;
+            bool hit = false;
+            uint32_t code = Q_NONE;
+            float3 o = f3(0.0f), d = o;
+            if (active) camera_path(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, i, o, d);
+            bool at_eye = false;
+            if (fixed) {
+                const float4 e = fixed_eye;
+                at_eye = __all_sync(0xFFFFFFFFu, !active || (__float_as_uint(o.x) == __float_as_uint(e.x) && __float_as_uint(o.y) == __float_as_uint(e.y) &&
+                                                              __float_as_uint(o.z) == __float_as_uint(e.z)));
+            }
+            if (active) {                                                   // overhang pixels of a chunked dispatch are born dead and still traced, as in k_extend
+                const float3 rd = normalize_ray(d);                         // SH/RayGen.slang:70-72
+                HitRec h;
+                hit = at_eye ? flat_fixed_trace(fixed_tab, bv.n_flat, rd, 0.01f, 100000.0f, h)
+                             : bvh_trace<true, false, false, false, false>(bv, o, rd, 0.01f, 100000.0f, h, stack, stride, max_stack);
+                hit_out[i] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
+                if (!UNIFORM) code = hit ? hit_code(sc, h.gid) : 0u;
+            }
+            if (UNIFORM) ut.add(it, lane, active, hit); else ct.add(it, lane, code);
+        }
+        if (UNIFORM) ut.flush(K, base_i, blockDim.x, lane, qc, sc.uniform_class, q); else ct.flush(K, base_i, blockDim.x, lane, qc, q);
+    }
 }
 
 // SH/RayGen.slang:116-128: an unsplit path adds all of pathLight, a path split by an atmosphere event only its colour channel
@@ -1271,8 +1369,11 @@ static int set_attrs_for_current_device() {
         if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)a.sharedSizeBytes);
         if (e != cudaSuccess && rc == 0) rc = (int)e;
     };
-    optin((const void *)k_extend<true, true>); optin((const void *)k_extend<true, false>);
-    optin((const void *)k_extend<false, true>); optin((const void *)k_extend<false, false>);
+#define B200PT_OPTIN_EXTEND(U) optin((const void *)k_extend<true, true, U>); optin((const void *)k_extend<true, false, U>); \
+                               optin((const void *)k_extend<false, true, U>); optin((const void *)k_extend<false, false, U>);
+    B200PT_OPTIN_EXTEND(true) B200PT_OPTIN_EXTEND(false)
+#undef B200PT_OPTIN_EXTEND
+    optin((const void *)k_camera<true>); optin((const void *)k_camera<false>);
     optin((const void *)k_connect<true, true>); optin((const void *)k_connect<false, true>); optin((const void *)k_connect<false, false>);
     optin((const void *)k_connect<true, true, true>); optin((const void *)k_connect<false, true, true>); optin((const void *)k_connect<false, false, true>);
     optin((const void *)k_extend_dyn<true, true, false>); optin((const void *)k_extend_dyn<true, false, false>);
@@ -1328,13 +1429,20 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
         lc->dyn_stack = need < cap ? need : cap;
         if (need - lc->dyn_stack > DYN_SPILL) lc->wide = false, lc->dyn_stack = lc->max_stack;   // deeper than shared column + overflow array: BVH2
     }
-    // fused bounce kernel (k_shade_hit<., ., 2>): the default for scenes whose BVH is staged in shared memory and walked one ray per thread.  It keeps
-    // the NEE requests, the payload and the next segment's origin on chip (~170 B of HBM traffic per shaded hit instead of ~450 B) and traces a warp's
-    // shadow and extension rays together from a shared-memory list, so no traversal runs in a half-empty warp.  Cornell box, H100 SXM at 700 W: see
-    // DESIGN.md section 8.  B200PT_FUSE=0|1|2 overrides (0: k_extend + k_shade_hit + k_connect, 1: NEE queries and the path epilogue fused,
-    // k_extend separate, 2: the default).
-    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? 2 : 0;
+    // Bounce pipeline of scenes whose BVH is staged in shared memory and walked one ray per thread (the default elsewhere is 0):
+    //   1 (default): k_shade_hit<., ., 1> traces each NEE query the moment it is built and finishes the path (roulette, radiance, compaction) in
+    //      the same thread; the next segment's closest hit runs in k_extend<true, false, .> at 24 warps per SM.
+    //   2 (big mode's only fused form): k_shade_hit<., ., 2> also traces the next segment, from a per-warp ray list in shared memory.
+    // On the Cornell box 1 is faster: the bounce kernel runs at 16 warps per SM with 118-128 registers, and handing it the closest-hit query
+    // costs more than the separate k_extend does.  Measured with k_camera and the 24-warp k_extend on an H100 at 400 W (DESIGN.md section 8,
+    // which chose this default); before them, on a 700 W card, FUSE=1 already led by 8.5 % (section 9).  B200PT_FUSE=0|1|2 overrides (0: k_extend + k_shade_hit
+    // + k_connect).
+    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? (lc->big ? 2 : 1) : 0;
     if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if (v >= 0 && v <= 2 && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = (lc->big && v == 1) ? 2 : v; }
+    // Camera rays of those scenes: generated and traced in one kernel (k_camera) instead of k_raygen + k_extend<true, true, .>, unless the scene
+    // needs a pre-pass (decided per call: Engine::path_trace).  B200PT_CAMERA=0 keeps the pair.
+    lc->camera = lc->bvh_in_smem && !lc->trav_dyn;
+    if (const char *e = getenv("B200PT_CAMERA")) { if (atoi(e) == 0) lc->camera = false; }
     const size_t sh_dyn = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, lc->bvh_in_smem);
     int occ_e = 0, occ_c = 0, occ_s = 0, occ_sh = 0, occ_b = 0;
     if (lc->trav_dyn) {
@@ -1350,10 +1458,13 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
         }
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<false, false>, 256, 0);
     } else if (lc->bvh_in_smem) {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<true, false>, lc->extend_threads, sh);
+        int occ_u = 0;                                                      // one grid for both tally forms: the smaller residency
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<true, false, false>, lc->extend_threads, sh);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_extend<true, false, true>, lc->extend_threads, sh);
+        if (occ_u < occ_e) occ_e = occ_u;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<true, true>, lc->extend_threads, sh);
     } else {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<false, false>, 256, sh);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<false, false, false>, 256, sh);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<false, true>, 256, sh);
     }
     if (occ_sh < 1) occ_sh = 1;
@@ -1366,16 +1477,35 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     { int occ_t = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, lc->bvh_in_smem ? k_trace_rays<true> : k_trace_rays<false>, 256, sh256); lc->grid_trace = sms * (occ_t < 1 ? 1 : occ_t); }
     lc->grid_shade = sms * occ_s;
     lc->grid_bounce = sms * occ_b;
+    int occ_cam = 0;
+    if (lc->camera) {
+        int occ_u = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_cam, k_camera<false>, lc->extend_threads, sh);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_camera<true>, lc->extend_threads, sh);
+        if (occ_u < occ_cam) occ_cam = occ_u;
+    }
+    lc->grid_camera = sms * (occ_cam < 1 ? 1 : occ_cam);
     lc->grid_light = sms * 8;
     if (getenv("B200PT_DEBUG"))
-        fprintf(stderr, "[b200pt] launch cfg: bvh depth %d (bvh4 %d) max_stack %d dyn_stack %d bvh_bytes %u smem %d dyn %d wide %d thresh %d fuse %d big %d | CTAs/SM extend %d connect %d shadow %d shade %d bounce %d\n",
-                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)lc->bvh_in_smem, (int)lc->trav_dyn, (int)lc->wide, lc->dyn_thresh, lc->fuse, (int)lc->big, occ_e, occ_c, occ_sh, occ_s, occ_b);
+        fprintf(stderr, "[b200pt] launch cfg: bvh depth %d (bvh4 %d) max_stack %d dyn_stack %d bvh_bytes %u smem %d dyn %d wide %d thresh %d fuse %d big %d camera %d | CTAs/SM extend %d connect %d shadow %d shade %d bounce %d camera %d\n",
+                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)lc->bvh_in_smem, (int)lc->trav_dyn, (int)lc->wide, lc->dyn_thresh, lc->fuse, (int)lc->big, (int)lc->camera,
+                occ_e, occ_c, occ_sh, occ_s, occ_b, occ_cam);
     return 0;
 }
 
 void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st) {
     k_raygen<<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr);
+}
+int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st) {
+    set_attrs_for_current_device();
+    const cudaError_t e = cudaMemsetAsync(ctrl, 0, CTRL_WORDS * sizeof(uint32_t), st);   // before any CTA appends to the parity-0 queues
+    if (e != cudaSuccess) return (int)e;
+    const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, true);
+    if (sc.uniform_class != 0xFFu) k_camera<true><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr);
+    else k_camera<false><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr);
+    return 0;
 }
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st) {
@@ -1391,13 +1521,13 @@ void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4
         return;
     }
     const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, smem);
-    if (smem) {
-        if (primary) k_extend<true, true><<<lc.grid_extend, lc.extend_threads, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr);
-        else k_extend<true, false><<<lc.grid_extend, lc.extend_threads, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr);
-    } else {
-        if (primary) k_extend<false, true><<<lc.grid_extend, 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr);
-        else k_extend<false, false><<<lc.grid_extend, 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr);
-    }
+    const bool uniform = sc.uniform_class != 0xFFu && sc.pre_pass == 0u;
+#define B200PT_EXT(S, P, U) k_extend<S, P, U><<<lc.grid_extend, S ? lc.extend_threads : 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr)
+#define B200PT_EXT_U(S, P) do { if (uniform) B200PT_EXT(S, P, true); else B200PT_EXT(S, P, false); } while (0)
+    if (smem) { if (primary) B200PT_EXT_U(true, true); else B200PT_EXT_U(true, false); }
+    else { if (primary) B200PT_EXT_U(false, true); else B200PT_EXT_U(false, false); }
+#undef B200PT_EXT_U
+#undef B200PT_EXT
 }
 // k_shade_miss + one k_shade_hit<CLASS> per material class present in the scene (+ k_shade_volume).  fuse (0 / 1 / 2): see k_shade_hit.
 // Returns the number of kernels launched.
