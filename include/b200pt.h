@@ -217,6 +217,22 @@ uint32_t b200pt_partition_local_row_count(uint32_t height, uint32_t rank, uint32
  * *done_out (optional) = 1 when all samples are accumulated (PathTrace's return value). */
 int32_t b200pt_path_trace(b200pt_handle h, uint32_t dispatches, uint32_t base_seed, int32_t *done_out);
 int32_t b200pt_samples_accumulated(b200pt_handle h, uint32_t *out);         /* GetSamplesAccumulated */
+
+/* ---- adaptive sampling (no reference equivalent) ----
+ * With Enable != 0 every local pixel keeps its frame count n_p and a Welford running mean / second moment of its per-frame luminance
+ * (acc / SamplesPerFrame, weights 0.212671 0.715160 0.072169).  Whenever the frame counter reaches a multiple of Interval, a pixel with
+ * n_p >= MinSamples stops for good once sqrt(M2 / (n_p - 1) / n_p) <= Threshold * max(mean, 1e-3) (Threshold 0 stops nothing).  Pixels
+ * are traced from frame 0 until they stop, so a stopped pixel holds bit for bit what the plain renderer holds after n_p frames.
+ * path_trace then also returns done once no local pixel is active, and launches nothing.  MaxSamplesAccumulated stays the cap.
+ * Not combinable with ScreenChunkCount > 1.  Any set resets the accumulation; so do reset / set_config / resize / set_partition. */
+typedef struct { uint32_t Enable; float Threshold; uint32_t MinSamples; uint32_t Interval; } b200pt_adaptive;   /* defaults {0, 0.01, 64, 32} */
+int32_t b200pt_default_adaptive(b200pt_adaptive *out);
+int32_t b200pt_set_adaptive(b200pt_handle h, const b200pt_adaptive *a);   /* WRONG_ARGUMENTS: Threshold < 0 or not finite, MinSamples < 2, Interval 0, chunks > 1 */
+int32_t b200pt_get_adaptive(b200pt_handle h, b200pt_adaptive *out);
+/* local rows: counts[i] = frames accumulated into pixel i (the frame count everywhere without adaptive sampling), rel_error[i] = its
+ * sqrt(M2 / (n_p - 1) / n_p) / max(mean, 1e-3) (NaN without adaptive sampling or with n_p < 2).  Either pointer may be NULL. */
+int32_t b200pt_get_pixel_stats(b200pt_handle h, uint32_t *counts, float *rel_error);
+int32_t b200pt_active_pixels(b200pt_handle h, uint32_t *out);             /* local pixels still traced (all of them without adaptive sampling) */
 int32_t b200pt_synchronize(b200pt_handle h);
 /* b200pt_path_trace is ASYNCHRONOUS: it returns once the waves are enqueued (two waves are in flight on the handle's internal streams so that the
  * latency-bound tail of one overlaps the head of the next, also across calls).  Every later call on the handle that touches the image (get_hdr,
@@ -239,7 +255,8 @@ int32_t b200pt_set_hdr(b200pt_handle h, const float *src, int32_t src_is_device)
 /* Checkpoint / resume of the progressive accumulation (the reference keeps it only in the GPU image and loses it on exit, PathTracer.h:183,
  * 199-201; SURVEY 5 / 8f row 4).  The file holds the RGBA32F accumulation of THIS handle's rows + the dispatch counters; after
  * b200pt_load_checkpoint into a handle with the same scene / config / size / partition, path_trace(frames, same base_seed) continues the
- * identical sample sequence: the final image equals an uninterrupted run bit for bit. */
+ * identical sample sequence: the final image equals an uninterrupted run bit for bit.  With adaptive sampling on, the file (version 2) also
+ * holds the adaptive block and the per-pixel state; it loads only into a handle with the same adaptive block, and a version-1 file does not. */
 int32_t b200pt_save_checkpoint(b200pt_handle h, const char *path);
 int32_t b200pt_load_checkpoint(b200pt_handle h, const char *path);
 int32_t b200pt_get_counters(b200pt_handle h, b200pt_counters *out);

@@ -29,6 +29,13 @@ def _het():
     return dict(Position=(0.2, -0.2, -5.5), Scale=(3.0, 3.0, 3.0), Density=4.0, Grid=orc.prepare_density_grid(d, index_min=(-18, -17, -10), temperature=d * 100.0))
 run("cornell_box", 40, 30, 1, 5, Volumes=[FOG, _het()])                                              # grid volume: delta tracking, ratio-tracked NEE transmittance in k_connect<.., true>
 run("cornell_box", 40, 30, 1, 5, EnableAtmosphere=1, SkyRotationAltitude=-20.0, Volumes=[_het()])    # ... under the atmosphere
+def _adaptive(name, **kw):                                          # adaptive sampling: k_camera<., true> / k_raygen<true>, k_resolve_adaptive, k_adaptive_update + _compact
+    T = util.product_tracer(name, 40, 30, MaxDepth=5, **kw)
+    T.set_adaptive(Enable=1, Threshold=0.3, MinSamples=4, Interval=4)
+    T.path_trace(12, util.BASE_SEED)
+    assert np.isfinite(T.get_hdr()).all() and 0 <= T.active_pixels() <= 40 * 30
+    print(name, "adaptive", T.active_pixels(), "ok")
+_adaptive("cornell_box"); _adaptive("cornell_box", Volumes=[FOG])
 run("cornell_box_glass", 48, 48, 2, 8)                              # dynamic-fetch BVH2 kernels, class queues (glass / diffuse)
 os.environ["B200PT_WIDE"] = "1"; run("viking_room", 48, 48, 1, 4); del os.environ["B200PT_WIDE"]              # BVH4 + textures
 print("sanitize_small done")

@@ -113,6 +113,16 @@ class Bloom(C.Structure):
     _fields_ = [("BloomThreshold", C.c_float), ("BloomStrength", C.c_float), ("MipCount", C.c_uint32), ("FalloffRange", C.c_float)]
 
 
+class Adaptive(C.Structure):    # b200pt_adaptive: per-pixel adaptive sampling (no reference equivalent)
+    _fields_ = [("Enable", C.c_uint32), ("Threshold", C.c_float), ("MinSamples", C.c_uint32), ("Interval", C.c_uint32)]
+
+
+def default_adaptive(**kw):
+    a = Adaptive(); lib().b200pt_default_adaptive(C.byref(a))
+    for k, v in kw.items(): setattr(a, k, v)
+    return a
+
+
 class Counters(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("paths", "extend_rays", "shade_invocations", "surface_hits", "misses", "shadow_rays", "medium_events", "kernel_launches")] + \
                [(n, C.c_float) for n in ("ms_total", "ms_raygen", "ms_extend", "ms_shade", "ms_connect", "ms_resolve")] + \
@@ -179,6 +189,9 @@ def lib():
             "b200pt_bvh2_reinsert": [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_int32, C.c_float, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.c_void_p],
             "b200pt_bvh2_sah_rebuild": [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.c_void_p],
             "b200pt_load_gltf": [C.c_char_p, C.POINTER(C.POINTER(SceneDesc))], "b200pt_free_scene": [C.POINTER(SceneDesc)],
+            "b200pt_default_adaptive": [C.POINTER(Adaptive)], "b200pt_set_adaptive": [C.c_void_p, C.POINTER(Adaptive)],
+            "b200pt_get_adaptive": [C.c_void_p, C.POINTER(Adaptive)], "b200pt_get_pixel_stats": [C.c_void_p, C.c_void_p, C.c_void_p],
+            "b200pt_active_pixels": [C.c_void_p, C.POINTER(C.c_uint32)],
         }
         for name, args in sig.items():
             fn = getattr(L, name); fn.restype = C.c_int32; fn.argtypes = args
@@ -474,6 +487,24 @@ class PathTracer:
     # ---- hot path
     def path_trace(self, dispatches, base_seed):
         done = C.c_int32(); self._ck(self.L.b200pt_path_trace(self.h, dispatches, base_seed & 0xFFFFFFFF, C.byref(done))); return bool(done.value)
+
+    # ---- adaptive sampling
+    def set_adaptive(self, adaptive=None, **kw):
+        """b200pt_adaptive fields (Enable, Threshold, MinSamples, Interval); unnamed fields take the defaults"""
+        a = adaptive if adaptive is not None else default_adaptive(**kw)
+        self._ck(self.L.b200pt_set_adaptive(self.h, C.byref(a)))
+
+    def get_adaptive(self):
+        a = Adaptive(); self._ck(self.L.b200pt_get_adaptive(self.h, C.byref(a))); return a
+
+    def pixel_stats(self):
+        """(frames accumulated per local pixel [rows, W] uint32, relative standard error of the mean luminance [rows, W] float32)"""
+        w, _ = self.size(); rows = self.local_rows()
+        counts = np.empty((rows, w), np.uint32); rel = np.empty((rows, w), np.float32)
+        self._ck(self.L.b200pt_get_pixel_stats(self.h, _p(counts), _p(rel))); return counts, rel
+
+    def active_pixels(self):
+        n = C.c_uint32(); self._ck(self.L.b200pt_active_pixels(self.h, C.byref(n))); return n.value
 
     def samples_accumulated(self):
         n = C.c_uint32(); self._ck(self.L.b200pt_samples_accumulated(self.h, C.byref(n))); return n.value

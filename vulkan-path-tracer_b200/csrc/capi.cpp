@@ -23,6 +23,7 @@ template <class F> static int32_t guard(b200pt_handle h, F &&f) {
 }
 
 static_assert(sizeof(b200pt_volume) == 148 && sizeof(b200pt_density_grid) == 80, "b200pt_volume / b200pt_density_grid layout (binding.py, INTEGRATION.md)");
+static_assert(sizeof(b200pt_adaptive) == 16, "b200pt_adaptive layout (binding.py, checkpoint version 2)");
 
 extern "C" {
 
@@ -181,6 +182,15 @@ uint32_t b200pt_partition_local_row_count(uint32_t H, uint32_t r, uint32_t w, ui
 int32_t b200pt_path_trace(b200pt_handle h, uint32_t dispatches, uint32_t seed, int32_t *done) {
     return guard(h, [&](Engine &e) { bool d = e.path_trace(dispatches, seed); if (done) *done = d ? 1 : 0; });
 }
+int32_t b200pt_default_adaptive(b200pt_adaptive *a) {
+    if (!a) return B200PT_ERR_WRONG_ARGUMENTS;
+    a->Enable = 0; a->Threshold = 0.01f; a->MinSamples = 64; a->Interval = 32;
+    return B200PT_OK;
+}
+int32_t b200pt_set_adaptive(b200pt_handle h, const b200pt_adaptive *a) { if (!a) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_adaptive(*a); }); }
+int32_t b200pt_get_adaptive(b200pt_handle h, b200pt_adaptive *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.adaptive(); }); }
+int32_t b200pt_get_pixel_stats(b200pt_handle h, uint32_t *counts, float *rel_error) { return guard(h, [&](Engine &e) { e.pixel_stats(counts, rel_error); }); }
+int32_t b200pt_active_pixels(b200pt_handle h, uint32_t *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.active_pixels(); }); }
 int32_t b200pt_flush(b200pt_handle h) { return guard(h, [&](Engine &e) { e.flush(); }); }
 int32_t b200pt_samples_accumulated(b200pt_handle h, uint32_t *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.samples_accumulated(); }); }
 int32_t b200pt_synchronize(b200pt_handle h) { return guard(h, [&](Engine &e) { e.synchronize(); }); }

@@ -22,6 +22,25 @@ static int fail(b200pt_handle h, const char *what, int32_t code) {
 }
 #define CALL(x) do { int32_t r_ = (x); if (r_ != B200PT_OK) return fail(h, #x, r_); } while (0)
 
+// --adaptive THRESHOLD[,MIN[,INTERVAL]]: a finite threshold >= 0, MIN >= 2, INTERVAL >= 1 (b200pt_set_adaptive's rules)
+static bool parse_adaptive(const char *s, b200pt_adaptive &a) {
+    b200pt_default_adaptive(&a);
+    a.Enable = 1;
+    char *end = nullptr;
+    const double t = strtod(s, &end);
+    if (end == s || !(t >= 0.0 && t < 1e30)) return false;
+    a.Threshold = (float)t;
+    for (uint32_t *field : { &a.MinSamples, &a.Interval }) {
+        if (*end == 0) break;
+        if (*end != ',') return false;
+        const char *p = end + 1;
+        const long v = strtol(p, &end, 10);
+        if (end == p || v < 1 || v > 0x7FFFFFFFL) return false;
+        *field = (uint32_t)v;
+    }
+    return *end == 0 && a.MinSamples >= 2;
+}
+
 static void usage() {
     fprintf(stderr,
         "usage: b200pt_render --scene s.gltf --env e.hdr --luts DIR --out image.png [options]\n"
@@ -34,6 +53,8 @@ static void usage() {
         "  --phase 0|1|2     phase function: Henyey-Greenstein, Draine, HG + Draine\n"
         "  --sky AZ ALT      sky / sun rotation in degrees (SetSkyAzimuth / SetSkyAltitude, Editor.cpp sky panel)\n"
         "  --atmosphere      render with the atmosphere (SetEnableAtmosphere(true): sun-disk NEE, Rayleigh / Mie / ozone scattering); --sun-color r g b\n"
+        "  --adaptive T[,MIN[,INTERVAL]]  adaptive sampling: stop a pixel once the relative standard error of its mean luminance is <= T\n"
+        "                    (checked every INTERVAL frames once it has MIN; defaults 64, 32); --spp stays the cap\n"
         "  --checkpoint FILE save the accumulation when done         --resume FILE  continue from a checkpoint\n"
         "  --preview-every K rewrite the output PNG after every K PathTrace calls (the editor's progressive view, Editor.cpp:83-121)\n"
         "  --bake-luts N     bake missing lookup tables into DIR with N samples per texel first (Application.cpp:35-72)\n"
@@ -46,6 +67,7 @@ int main(int argc, char **argv) {
     int device = 0; bool quiet = false, atmosphere = false, sky = false; float sky_az = 0.0f, sky_al = 0.0f, sun[3] = { 1.0f, 1.0f, 1.0f };
     b200pt_tonemap tm{ 1.0f, 2.2f }; b200pt_bloom bl{ 2.0f, 1.0f, 10, 5.0f };
     std::vector<b200pt_volume> vols;
+    b200pt_adaptive adaptive; b200pt_default_adaptive(&adaptive);
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
         auto need = [&](int n) { if (i + n >= argc) { usage(); exit(2); } };
@@ -71,6 +93,7 @@ int main(int argc, char **argv) {
         else if (a == "--atmosphere") atmosphere = true;
         else if (a == "--sun-color") { need(3); for (int k = 0; k < 3; k++) sun[k] = (float)atof(argv[++i]); }
         else if (a == "--preview-every") { need(1); preview = (uint32_t)atoi(argv[++i]); }
+        else if (a == "--adaptive") { need(1); if (!parse_adaptive(argv[++i], adaptive)) { usage(); return 2; } }
         else if (a == "--checkpoint") { need(1); ckpt_out = argv[++i]; } else if (a == "--resume") { need(1); ckpt_in = argv[++i]; }
         else if (a == "--bake-luts") { need(1); bake = (uint32_t)atoi(argv[++i]); } else if (a == "--device") { need(1); device = atoi(argv[++i]); }
         else if (a == "--quiet") quiet = true;
@@ -90,6 +113,7 @@ int main(int argc, char **argv) {
     cfg.MaxDepth = depth; cfg.ScreenChunkCount = chunks; cfg.MaxSamplesAccumulated = spp;
     if (sky) { cfg.SkyRotationAzimuth = sky_az; cfg.SkyRotationAltitude = sky_al; }
     CALL(b200pt_set_config(h, &cfg));
+    if (adaptive.Enable) CALL(b200pt_set_adaptive(h, &adaptive));
     if (atmosphere) {
         b200pt_atmosphere atm; CALL(b200pt_get_atmosphere(h, &atm));
         atm.Enable = 1; for (int k = 0; k < 3; k++) atm.SunColor[k] = sun[k];
@@ -124,9 +148,10 @@ int main(int argc, char **argv) {
     CALL(b200pt_post_process(h));
     CALL(b200pt_save_png(h, out.c_str()));
     b200pt_counters c; CALL(b200pt_get_counters(h, &c));
+    uint32_t active = 0; CALL(b200pt_active_pixels(h, &active));
     const double s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    printf("{\"image\": \"%s\", \"size\": [%u, %u], \"spp\": %u, \"seconds\": %.3f, \"paths\": %llu, \"kernel_launches\": %llu}\n",
-           out.c_str(), W, H, acc, s, (unsigned long long)c.paths, (unsigned long long)c.kernel_launches);
+    printf("{\"image\": \"%s\", \"size\": [%u, %u], \"spp\": %u, \"seconds\": %.3f, \"paths\": %llu, \"kernel_launches\": %llu, \"active_pixels\": %u}\n",
+           out.c_str(), W, H, acc, s, (unsigned long long)c.paths, (unsigned long long)c.kernel_launches, active);
     b200pt_destroy(h);
     return 0;
 }

@@ -2,6 +2,7 @@
 // Orchestration per b200pt_path_trace call (all on one CUDA stream, no host sync inside a wave unless the
 // scene can scatter inside a medium or MaxDepth is large enough that early exit pays):
 //   upload dispatch table -> for each wave of F dispatches: raygen -> [extend, shade, connect] x bounces -> resolve
+// (adaptive sampling: the waves of each interval trace the active pixels only; k_adaptive_update + one 4-byte read-back at its end)
 #include "engine.h"
 #include <cstring>
 #include <cstdio>
@@ -38,6 +39,8 @@ Engine::Engine(int device) : device_(device) {
         CK(cudaMalloc(&wb_[c].d_disp, kMaxDispatchTable * sizeof(DevDispatch))); CK(cudaMallocHost(&wb_[c].h_disp, kMaxDispatchTable * sizeof(DevDispatch)));
     }
     CK(cudaEventCreateWithFlags(&image_free_ev_, cudaEventDisableTiming));
+    CK(cudaMallocHost(&h_active_count_, sizeof(uint32_t)));
+    b200pt_default_adaptive(&adaptive_);
     b200pt_default_atmosphere(&atmosphere_);
     memset(&last_, 0, sizeof last_);
 }
@@ -46,7 +49,8 @@ Engine::~Engine() {
     cudaSetDevice(device_);
     for (auto &st : aux_stream_) if (st) cudaStreamSynchronize(st);
     if (stream_) cudaStreamSynchronize(stream_);
-    free_scene(); free_wave(); free_post();
+    free_scene(); free_wave(); free_post(); free_adaptive();
+    if (h_active_count_) cudaFreeHost(h_active_count_);
     dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_); for (auto &l : d_luts_) dfree(l);
     dfree(d_image_); dfree(d_ctr_); dfree(d_volumes_); dfree(d_grids_); grids_.clear(); dfree(d_tri_class_);
     for (int c = 0; c < 2; c++) {
@@ -418,12 +422,79 @@ void Engine::set_luts(const float *refl, const float *rout, const float *rin) {
 void Engine::set_config(const b200pt_config &c) {
     if (c.SamplesPerFrame == 0 || c.ScreenChunkCount == 0 || c.ScreenChunkCount > 64) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "SamplesPerFrame and ScreenChunkCount must be >= 1" };
     if (c.ScreenChunkCount > 1 && world_ > 1) throw CudaError{ B200PT_ERR_NOT_IMPLEMENTED, "ScreenChunkCount > 1 cannot be combined with a multi-GPU partition" };
+    if (c.ScreenChunkCount > 1 && adaptive_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "ScreenChunkCount > 1 cannot be combined with adaptive sampling" };
     cfg_ = c;
     reset();
 }
+
+// ---------------------------------------------------------------- adaptive sampling
+void Engine::set_adaptive(const b200pt_adaptive &a) {
+    if (!std::isfinite(a.Threshold) || a.Threshold < 0.0f) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "adaptive Threshold must be finite and >= 0" };
+    if (a.MinSamples < 2 || a.Interval == 0) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "adaptive MinSamples must be >= 2 and Interval >= 1" };
+    if (a.Enable && cfg_.ScreenChunkCount > 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "adaptive sampling cannot be combined with ScreenChunkCount > 1" };
+    CK(cudaSetDevice(device_));
+    sync_all();
+    adaptive_ = a;
+    adaptive_.Enable = a.Enable ? 1u : 0u;
+    if (!adaptive_.Enable) free_adaptive();
+    reset();
+}
+void Engine::free_adaptive() {
+    dfree(d_px_state_); dfree(d_active_); dfree(d_tile_count_); dfree(d_active_count_);
+    adaptive_pixels_ = 0; adaptive_ready_ = false;
+}
+void Engine::update_active(bool decide, cudaStream_t st) {
+    const uint32_t npix = (uint32_t)adaptive_pixels_;
+    launch_adaptive_update(d_px_state_, npix, adaptive_.Threshold, adaptive_.MinSamples, decide, d_tile_count_, d_active_, d_active_count_, st);
+    CK(cudaMemcpyAsync(h_active_count_, d_active_count_, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    active_count_ = *h_active_count_;
+}
+// After a reset: every local pixel active with an empty record.
+void Engine::prepare_adaptive() {
+    if (adaptive_ready_) return;
+    sync_all();
+    const size_t npix = (size_t)W_ * local_rows_;
+    if (npix != adaptive_pixels_ || !d_px_state_) {
+        free_adaptive();
+        const size_t n = std::max<size_t>(npix, 1), tiles = (n + ADAPTIVE_TILE - 1) / ADAPTIVE_TILE;
+        CK(cudaMalloc(&d_px_state_, n * sizeof(uint4))); CK(cudaMalloc(&d_active_, n * sizeof(uint32_t)));
+        CK(cudaMalloc(&d_tile_count_, tiles * sizeof(uint32_t))); CK(cudaMalloc(&d_active_count_, sizeof(uint32_t)));
+        adaptive_pixels_ = npix;
+    }
+    CK(cudaMemsetAsync(d_px_state_, 0, std::max<size_t>(npix, 1) * sizeof(uint4), stream_));
+    update_active(false, stream_);
+    adaptive_ready_ = true;
+}
+uint32_t Engine::active_pixels() {
+    CK(cudaSetDevice(device_));
+    if (!adaptive_.Enable) return W_ * local_rows_;
+    if (!adaptive_ready_) { if (!has_scene_ || !W_) return W_ * local_rows_; prepare_adaptive(); }
+    return active_count_;
+}
+void Engine::pixel_stats(uint32_t *counts, float *rel_error) {
+    CK(cudaSetDevice(device_));
+    const size_t npix = (size_t)W_ * local_rows_;
+    if (!adaptive_.Enable || !adaptive_ready_) {
+        if (counts) std::fill(counts, counts + npix, frame_count_);
+        if (rel_error) std::fill(rel_error, rel_error + npix, std::nanf(""));
+        return;
+    }
+    sync_all();
+    std::vector<uint4> st(npix);
+    CK(cudaMemcpy(st.data(), d_px_state_, npix * sizeof(uint4), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < npix; i++) {
+        const uint32_t n = st[i].z;
+        if (counts) counts[i] = n;
+        if (rel_error) {
+            float meanL, M2; memcpy(&meanL, &st[i].x, 4); memcpy(&M2, &st[i].y, 4);
+            rel_error[i] = n < 2 ? std::nanf("") : (float)(std::sqrt((double)M2 / (double)(n - 1) / (double)n) / std::max((double)meanL, 1e-3));
+        }
+    }
+}
 void Engine::set_camera(const float vi[16], const float pi[16]) { memcpy(view_inv_, vi, sizeof view_inv_); memcpy(proj_inv_, pi, sizeof proj_inv_); reset(); }
 void Engine::get_camera(float vi[16], float pi[16]) const { memcpy(vi, view_inv_, sizeof view_inv_); memcpy(pi, proj_inv_, sizeof proj_inv_); }
-void Engine::reset() { dispatch_count_ = 0; frame_count_ = 0; samples_accumulated_ = 0; }   // PathTracer.h:183
+void Engine::reset() { dispatch_count_ = 0; frame_count_ = 0; samples_accumulated_ = 0; adaptive_ready_ = false; }   // PathTracer.h:183
 
 void Engine::resize(uint32_t w, uint32_t h) {                                                  // PathTracer::ResizeImage
     if (!w || !h || w > 65535 || h > 65535) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bad image size" };
@@ -505,6 +576,11 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "no environment map (PathTracer always loads one, PathTracer.cpp:202)" };
     if (!has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "no energy-compensation lookup tables (PathTracer.cpp:199-201)" };
     const uint32_t S = cfg_.ScreenChunkCount, S2 = S * S;
+    const bool adaptive = adaptive_.Enable != 0u;              // S == 1 (set_config / set_adaptive)
+    if (adaptive) {
+        prepare_adaptive();
+        if (active_count_ == 0) return true;                   // every local pixel has converged: nothing to launch, the dispatch counter stays
+    }
     // how many dispatches until MaxSamplesAccumulated (PathTracer.cpp:124-125,151-153)
     uint32_t todo = 0;
     { uint64_t d = dispatch_count_; uint32_t acc = samples_accumulated_;
@@ -524,22 +600,27 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     // B200PT_OVERLAP=0 runs one wave at a time on the caller's stream (also used while profiling per-kernel times).
     bool overlap = !profiling_;
     if (const char *e = getenv("B200PT_OVERLAP")) { if (atoi(e) == 0) overlap = false; }
-    uint32_t F = cfg_.FramesInFlight;
-    if (F == 0) {
+    uint64_t target = 0;                                      // auto wave size (paths per context), when FramesInFlight == 0
+    if (cfg_.FramesInFlight == 0) {
         // Auto wave size: up to 64 M paths per context (~24 GB of wavefront state at ~380 B per path; all contexts capped to a quarter of the free HBM): large enough
         // to amortise the floors above.  On an 80 GB H100 the quarter of free HBM, not the 64 M cap, sets the size.
-        uint64_t target = 64ull << 20;
+        target = 64ull << 20;
         size_t free_b = 0, total_b = 0;
         if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
             uint64_t have = 0; for (const auto &B : wb_) have += (uint64_t)B.cap * 400ull;       // what this engine already holds counts as available
             target = std::min<uint64_t>(target, std::max<uint64_t>(1ull << 20, ((uint64_t)free_b + have) / 4ull / 400ull / (overlap ? 2ull : 1ull)));
         }
-        F = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(256, target / P));
     }
-    F = std::min(F, todo);
-    { const uint32_t n_waves = (todo + F - 1) / F; F = (todo + n_waves - 1) / n_waves; }          // equal waves: 128 frames at F = 123 become 64 + 64, not 123 + 5
+    // frames per wave for `frames` frames of P paths each, at most `cap_frames`
+    auto wave_frames = [&](uint32_t frames, uint32_t Pw, uint32_t cap_frames) {
+        uint32_t F = cfg_.FramesInFlight;
+        if (F == 0) F = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(256, target / Pw));
+        F = std::max(1u, std::min({ F, frames, cap_frames }));
+        const uint32_t n_waves = (frames + F - 1) / F; return (frames + n_waves - 1) / n_waves;   // equal waves: 128 frames at F = 123 become 64 + 64, not 123 + 5
+    };
+    const uint32_t F = wave_frames(todo, P, todo);
     const int n_ctx = overlap ? 2 : 1;
-    ensure_wave((size_t)F * P, n_ctx);
+    ensure_wave((size_t)F * P, n_ctx);                        // adaptive: A <= P, so F * P is the worst case of every interval's waves too
     if (!overlap) join_waves();                               // single-stream mode runs on the caller's stream, behind whatever the internal streams still hold
     else CK(cudaEventRecord(image_free_ev_, stream_));        // what the caller has enqueued on the image so far (gather copy, post chain, set_hdr) precedes this call's resolves
     const DevConfig dc = make_dev_config();
@@ -570,63 +651,82 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     };
     mark(-1);
     cudaStream_t last_st = stream_;
-    for (uint32_t w0 = 0; w0 < todo; w0 += F) {
-        const uint32_t nd = std::min(F, todo - w0);
-        const int ctx = overlap ? (int)(wave_seq_ & 1ull) : 0;
-        WaveBuf &B = wb_[ctx];
-        cudaStream_t st = overlap ? aux_stream_[ctx] : stream_;
-        if (w0 == 0) CK(cudaEventRecord(ev_[0], st));
-        // this wave's slice of the dispatch table (PathTracer.cpp:127-150: FrameCount, Seed = PCG(seed + dispatch), ChunkIndex) travels on the wave's own stream
-        CK(cudaEventSynchronize(B.disp_ev));                  // the pinned copy is reusable once ITS last upload has executed
-        for (uint32_t i = 0; i < nd; i++) {
-            const uint64_t d = dispatch_count_ + w0 + i;
-            B.h_disp[i].FrameCount = (uint32_t)(d / S2); B.h_disp[i].Seed = pcg(base_seed + (uint32_t)d); B.h_disp[i].ChunkIndex = (uint32_t)(d % S2); B.h_disp[i]._pad = 0;
+    // Adaptive sampling cuts the frames into intervals: the waves of an interval trace the A pixels still active (P = A), and at the
+    // interval's end k_adaptive_update runs behind the last resolve and A is read back (one host sync per interval).
+    for (uint32_t s0 = 0; s0 < todo;) {
+        uint32_t seg = todo - s0, Pw = P, Fw = F;
+        const uint32_t *const act = adaptive ? d_active_ : nullptr;
+        if (adaptive) {
+            seg = (uint32_t)std::min<uint64_t>(seg, adaptive_.Interval - (dispatch_count_ + s0) % adaptive_.Interval);
+            Pw = active_count_;
+            Fw = wave_frames(seg, Pw, (uint32_t)std::min<size_t>(wave_cap_ / Pw, 1u << 30));
         }
-        CK(cudaMemcpyAsync(B.d_disp, B.h_disp, nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
-        CK(cudaEventRecord(B.disp_ev, st));
-        PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
-        if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
-        float4 *const hitb[2] = { B.so.hit, fuse == 2 ? B.so.bxdf_pdf : B.so.hit };
-        for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
-            if (camera) {
-                const Queues q0{ B.q_miss[0], B.q_hit[0], qcap };
-                CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, P, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, hitb[0], B.counts, q0, d_ctr_, st));
-            } else launch_raygen(lc_, dc, B.d_disp, nd, P, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st);
-            launches++; mark(0);
-            int cur = 0; uint32_t k = 0;
-            for (;;) {
-                uint32_t chunk = 16;
-                if (!medium && cfg_.MaxDepth - std::min(cfg_.MaxDepth, k) < chunk) chunk = cfg_.MaxDepth - std::min(cfg_.MaxDepth, k);
-                if (chunk == 0) break;
-                for (uint32_t b = 0; b < chunk; b++, k++) {
-                    const uint32_t par = k & 1u;
-                    const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
-                    if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
-                    if ((fuse != 2 || k == 0) && !(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
-                    launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
-                                             fuse, cmask, st); mark(2);
-                    if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
-                    cur ^= 1;
-                }
-                if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty
-                CK(cudaMemcpyAsync(B.h_count, B.counts + (k & 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-                CK(cudaStreamSynchronize(st));
-                if (B.h_count[0] == 0) break;
-                if (k > (1u << 20)) break;                    // runaway guard
+        for (uint32_t w0 = s0; w0 < s0 + seg; w0 += Fw) {
+            const uint32_t nd = std::min(Fw, s0 + seg - w0);
+            const int ctx = overlap ? (int)(wave_seq_ & 1ull) : 0;
+            WaveBuf &B = wb_[ctx];
+            cudaStream_t st = overlap ? aux_stream_[ctx] : stream_;
+            if (w0 == 0) CK(cudaEventRecord(ev_[0], st));
+            // this wave's slice of the dispatch table (PathTracer.cpp:127-150: FrameCount, Seed = PCG(seed + dispatch), ChunkIndex) travels on the wave's own stream
+            CK(cudaEventSynchronize(B.disp_ev));                  // the pinned copy is reusable once ITS last upload has executed
+            for (uint32_t i = 0; i < nd; i++) {
+                const uint64_t d = dispatch_count_ + w0 + i;
+                B.h_disp[i].FrameCount = (uint32_t)(d / S2); B.h_disp[i].Seed = pcg(base_seed + (uint32_t)d); B.h_disp[i].ChunkIndex = (uint32_t)(d % S2); B.h_disp[i]._pad = 0;
             }
-            bounces_total += k;
+            CK(cudaMemcpyAsync(B.d_disp, B.h_disp, nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
+            CK(cudaEventRecord(B.disp_ev, st));
+            PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
+            if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
+            float4 *const hitb[2] = { B.so.hit, fuse == 2 ? B.so.bxdf_pdf : B.so.hit };
+            for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
+                if (camera) {
+                    const Queues q0{ B.q_miss[0], B.q_hit[0], qcap };
+                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, hitb[0], B.counts, q0, d_ctr_, st, act));
+                } else launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
+                launches++; mark(0);
+                int cur = 0; uint32_t k = 0;
+                for (;;) {
+                    uint32_t chunk = 16;
+                    if (!medium && cfg_.MaxDepth - std::min(cfg_.MaxDepth, k) < chunk) chunk = cfg_.MaxDepth - std::min(cfg_.MaxDepth, k);
+                    if (chunk == 0) break;
+                    for (uint32_t b = 0; b < chunk; b++, k++) {
+                        const uint32_t par = k & 1u;
+                        const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
+                        if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
+                        if ((fuse != 2 || k == 0) && !(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
+                        launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
+                                                 fuse, cmask, st); mark(2);
+                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
+                        cur ^= 1;
+                    }
+                    if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty
+                    CK(cudaMemcpyAsync(B.h_count, B.counts + (k & 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+                    CK(cudaStreamSynchronize(st));
+                    if (B.h_count[0] == 0) break;
+                    if (k > (1u << 20)) break;                    // runaway guard
+                }
+                bounces_total += k;
+            }
+            // the running mean folds the waves in dispatch order: this wave's resolve waits for the previous wave's (the other stream, possibly an earlier call)
+            // and for whatever the caller enqueued on the image before this call
+            if (overlap) {
+                if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1], 0));
+                CK(cudaStreamWaitEvent(st, image_free_ev_, 0));
+            }
+            if (adaptive) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_, B.sample_buf, d_image_, d_px_state_, st);
+            else launch_resolve(lc_, dc, B.d_disp, nd, P, B.sample_buf, d_image_, st);
+            CK(cudaEventRecord(resolved_ev_[ctx], st));
+            wave_seq_++;
+            launches++; waves++; mark(4);
+            last_st = st;
         }
-        // the running mean folds the waves in dispatch order: this wave's resolve waits for the previous wave's (the other stream, possibly an earlier call)
-        // and for whatever the caller enqueued on the image before this call
-        if (overlap) {
-            if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1], 0));
-            CK(cudaStreamWaitEvent(st, image_free_ev_, 0));
+        s0 += seg;
+        if (adaptive && (dispatch_count_ + s0) % adaptive_.Interval == 0) {
+            // the last resolve of the interval follows every earlier wave's resolve (and so every camera kernel that read the list)
+            update_active(true, last_st);
+            launches += 2;
+            if (active_count_ == 0) { todo = s0; break; }     // the frames not traced do not count
         }
-        launch_resolve(lc_, dc, B.d_disp, nd, P, B.sample_buf, d_image_, st);
-        CK(cudaEventRecord(resolved_ev_[ctx], st));
-        wave_seq_++;
-        launches++; waves++; mark(4);
-        last_st = st;
     }
     CK(cudaEventRecord(ev_[1], last_st));                     // ms_total: first kernel of the first wave .. resolve of the last (counters() synchronises before reading it)
     CK(cudaGetLastError());
@@ -640,7 +740,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
         float *acc[5] = { &last_.ms_raygen, &last_.ms_extend, &last_.ms_shade, &last_.ms_connect, &last_.ms_resolve };
         for (size_t i = 1; i < prof_n; i++) { float ms = 0.0f; CK(cudaEventElapsedTime(&ms, prof_ev_[i - 1], prof_ev_[i])); if (prof_kind[i] >= 0) *acc[prof_kind[i]] += ms; }
     }
-    return samples_accumulated_ >= cfg_.MaxSamplesAccumulated;
+    return samples_accumulated_ >= cfg_.MaxSamplesAccumulated || (adaptive && active_count_ == 0);
 }
 
 void Engine::set_stream(cudaStream_t s) {
@@ -681,7 +781,8 @@ void Engine::set_hdr(const float *src, bool dev) {
 // ---------------------------------------------------------------- checkpoint / resume
 // The whole progressive state of the reference is the RGBA32F image + three counters (PT/PathTracer.h:199-201); frame f always uses
 // Seed_f = PCG(base_seed + dispatch index), so a render resumed from a checkpoint continues the SAME sample sequence: N frames in one go
-// and k frames + checkpoint + (N - k) frames give bit-identical images (tested).  File: 64-byte header + local rows of float4.
+// and k frames + checkpoint + (N - k) frames give bit-identical images (tested).  File: 64-byte header + local rows of float4; version 2
+// (adaptive sampling on) appends the 16-byte b200pt_adaptive block and one 16-byte record per local pixel.
 namespace {
 struct CkptHeader { char magic[8]; uint32_t version, W, H, rank, world, band, local_rows, frame_count, samples_accumulated, samples_per_frame, chunk_count, _pad; uint64_t dispatch_count; };
 static_assert(sizeof(CkptHeader) == 64, "checkpoint header is 64 B");
@@ -691,12 +792,20 @@ void Engine::save_checkpoint(const char *path) {
     if (!d_image_ || !path) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no image to checkpoint" };
     std::vector<float> img((size_t)W_ * local_rows_ * 4);
     get_hdr(img.data(), false);
-    CkptHeader h{}; memcpy(h.magic, "B2PTCKPT", 8); h.version = 1; h.W = W_; h.H = H_; h.rank = rank_; h.world = world_; h.band = band_; h.local_rows = local_rows_;
+    const bool adaptive = adaptive_.Enable != 0u;
+    std::vector<uint4> px;                                    // version 2 (adaptive sampling on): + the adaptive block + one 16-B record per local pixel
+    if (adaptive) {
+        prepare_adaptive();
+        px.resize((size_t)W_ * local_rows_);
+        CK(cudaMemcpy(px.data(), d_px_state_, px.size() * sizeof(uint4), cudaMemcpyDeviceToHost));
+    }
+    CkptHeader h{}; memcpy(h.magic, "B2PTCKPT", 8); h.version = adaptive ? 2 : 1; h.W = W_; h.H = H_; h.rank = rank_; h.world = world_; h.band = band_; h.local_rows = local_rows_;
     h.frame_count = frame_count_; h.samples_accumulated = samples_accumulated_; h.samples_per_frame = cfg_.SamplesPerFrame; h.chunk_count = cfg_.ScreenChunkCount;
     h.dispatch_count = dispatch_count_;
     FILE *f = fopen(path, "wb");
     if (!f) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, std::string("cannot open checkpoint for writing: ") + path };
-    const bool ok = fwrite(&h, sizeof h, 1, f) == 1 && fwrite(img.data(), sizeof(float), img.size(), f) == img.size();
+    bool ok = fwrite(&h, sizeof h, 1, f) == 1 && fwrite(img.data(), sizeof(float), img.size(), f) == img.size();
+    if (ok && adaptive) ok = fwrite(&adaptive_, sizeof adaptive_, 1, f) == 1 && fwrite(px.data(), sizeof(uint4), px.size(), f) == px.size();
     if (fclose(f) != 0 || !ok) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "short write of the checkpoint" };
 }
 void Engine::load_checkpoint(const char *path) {
@@ -706,14 +815,28 @@ void Engine::load_checkpoint(const char *path) {
     if (!f) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, std::string("cannot open checkpoint: ") + path };
     CkptHeader h{};
     std::vector<float> img;
-    bool ok = fread(&h, sizeof h, 1, f) == 1 && memcmp(h.magic, "B2PTCKPT", 8) == 0 && h.version == 1;
+    bool ok = fread(&h, sizeof h, 1, f) == 1 && memcmp(h.magic, "B2PTCKPT", 8) == 0 && (h.version == 1 || h.version == 2);
     const bool fits = ok && h.W == W_ && h.H == H_ && h.rank == rank_ && h.world == world_ && h.band == band_ && h.local_rows == local_rows_ &&
                       h.samples_per_frame == cfg_.SamplesPerFrame && h.chunk_count == cfg_.ScreenChunkCount;
     if (fits) { img.resize((size_t)W_ * local_rows_ * 4); ok = fread(img.data(), sizeof(float), img.size(), f) == img.size(); }
+    // version 2 (adaptive sampling): the adaptive block must equal this handle's; version 1 cannot resume an adaptive render
+    b200pt_adaptive blk{}; std::vector<uint4> px;
+    bool same_mode = h.version == (adaptive_.Enable ? 2u : 1u);
+    if (fits && ok && same_mode && h.version == 2) {
+        ok = fread(&blk, sizeof blk, 1, f) == 1;
+        same_mode = ok && memcmp(&blk, &adaptive_, sizeof blk) == 0;
+        if (same_mode) { px.resize((size_t)W_ * local_rows_); ok = fread(px.data(), sizeof(uint4), px.size(), f) == px.size(); }
+    }
     fclose(f);
     if (!ok) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "not a b200pt checkpoint (bad magic / version / truncated)" };
     if (!fits) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "checkpoint was taken with another image size, partition, SamplesPerFrame or ScreenChunkCount" };
+    if (!same_mode) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "checkpoint was taken with other adaptive-sampling settings" };
     set_hdr(img.data(), false);
+    if (adaptive_.Enable) {                                   // the records, then the active list rebuilt from their flags
+        reset(); prepare_adaptive();
+        CK(cudaMemcpy(d_px_state_, px.data(), px.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+        update_active(false, stream_);
+    }
     dispatch_count_ = h.dispatch_count; frame_count_ = h.frame_count; samples_accumulated_ = h.samples_accumulated;
 }
 

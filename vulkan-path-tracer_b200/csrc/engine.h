@@ -43,7 +43,13 @@ public:
     uint32_t local_rows() const { return local_rows_; }
     uint32_t samples_accumulated() const { return samples_accumulated_; }
 
-    // PathTracer::PathTrace x dispatches; returns true when all samples are accumulated
+    // adaptive sampling (no reference equivalent): per-pixel stop once the running mean has converged; any set resets the accumulation
+    void set_adaptive(const b200pt_adaptive &a);
+    const b200pt_adaptive &adaptive() const { return adaptive_; }
+    void pixel_stats(uint32_t *counts, float *rel_error);   // local pixels: frames accumulated, relative standard error of the mean luminance
+    uint32_t active_pixels();                               // local pixels still traced
+
+    // PathTracer::PathTrace x dispatches; returns true when all samples are accumulated (or, adaptive, no local pixel is active)
     bool path_trace(uint32_t dispatches, uint32_t base_seed);
     void synchronize();
     void flush() { check(cudaSetDevice(device_), "cudaSetDevice"); join_waves(); }   // device-side: the caller's stream waits for every launched wave
@@ -146,6 +152,17 @@ private:
     void join_waves();                              // work enqueued on the caller's stream from here on sees every launched wave resolved into the image
     WaveCounters *d_ctr_ = nullptr;
     b200pt_counters last_{};
+
+    // adaptive sampling: allocated only while enabled.  The state is rebuilt lazily (prepare_adaptive) after every reset.
+    b200pt_adaptive adaptive_{};
+    uint4 *d_px_state_ = nullptr;                   // one record per local pixel (kernels.h: meanL, M2, n_p, flags)
+    uint32_t *d_active_ = nullptr, *d_tile_count_ = nullptr, *d_active_count_ = nullptr, *h_active_count_ = nullptr;
+    size_t adaptive_pixels_ = 0;                    // local pixels the buffers were sized for
+    uint32_t active_count_ = 0;                     // A: entries of d_active_ (host copy, read back at every interval boundary)
+    bool adaptive_ready_ = false;                   // the state matches the accumulation (false after reset)
+    void prepare_adaptive();
+    void free_adaptive();
+    void update_active(bool decide, cudaStream_t st);   // decision / list rebuild on st, then A read back (blocks the host)
 };
 
 } // namespace b200pt

@@ -26,12 +26,24 @@ struct LaunchCfg {
 };
 
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc);
+// active (adaptive sampling): P is the active count and wave entry i of a dispatch traces local pixel active[i]; nullptr = every pixel
 void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st);
+                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active = nullptr);
 // launch_raygen + the camera rays' launch_extend in one kernel (LaunchCfg::camera, no pre-pass): clears the control block on `st`, writes the
 // path state, the hit records (hit_out) and the parity-0 queues.  Returns cudaError_t as int.
 int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st);
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st,
+                  const uint32_t *active = nullptr);
+// ---- adaptive sampling: per local pixel one 16-B record {meanL, M2 (float bits), n_p, flags} (Engine::d_px_state_) ----
+constexpr uint32_t ADAPTIVE_TILE = 2048;      // pixels per block of the two compaction passes
+constexpr uint32_t PX_CONVERGED = 1u;         // flags bit: the pixel is never traced again
+// k_resolve over the active list: folds slot b * A + i of every dispatch into pixel active[i] with the pixel's own count, updates its record
+void launch_resolve_adaptive(const LaunchCfg &lc, const DevConfig &cfg, uint32_t n_disp, uint32_t A, const uint32_t *active,
+                             const float4 *sample_buf, float4 *image, uint4 *state, cudaStream_t st);
+// decision at an interval boundary (decide: flag the converged pixels; otherwise only rebuild the list), then the stable compaction of the
+// active pixels into `active` and their count into *active_count (device).  tile_count: ceil(npix / ADAPTIVE_TILE) words of scratch.
+void launch_adaptive_update(uint4 *state, uint32_t npix, float threshold, uint32_t min_samples, bool decide, uint32_t *tile_count,
+                            uint32_t *active, uint32_t *active_count, cudaStream_t st);
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st);
 // k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.

@@ -18,6 +18,8 @@
 //   run the bounce as ONE kernel per class (k_shade_hit<CLASS, ., 2>): shading + both NEE shadow queries + roulette + the next segment's
 //   closest-hit query + queue append.
 //   k_resolve  NaN/Inf rejection + running mean                SH/RayGen.slang:116-159
+//   (adaptive sampling, no reference equivalent: k_raygen / k_camera over a list of active pixels, k_resolve_adaptive, and
+//    k_adaptive_update + k_adaptive_compact at interval boundaries)
 //
 // Every path owns one sample slot, so radiance accumulation needs no atomics and is deterministic.
 // All per-path state is SoA float4 (coalesced 16-B lanes); live paths are kept dense by compaction.
@@ -51,14 +53,18 @@ __device__ __forceinline__ float3 camera_eye(const DevConfig &cfg) {
 
 // ------------------------------------------------------------------------------------------------
 // camera_path : camera sample + payload init of path j of a wave (k_raygen, k_camera); returns the camera ray
+// ADAPTIVE: the wave holds P = A active pixels per dispatch, entry i of a dispatch traces local pixel active[i] (adaptive sampling).  Only the
+// pixel changes: the slot stays j, and the RNG is keyed on the pixel as always, so a pixel's frames are those of the plain renderer.
 // ------------------------------------------------------------------------------------------------
+template <bool ADAPTIVE>
 __device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispatch *__restrict__ disp, uint32_t P, uint32_t first_sample,
                                             const uint32_t *__restrict__ rng_carry, const PathState &ps, float4 *__restrict__ sample_buf,
-                                            uint32_t j, float3 &ray_o, float3 &ray_d) {
+                                            uint32_t j, float3 &ray_o, float3 &ray_d, const uint32_t *__restrict__ active) {
     const uint32_t S = cfg.ScreenSplitCount;
     const uint32_t LW = (cfg.W + S - 1) / S;
     {
-        const uint32_t b = j / P, p = j - b * P;
+        const uint32_t b = j / P, i = j - b * P;
+        const uint32_t p = ADAPTIVE ? __ldg(active + i) : i;
         const DevDispatch dd = disp[b];
         uint32_t x, y;
         if (S == 1) {
@@ -102,14 +108,16 @@ __device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispa
 // ------------------------------------------------------------------------------------------------
 // k_raygen (pipelines without k_camera: volumes / atmosphere pre-pass, BVH outside shared memory, B200PT_CAMERA=0)
 // ------------------------------------------------------------------------------------------------
+// ADAPTIVE: P = the active count, entry i traces pixel active[i] (camera_path); `active` is unused otherwise.
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
                                                  uint32_t first_sample, const uint32_t *__restrict__ rng_carry,
                                                  PathState ps, float4 *__restrict__ sample_buf, uint32_t *__restrict__ ctrl,
-                                                 WaveCounters *ctr) {
+                                                 WaveCounters *ctr, const uint32_t *__restrict__ active) {
     const uint32_t n = n_disp * P;
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
         float3 o, d;
-        camera_path(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, j, o, d);
+        camera_path<ADAPTIVE>(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, j, o, d, active);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { for (uint32_t w = 0; w < CTRL_WORDS; w++) ctrl[w] = 0; ctrl[0] = n; atomicAdd(&ctr->paths, (unsigned long long)n); }
 }
@@ -290,12 +298,12 @@ __global__ void __launch_bounds__(SMEM ? EXTEND_SMEM_MAX_THREADS : 512) k_extend
 //            The control block is cleared on the stream before the launch (launch_camera): the appends of other CTAs may run before
 //            block 0 does.
 // ------------------------------------------------------------------------------------------------
-// 64 registers: 4 CTAs of 256 threads per SM (big mode: 2 of 512).
-template <bool UNIFORM>
+// 64 registers: 4 CTAs of 256 threads per SM (big mode: 2 of 512).  ADAPTIVE: as k_raygen<true> (P = active count, `active_px` unused otherwise).
+template <bool UNIFORM, bool ADAPTIVE>
 __global__ void __launch_bounds__(512, 2) k_camera(DevScene sc, DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
                                                    uint32_t first_sample, const uint32_t *__restrict__ rng_carry, PathState ps,
                                                    float4 *__restrict__ sample_buf, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl,
-                                                   Queues q, int max_stack, WaveCounters *ctr) {
+                                                   Queues q, int max_stack, WaveCounters *ctr, const uint32_t *__restrict__ active_px) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
@@ -331,7 +339,7 @@ __global__ void __launch_bounds__(512, 2) k_camera(DevScene sc, DevConfig cfg, c
             bool hit = false;
             uint32_t code = Q_NONE;
             float3 o = f3(0.0f), d = o;
-            if (active) camera_path(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, i, o, d);
+            if (active) camera_path<ADAPTIVE>(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, i, o, d, active_px);
             bool at_eye = false;
             if (fixed) {
                 const float4 e = fixed_eye;
@@ -1314,6 +1322,98 @@ __global__ void __launch_bounds__(256) k_resolve(DevConfig cfg, const DevDispatc
 }
 
 // ------------------------------------------------------------------------------------------------
+// adaptive sampling (no reference equivalent).  Per local pixel one 16-B record (AdaptivePixel): the running mean and Welford second-moment
+// term of the per-frame luminance, the pixel's own frame count n_p and the converged flag.
+// ------------------------------------------------------------------------------------------------
+// k_resolve_adaptive : k_resolve over the active list.  Entry i of dispatch b (slot b * A + i) belongs to pixel active[i]; the running mean
+// uses the pixel's own count n_p in place of FrameCount, which is the same arithmetic for a pixel traced in every frame.
+__global__ void __launch_bounds__(256) k_resolve_adaptive(DevConfig cfg, uint32_t n_disp, uint32_t A, const uint32_t *__restrict__ active,
+                                                           const float4 *__restrict__ sample_buf, float4 *__restrict__ image, uint4 *__restrict__ state) {
+    const float inv_spp = (float)cfg.SampleCount;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A; i += gridDim.x * blockDim.x) {
+        const uint32_t q = active[i];
+        const uint4 st = state[q];
+        float meanL = __uint_as_float(st.x), M2 = __uint_as_float(st.y);
+        uint32_t n = st.z;
+        float3 color = f3(image[q]);
+        for (uint32_t b = 0; b < n_disp; b++) {
+            const float3 acc = f3(sample_buf[(size_t)b * A + i]) / inv_spp;
+            if (n > 0) {                                                            // mix3 rounded as k_resolve compiles it: fma(acc, a, color * (1 - a))
+                const float a = 1.0f / (float)(n + 1u), ra = 1.0f - a;
+                color = f3(__fmaf_rn(acc.x, a, __fmul_rn(color.x, ra)), __fmaf_rn(acc.y, a, __fmul_rn(color.y, ra)), __fmaf_rn(acc.z, a, __fmul_rn(color.z, ra)));
+            } else color = acc;
+            n++;
+            const float L = dot(acc, f3(0.212671f, 0.715160f, 0.072169f));          // the MaxLuminance clamp's weights
+            const float delta = L - meanL;                                          // Welford
+            meanL += delta / (float)n;
+            M2 += delta * (L - meanL);
+        }
+        image[q] = make_float4(color.x, color.y, color.z, 1.0f);
+        state[q] = make_uint4(__float_as_uint(meanL), __float_as_uint(M2), n, st.w);
+    }
+}
+
+// Relative standard error of the mean luminance with an absolute floor for black pixels: converged iff it is <= Threshold.  Threshold 0 stops
+// nothing (a pixel of constant luminance would otherwise meet 0 <= 0).
+__device__ __forceinline__ bool adaptive_converged(uint4 st, float threshold, uint32_t min_samples) {
+    const uint32_t n = st.z;
+    if (threshold <= 0.0f || n < min_samples) return false;
+    const float err = sqrtf(__uint_as_float(st.y) / (float)(n - 1u) / (float)n);
+    return err <= threshold * fmaxf(__uint_as_float(st.x), 1e-3f);
+}
+
+// k_adaptive_update : the decision at an interval boundary (decide == 0: none, the active list is only rebuilt from the flags).  Block t owns
+// pixels [t * ADAPTIVE_TILE, (t + 1) * ADAPTIVE_TILE): it flags the pixels that converge and writes how many of its pixels stay active.
+__global__ void __launch_bounds__(256) k_adaptive_update(uint4 *__restrict__ state, uint32_t npix, float threshold, uint32_t min_samples, uint32_t decide,
+                                                          uint32_t *__restrict__ tile_count) {
+    const uint32_t base = blockIdx.x * ADAPTIVE_TILE;
+    uint32_t keep = 0;
+    for (uint32_t k = threadIdx.x; k < ADAPTIVE_TILE; k += blockDim.x) {
+        const uint32_t q = base + k;
+        if (q >= npix) break;
+        uint4 st = state[q];
+        if (!(st.w & PX_CONVERGED) && decide && adaptive_converged(st, threshold, min_samples)) { st.w |= PX_CONVERGED; state[q].w = st.w; }
+        keep += (st.w & PX_CONVERGED) ? 0u : 1u;
+    }
+    keep = __reduce_add_sync(0xFFFFFFFFu, keep);
+    __shared__ uint32_t warp_sum[8];
+    if ((threadIdx.x & 31u) == 0u) warp_sum[threadIdx.x >> 5] = keep;
+    __syncthreads();
+    if (threadIdx.x == 0) { uint32_t s = 0; for (uint32_t w = 0; w < blockDim.x / 32u; w++) s += warp_sum[w]; tile_count[blockIdx.x] = s; }
+}
+
+// k_adaptive_compact : second pass, stable compaction of the pixels that stay active into the active list (pixel order, so neighbouring pixels
+// keep neighbouring lanes and their camera rays stay coherent).  A tile's offset is the sum of the counts of the tiles before it; inside the
+// tile, 256 pixels per round are placed by a warp ballot / popc and a scan over the 8 warp counts.  The last block writes the active count A.
+__global__ void __launch_bounds__(256) k_adaptive_compact(const uint4 *__restrict__ state, uint32_t npix, const uint32_t *__restrict__ tile_count,
+                                                           uint32_t *__restrict__ active, uint32_t *__restrict__ active_count) {
+    __shared__ uint32_t warp_sum[8], s_base;
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    uint32_t part = 0;
+    for (uint32_t t = threadIdx.x; t < blockIdx.x; t += blockDim.x) part += tile_count[t];
+    part = __reduce_add_sync(0xFFFFFFFFu, part);
+    if (lane == 0u) warp_sum[warp] = part;
+    __syncthreads();
+    if (threadIdx.x == 0) { uint32_t s = 0; for (uint32_t w = 0; w < 8u; w++) s += warp_sum[w]; s_base = s; }
+    __syncthreads();
+    uint32_t base = s_base;
+    for (uint32_t r = 0; r < ADAPTIVE_TILE / 256u; r++) {
+        const uint32_t q = blockIdx.x * ADAPTIVE_TILE + r * 256u + threadIdx.x;
+        const bool keep = q < npix && !(state[q].w & PX_CONVERGED);
+        const uint32_t bal = __ballot_sync(0xFFFFFFFFu, keep);
+        __syncthreads();                                                    // warp_sum of the previous round has been read
+        if (lane == 0u) warp_sum[warp] = (uint32_t)__popc(bal);
+        __syncthreads();
+        uint32_t before = 0, total = 0;
+        #pragma unroll
+        for (uint32_t w = 0; w < 8u; w++) { const uint32_t c = warp_sum[w]; before += w < warp ? c : 0u; total += c; }
+        if (keep) active[base + before + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = q;
+        base += total;
+    }
+    if (blockIdx.x == gridDim.x - 1u && threadIdx.x == 0) *active_count = base;
+}
+
+// ------------------------------------------------------------------------------------------------
 // test hook: closest-hit for arbitrary rays (b200pt_trace_closest)
 // ------------------------------------------------------------------------------------------------
 template <bool SMEM>
@@ -1373,7 +1473,8 @@ static int set_attrs_for_current_device() {
                                optin((const void *)k_extend<false, true, U>); optin((const void *)k_extend<false, false, U>);
     B200PT_OPTIN_EXTEND(true) B200PT_OPTIN_EXTEND(false)
 #undef B200PT_OPTIN_EXTEND
-    optin((const void *)k_camera<true>); optin((const void *)k_camera<false>);
+    optin((const void *)k_camera<true, false>); optin((const void *)k_camera<false, false>);
+    optin((const void *)k_camera<true, true>); optin((const void *)k_camera<false, true>);
     optin((const void *)k_connect<true, true>); optin((const void *)k_connect<false, true>); optin((const void *)k_connect<false, false>);
     optin((const void *)k_connect<true, true, true>); optin((const void *)k_connect<false, true, true>); optin((const void *)k_connect<false, false, true>);
     optin((const void *)k_extend_dyn<true, true, false>); optin((const void *)k_extend_dyn<true, false, false>);
@@ -1480,8 +1581,8 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     int occ_cam = 0;
     if (lc->camera) {
         int occ_u = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_cam, k_camera<false>, lc->extend_threads, sh);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_camera<true>, lc->extend_threads, sh);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_cam, k_camera<false, false>, lc->extend_threads, sh);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_camera<true, false>, lc->extend_threads, sh);
         if (occ_u < occ_cam) occ_cam = occ_u;
     }
     lc->grid_camera = sms * (occ_cam < 1 ? 1 : occ_cam);
@@ -1494,18 +1595,33 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
 }
 
 void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st) {
-    k_raygen<<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr);
+                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active) {
+    if (active) k_raygen<true><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr, active);
+    else k_raygen<false><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr, nullptr);
 }
 int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st) {
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st,
+                  const uint32_t *active) {
     set_attrs_for_current_device();
     const cudaError_t e = cudaMemsetAsync(ctrl, 0, CTRL_WORDS * sizeof(uint32_t), st);   // before any CTA appends to the parity-0 queues
     if (e != cudaSuccess) return (int)e;
     const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, true);
-    if (sc.uniform_class != 0xFFu) k_camera<true><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr);
-    else k_camera<false><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr);
+#define B200PT_CAM(U, A) k_camera<U, A><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr, active)
+    if (sc.uniform_class != 0xFFu) { if (active) B200PT_CAM(true, true); else B200PT_CAM(true, false); }
+    else { if (active) B200PT_CAM(false, true); else B200PT_CAM(false, false); }
+#undef B200PT_CAM
     return 0;
+}
+void launch_resolve_adaptive(const LaunchCfg &lc, const DevConfig &cfg, uint32_t n_disp, uint32_t A, const uint32_t *active,
+                             const float4 *sample_buf, float4 *image, uint4 *state, cudaStream_t st) {
+    k_resolve_adaptive<<<lc.grid_light, 256, 0, st>>>(cfg, n_disp, A, active, sample_buf, image, state);
+}
+void launch_adaptive_update(uint4 *state, uint32_t npix, float threshold, uint32_t min_samples, bool decide, uint32_t *tile_count,
+                            uint32_t *active, uint32_t *active_count, cudaStream_t st) {
+    const uint32_t tiles = (npix + ADAPTIVE_TILE - 1u) / ADAPTIVE_TILE;
+    if (!tiles) { cudaMemsetAsync(active_count, 0, sizeof(uint32_t), st); return; }
+    k_adaptive_update<<<tiles, 256, 0, st>>>(state, npix, threshold, min_samples, decide ? 1u : 0u, tile_count);
+    k_adaptive_compact<<<tiles, 256, 0, st>>>(state, npix, tile_count, active, active_count);
 }
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st) {
