@@ -233,6 +233,36 @@ int32_t b200pt_get_adaptive(b200pt_handle h, b200pt_adaptive *out);
  * sqrt(M2 / (n_p - 1) / n_p) / max(mean, 1e-3) (NaN without adaptive sampling or with n_p < 2).  Either pointer may be NULL. */
 int32_t b200pt_get_pixel_stats(b200pt_handle h, uint32_t *counts, float *rel_error);
 int32_t b200pt_active_pixels(b200pt_handle h, uint32_t *out);             /* local pixels still traced (all of them without adaptive sampling) */
+/* Per-pixel statistics without adaptive sampling: with enable != 0 the handle keeps the same per-pixel records as adaptive sampling
+ * (frame count, Welford mean / M2 of the per-frame luminance) for every local pixel, but takes no decisions: every pixel is traced in every
+ * frame, and the image and the work counters are bit-identical to a run without statistics.  b200pt_get_pixel_stats then reports rel_error,
+ * and checkpoints use version 2 (the adaptive block as set, then the records).  With adaptive sampling on, its records are the statistics.
+ * Not combinable with ScreenChunkCount > 1.  Any set resets the accumulation, as b200pt_set_adaptive does. */
+int32_t b200pt_set_track_variance(b200pt_handle h, int32_t enable);
+int32_t b200pt_get_track_variance(b200pt_handle h, int32_t *out);
+
+/* ---- denoiser (no reference equivalent; DESIGN.md section 12) ----
+ * An a-trous wavelet filter (Dammertz et al. 2010) with the edge-stopping weights of SVGF (Schied et al. 2017) on the albedo-demodulated
+ * accumulation, guided by per-pixel features of the first surface seen through the pixel and by the variance of the pixel's mean luminance.
+ * Features: FeatureSamples camera rays per pixel (jitter and depth of field as the render), closest hit only (volumes and the atmosphere are
+ * not seen).  albedo_cov = (mean albedo (pd + pm) * BaseColor + pg, a miss counting 1; coverage = fraction of rays that hit),
+ * normal_depth = (mean world-space shading normal, misses counting 0, not renormalised; mean view depth of the hits, 0 without hits).
+ * variance = M2 / (n - 1) / n of the records, 1e30 below two frames.  The denoised image is biased by design; the accumulation stays the
+ * reference-matching output.  WRONG_ARGUMENTS: Iterations > 10, FeatureSamples 0 or > 256, a sigma negative or not finite, null pointers. */
+typedef struct { uint32_t Iterations; uint32_t FeatureSamples; float SigmaLuminance; float SigmaNormal; float SigmaDepth; } b200pt_denoise_params;   /* defaults {5, 8, 4, 128, 1} */
+int32_t b200pt_default_denoise(b200pt_denoise_params *out);
+/* feature pass + filter into a denoised RGBA32F W*H image owned by the handle; the accumulation image is not touched.  Needs statistics or
+ * adaptive sampling on and world == 1 (WRONG_ARGUMENTS otherwise).  elapsed_ms (optional): device time of the feature pass and the filter. */
+int32_t b200pt_denoise(b200pt_handle h, const b200pt_denoise_params *p, float *elapsed_ms);
+int32_t b200pt_get_denoised(b200pt_handle h, float *dst_rgba32f, int32_t dst_is_device);   /* W*H*4 floats of the last b200pt_denoise */
+/* the filter's inputs for this handle's local rows (any partition; host memory; each pointer may be NULL): albedo_cov and normal_depth
+ * local_rows*W*4 floats, variance local_rows*W floats.  Needs statistics or adaptive sampling on.  What an external denoiser is fed, and
+ * what a multi-GPU caller gathers to rank 0 for b200pt_denoise_image. */
+int32_t b200pt_get_denoise_inputs(b200pt_handle h, const b200pt_denoise_params *p, float *albedo_cov, float *normal_depth, float *variance);
+/* the filter alone on caller buffers of a width x height image (all host or all device memory): color / albedo_cov / normal_depth / out
+ * RGBA32F, variance one float per pixel.  Iterations == 0 copies color to out bit for bit. */
+int32_t b200pt_denoise_image(b200pt_handle h, uint32_t width, uint32_t height, const float *color, const float *albedo_cov, const float *normal_depth,
+                             const float *variance, const b200pt_denoise_params *p, float *out, int32_t is_device);
 int32_t b200pt_synchronize(b200pt_handle h);
 /* b200pt_path_trace is ASYNCHRONOUS: it returns once the waves are enqueued (two waves are in flight on the handle's internal streams so that the
  * latency-bound tail of one overlaps the head of the next, also across calls).  Every later call on the handle that touches the image (get_hdr,
@@ -265,6 +295,7 @@ int32_t b200pt_get_counters(b200pt_handle h, b200pt_counters *out);
 int32_t b200pt_post_set_tonemap(b200pt_handle h, const b200pt_tonemap *t);  /* SetTonemappingData */
 int32_t b200pt_post_set_bloom(b200pt_handle h, const b200pt_bloom *b);      /* SetBloomData */
 int32_t b200pt_post_process(b200pt_handle h);                               /* PostProcess(cmd); input = GetOutputImage() */
+int32_t b200pt_post_process_denoised(b200pt_handle h);                      /* the same chain on the image of the last b200pt_denoise */
 int32_t b200pt_get_ldr(b200pt_handle h, uint8_t *dst_rgba8, int32_t dst_is_device); /* GetOutputImageView() -> RGBA8 */
 /* Multi-GPU post pass (BASELINE config 5; no reference equivalent): PostProcess for output rows [y0, y1) only.  Every rank holds the full HDR input
  * (b200pt_set_hdr) and recomputes the few halo rows of each bloom mip its block depends on, so the rows equal those of b200pt_post_process bit for

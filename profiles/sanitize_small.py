@@ -36,6 +36,15 @@ def _adaptive(name, **kw):                                          # adaptive s
     assert np.isfinite(T.get_hdr()).all() and 0 <= T.active_pixels() <= 40 * 30
     print(name, "adaptive", T.active_pixels(), "ok")
 _adaptive("cornell_box"); _adaptive("cornell_box", Volumes=[FOG])
+def _denoise(name, **kw):                                           # per-pixel statistics, k_features<SMEM>, k_record_variance, the a-trous filter, its post chain
+    T = util.product_tracer(name, 40, 30, MaxDepth=5, **kw)
+    T.set_track_variance(True)
+    T.path_trace(4, util.BASE_SEED)
+    T.denoise(FeatureSamples=2); d = T.get_denoised(); assert np.isfinite(d).all()
+    a, nd, v = T.denoise_inputs(FeatureSamples=2); T.denoise_image(T.get_hdr(), a, nd, v, Iterations=2)
+    T.post_process_denoised(); T.get_ldr()
+    print(name, "denoise ok")
+_denoise("cornell_box"); _denoise("cornell_box_glass")
 run("cornell_box_glass", 48, 48, 2, 8)                              # dynamic-fetch BVH2 kernels, class queues (glass / diffuse)
 os.environ["B200PT_WIDE"] = "1"; run("viking_room", 48, 48, 1, 4); del os.environ["B200PT_WIDE"]              # BVH4 + textures
 print("sanitize_small done")

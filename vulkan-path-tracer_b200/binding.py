@@ -123,6 +123,16 @@ def default_adaptive(**kw):
     return a
 
 
+class DenoiseParams(C.Structure):    # b200pt_denoise_params: the a-trous denoiser (no reference equivalent)
+    _fields_ = [("Iterations", C.c_uint32), ("FeatureSamples", C.c_uint32), ("SigmaLuminance", C.c_float), ("SigmaNormal", C.c_float), ("SigmaDepth", C.c_float)]
+
+
+def default_denoise(**kw):
+    d = DenoiseParams(); lib().b200pt_default_denoise(C.byref(d))
+    for k, v in kw.items(): setattr(d, k, v)
+    return d
+
+
 class Counters(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("paths", "extend_rays", "shade_invocations", "surface_hits", "misses", "shadow_rays", "medium_events", "kernel_launches")] + \
                [(n, C.c_float) for n in ("ms_total", "ms_raygen", "ms_extend", "ms_shade", "ms_connect", "ms_resolve")] + \
@@ -192,6 +202,12 @@ def lib():
             "b200pt_default_adaptive": [C.POINTER(Adaptive)], "b200pt_set_adaptive": [C.c_void_p, C.POINTER(Adaptive)],
             "b200pt_get_adaptive": [C.c_void_p, C.POINTER(Adaptive)], "b200pt_get_pixel_stats": [C.c_void_p, C.c_void_p, C.c_void_p],
             "b200pt_active_pixels": [C.c_void_p, C.POINTER(C.c_uint32)],
+            "b200pt_set_track_variance": [C.c_void_p, C.c_int32], "b200pt_get_track_variance": [C.c_void_p, C.POINTER(C.c_int32)],
+            "b200pt_default_denoise": [C.POINTER(DenoiseParams)], "b200pt_denoise": [C.c_void_p, C.POINTER(DenoiseParams), C.POINTER(C.c_float)],
+            "b200pt_get_denoised": [C.c_void_p, C.c_void_p, C.c_int32],
+            "b200pt_get_denoise_inputs": [C.c_void_p, C.POINTER(DenoiseParams), C.c_void_p, C.c_void_p, C.c_void_p],
+            "b200pt_denoise_image": [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(DenoiseParams), C.c_void_p, C.c_int32],
+            "b200pt_post_process_denoised": [C.c_void_p],
         }
         for name, args in sig.items():
             fn = getattr(L, name); fn.restype = C.c_int32; fn.argtypes = args
@@ -505,6 +521,41 @@ class PathTracer:
 
     def active_pixels(self):
         n = C.c_uint32(); self._ck(self.L.b200pt_active_pixels(self.h, C.byref(n))); return n.value
+
+    # ---- per-pixel statistics and the denoiser
+    def set_track_variance(self, enable=True): self._ck(self.L.b200pt_set_track_variance(self.h, 1 if enable else 0))
+
+    def get_track_variance(self):
+        v = C.c_int32(); self._ck(self.L.b200pt_get_track_variance(self.h, C.byref(v))); return bool(v.value)
+
+    def denoise(self, params=None, **kw):
+        """b200pt_denoise (fields of b200pt_denoise_params; unnamed fields take the defaults); returns the device time in ms"""
+        p = params if params is not None else default_denoise(**kw)
+        ms = C.c_float(); self._ck(self.L.b200pt_denoise(self.h, C.byref(p), C.byref(ms))); return ms.value
+
+    def get_denoised(self, out=None):
+        w, h = self.size()
+        if out is None: out = np.empty((h, w, 4), np.float32)
+        self._ck(self.L.b200pt_get_denoised(self.h, _p(out), 0)); return out
+
+    def denoise_inputs(self, params=None, **kw):
+        """(albedo_cov [rows, W, 4], normal_depth [rows, W, 4], variance [rows, W]) of the local rows"""
+        p = params if params is not None else default_denoise(**kw)
+        w, _ = self.size(); rows = self.local_rows()
+        a = np.empty((rows, w, 4), np.float32); n = np.empty((rows, w, 4), np.float32); v = np.empty((rows, w), np.float32)
+        self._ck(self.L.b200pt_get_denoise_inputs(self.h, C.byref(p), _p(a), _p(n), _p(v))); return a, n, v
+
+    def denoise_image(self, color, albedo_cov, normal_depth, variance, params=None, **kw):
+        """the filter alone on [H, W, 4] / [H, W] arrays; returns the denoised [H, W, 4] float32 image"""
+        p = params if params is not None else default_denoise(**kw)
+        c, a, n = (np.ascontiguousarray(x, np.float32) for x in (color, albedo_cov, normal_depth))
+        v = np.ascontiguousarray(variance, np.float32)
+        h, w = c.shape[:2]
+        assert a.shape == n.shape == c.shape == (h, w, 4) and v.shape == (h, w)
+        out = np.empty((h, w, 4), np.float32)
+        self._ck(self.L.b200pt_denoise_image(self.h, w, h, _p(c), _p(a), _p(n), _p(v), C.byref(p), _p(out), 0)); return out
+
+    def post_process_denoised(self): self._ck(self.L.b200pt_post_process_denoised(self.h))
 
     def samples_accumulated(self):
         n = C.c_uint32(); self._ck(self.L.b200pt_samples_accumulated(self.h, C.byref(n))); return n.value

@@ -24,6 +24,7 @@ template <class F> static int32_t guard(b200pt_handle h, F &&f) {
 
 static_assert(sizeof(b200pt_volume) == 148 && sizeof(b200pt_density_grid) == 80, "b200pt_volume / b200pt_density_grid layout (binding.py, INTEGRATION.md)");
 static_assert(sizeof(b200pt_adaptive) == 16, "b200pt_adaptive layout (binding.py, checkpoint version 2)");
+static_assert(sizeof(b200pt_denoise_params) == 20, "b200pt_denoise_params layout (binding.py)");
 
 extern "C" {
 
@@ -190,6 +191,28 @@ int32_t b200pt_default_adaptive(b200pt_adaptive *a) {
 int32_t b200pt_set_adaptive(b200pt_handle h, const b200pt_adaptive *a) { if (!a) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_adaptive(*a); }); }
 int32_t b200pt_get_adaptive(b200pt_handle h, b200pt_adaptive *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.adaptive(); }); }
 int32_t b200pt_get_pixel_stats(b200pt_handle h, uint32_t *counts, float *rel_error) { return guard(h, [&](Engine &e) { e.pixel_stats(counts, rel_error); }); }
+int32_t b200pt_set_track_variance(b200pt_handle h, int32_t enable) { return guard(h, [&](Engine &e) { e.set_track_variance(enable != 0); }); }
+int32_t b200pt_get_track_variance(b200pt_handle h, int32_t *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.track_variance() ? 1 : 0; }); }
+int32_t b200pt_default_denoise(b200pt_denoise_params *p) {
+    if (!p) return B200PT_ERR_WRONG_ARGUMENTS;
+    p->Iterations = 5; p->FeatureSamples = 8; p->SigmaLuminance = 4.0f; p->SigmaNormal = 128.0f; p->SigmaDepth = 1.0f;
+    return B200PT_OK;
+}
+int32_t b200pt_denoise(b200pt_handle h, const b200pt_denoise_params *p, float *elapsed_ms) {
+    if (!p) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.denoise(*p, elapsed_ms); });
+}
+int32_t b200pt_get_denoised(b200pt_handle h, float *dst, int32_t dev) { if (!dst) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.get_denoised(dst, dev != 0); }); }
+int32_t b200pt_get_denoise_inputs(b200pt_handle h, const b200pt_denoise_params *p, float *albedo_cov, float *normal_depth, float *variance) {
+    if (!p) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.denoise_inputs(*p, albedo_cov, normal_depth, variance); });
+}
+int32_t b200pt_denoise_image(b200pt_handle h, uint32_t w, uint32_t ht, const float *color, const float *albedo_cov, const float *normal_depth,
+                             const float *variance, const b200pt_denoise_params *p, float *out, int32_t dev) {
+    if (!color || !albedo_cov || !normal_depth || !variance || !p || !out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.denoise_image(w, ht, color, albedo_cov, normal_depth, variance, *p, out, dev != 0); });
+}
+int32_t b200pt_post_process_denoised(b200pt_handle h) { return guard(h, [&](Engine &e) { e.post_process_denoised(); }); }
 int32_t b200pt_active_pixels(b200pt_handle h, uint32_t *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.active_pixels(); }); }
 int32_t b200pt_flush(b200pt_handle h) { return guard(h, [&](Engine &e) { e.flush(); }); }
 int32_t b200pt_samples_accumulated(b200pt_handle h, uint32_t *out) { if (!out) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { *out = e.samples_accumulated(); }); }

@@ -55,6 +55,8 @@ static void usage() {
         "  --atmosphere      render with the atmosphere (SetEnableAtmosphere(true): sun-disk NEE, Rayleigh / Mie / ozone scattering); --sun-color r g b\n"
         "  --adaptive T[,MIN[,INTERVAL]]  adaptive sampling: stop a pixel once the relative standard error of its mean luminance is <= T\n"
         "                    (checked every INTERVAL frames once it has MIN; defaults 64, 32); --spp stays the cap\n"
+        "  --denoise [ITER]  keep per-pixel statistics and write the PNG of the denoised image (ITER a-trous iterations, 0 .. 10, default 5);\n"
+        "                    --checkpoint still saves the raw accumulation\n"
         "  --checkpoint FILE save the accumulation when done         --resume FILE  continue from a checkpoint\n"
         "  --preview-every K rewrite the output PNG after every K PathTrace calls (the editor's progressive view, Editor.cpp:83-121)\n"
         "  --bake-luts N     bake missing lookup tables into DIR with N samples per texel first (Application.cpp:35-72)\n"
@@ -68,6 +70,7 @@ int main(int argc, char **argv) {
     b200pt_tonemap tm{ 1.0f, 2.2f }; b200pt_bloom bl{ 2.0f, 1.0f, 10, 5.0f };
     std::vector<b200pt_volume> vols;
     b200pt_adaptive adaptive; b200pt_default_adaptive(&adaptive);
+    b200pt_denoise_params dn; b200pt_default_denoise(&dn); bool denoise = false;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
         auto need = [&](int n) { if (i + n >= argc) { usage(); exit(2); } };
@@ -94,6 +97,14 @@ int main(int argc, char **argv) {
         else if (a == "--sun-color") { need(3); for (int k = 0; k < 3; k++) sun[k] = (float)atof(argv[++i]); }
         else if (a == "--preview-every") { need(1); preview = (uint32_t)atoi(argv[++i]); }
         else if (a == "--adaptive") { need(1); if (!parse_adaptive(argv[++i], adaptive)) { usage(); return 2; } }
+        else if (a == "--denoise") {                                        // optional ITER: the next argument when it is a number
+            denoise = true;
+            if (i + 1 < argc && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '9') {
+                char *end = nullptr; const long v = strtol(argv[++i], &end, 10);
+                if (*end != 0 || v < 0 || v > 10) { usage(); return 2; }
+                dn.Iterations = (uint32_t)v;
+            }
+        }
         else if (a == "--checkpoint") { need(1); ckpt_out = argv[++i]; } else if (a == "--resume") { need(1); ckpt_in = argv[++i]; }
         else if (a == "--bake-luts") { need(1); bake = (uint32_t)atoi(argv[++i]); } else if (a == "--device") { need(1); device = atoi(argv[++i]); }
         else if (a == "--quiet") quiet = true;
@@ -114,6 +125,7 @@ int main(int argc, char **argv) {
     if (sky) { cfg.SkyRotationAzimuth = sky_az; cfg.SkyRotationAltitude = sky_al; }
     CALL(b200pt_set_config(h, &cfg));
     if (adaptive.Enable) CALL(b200pt_set_adaptive(h, &adaptive));
+    if (denoise) CALL(b200pt_set_track_variance(h, 1));
     if (atmosphere) {
         b200pt_atmosphere atm; CALL(b200pt_get_atmosphere(h, &atm));
         atm.Enable = 1; for (int k = 0; k < 3; k++) atm.SunColor[k] = sun[k];
@@ -145,7 +157,8 @@ int main(int argc, char **argv) {
     }
     if (!quiet) fprintf(stderr, "\n");
     if (!ckpt_out.empty()) CALL(b200pt_save_checkpoint(h, ckpt_out.c_str()));
-    CALL(b200pt_post_process(h));
+    if (denoise) { CALL(b200pt_denoise(h, &dn, nullptr)); CALL(b200pt_post_process_denoised(h)); }
+    else CALL(b200pt_post_process(h));
     CALL(b200pt_save_png(h, out.c_str()));
     b200pt_counters c; CALL(b200pt_get_counters(h, &c));
     uint32_t active = 0; CALL(b200pt_active_pixels(h, &active));

@@ -49,7 +49,7 @@ Engine::~Engine() {
     cudaSetDevice(device_);
     for (auto &st : aux_stream_) if (st) cudaStreamSynchronize(st);
     if (stream_) cudaStreamSynchronize(stream_);
-    free_scene(); free_wave(); free_post(); free_adaptive();
+    free_scene(); free_wave(); free_post(); free_adaptive(); free_denoise(); dfree(d_dn_img_);
     if (h_active_count_) cudaFreeHost(h_active_count_);
     dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_); for (auto &l : d_luts_) dfree(l);
     dfree(d_image_); dfree(d_ctr_); dfree(d_volumes_); dfree(d_grids_); grids_.clear(); dfree(d_tri_class_);
@@ -423,6 +423,7 @@ void Engine::set_config(const b200pt_config &c) {
     if (c.SamplesPerFrame == 0 || c.ScreenChunkCount == 0 || c.ScreenChunkCount > 64) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "SamplesPerFrame and ScreenChunkCount must be >= 1" };
     if (c.ScreenChunkCount > 1 && world_ > 1) throw CudaError{ B200PT_ERR_NOT_IMPLEMENTED, "ScreenChunkCount > 1 cannot be combined with a multi-GPU partition" };
     if (c.ScreenChunkCount > 1 && adaptive_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "ScreenChunkCount > 1 cannot be combined with adaptive sampling" };
+    if (c.ScreenChunkCount > 1 && track_variance_) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "ScreenChunkCount > 1 cannot be combined with per-pixel statistics" };
     cfg_ = c;
     reset();
 }
@@ -436,7 +437,15 @@ void Engine::set_adaptive(const b200pt_adaptive &a) {
     sync_all();
     adaptive_ = a;
     adaptive_.Enable = a.Enable ? 1u : 0u;
-    if (!adaptive_.Enable) free_adaptive();
+    if (!records()) free_adaptive();
+    reset();
+}
+void Engine::set_track_variance(bool on) {
+    if (on && cfg_.ScreenChunkCount > 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "per-pixel statistics cannot be combined with ScreenChunkCount > 1" };
+    CK(cudaSetDevice(device_));
+    sync_all();
+    track_variance_ = on;
+    if (!records()) free_adaptive();
     reset();
 }
 void Engine::free_adaptive() {
@@ -475,7 +484,7 @@ uint32_t Engine::active_pixels() {
 void Engine::pixel_stats(uint32_t *counts, float *rel_error) {
     CK(cudaSetDevice(device_));
     const size_t npix = (size_t)W_ * local_rows_;
-    if (!adaptive_.Enable || !adaptive_ready_) {
+    if (!records() || !adaptive_ready_) {
         if (counts) std::fill(counts, counts + npix, frame_count_);
         if (rel_error) std::fill(rel_error, rel_error + npix, std::nanf(""));
         return;
@@ -576,11 +585,10 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "no environment map (PathTracer always loads one, PathTracer.cpp:202)" };
     if (!has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "no energy-compensation lookup tables (PathTracer.cpp:199-201)" };
     const uint32_t S = cfg_.ScreenChunkCount, S2 = S * S;
-    const bool adaptive = adaptive_.Enable != 0u;              // S == 1 (set_config / set_adaptive)
-    if (adaptive) {
-        prepare_adaptive();
-        if (active_count_ == 0) return true;                   // every local pixel has converged: nothing to launch, the dispatch counter stays
-    }
+    const bool adaptive = adaptive_.Enable != 0u;              // S == 1 (set_config / set_adaptive / set_track_variance)
+    const bool tracked = records();                           // statistics without adaptive sampling: the records over the identity list, no decisions
+    if (tracked) prepare_adaptive();
+    if (adaptive && active_count_ == 0) return true;          // every local pixel has converged: nothing to launch, the dispatch counter stays
     // how many dispatches until MaxSamplesAccumulated (PathTracer.cpp:124-125,151-153)
     uint32_t todo = 0;
     { uint64_t d = dispatch_count_; uint32_t acc = samples_accumulated_;
@@ -713,7 +721,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                 if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1], 0));
                 CK(cudaStreamWaitEvent(st, image_free_ev_, 0));
             }
-            if (adaptive) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_, B.sample_buf, d_image_, d_px_state_, st);
+            if (tracked) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_, B.sample_buf, d_image_, d_px_state_, st);
             else launch_resolve(lc_, dc, B.d_disp, nd, P, B.sample_buf, d_image_, st);
             CK(cudaEventRecord(resolved_ev_[ctx], st));
             wave_seq_++;
@@ -782,7 +790,7 @@ void Engine::set_hdr(const float *src, bool dev) {
 // The whole progressive state of the reference is the RGBA32F image + three counters (PT/PathTracer.h:199-201); frame f always uses
 // Seed_f = PCG(base_seed + dispatch index), so a render resumed from a checkpoint continues the SAME sample sequence: N frames in one go
 // and k frames + checkpoint + (N - k) frames give bit-identical images (tested).  File: 64-byte header + local rows of float4; version 2
-// (adaptive sampling on) appends the 16-byte b200pt_adaptive block and one 16-byte record per local pixel.
+// (adaptive sampling or per-pixel statistics on) appends the 16-byte b200pt_adaptive block and one 16-byte record per local pixel.
 namespace {
 struct CkptHeader { char magic[8]; uint32_t version, W, H, rank, world, band, local_rows, frame_count, samples_accumulated, samples_per_frame, chunk_count, _pad; uint64_t dispatch_count; };
 static_assert(sizeof(CkptHeader) == 64, "checkpoint header is 64 B");
@@ -792,8 +800,8 @@ void Engine::save_checkpoint(const char *path) {
     if (!d_image_ || !path) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no image to checkpoint" };
     std::vector<float> img((size_t)W_ * local_rows_ * 4);
     get_hdr(img.data(), false);
-    const bool adaptive = adaptive_.Enable != 0u;
-    std::vector<uint4> px;                                    // version 2 (adaptive sampling on): + the adaptive block + one 16-B record per local pixel
+    const bool adaptive = records();
+    std::vector<uint4> px;                                    // version 2 (adaptive sampling or statistics on): + the adaptive block + one 16-B record per local pixel
     if (adaptive) {
         prepare_adaptive();
         px.resize((size_t)W_ * local_rows_);
@@ -819,9 +827,9 @@ void Engine::load_checkpoint(const char *path) {
     const bool fits = ok && h.W == W_ && h.H == H_ && h.rank == rank_ && h.world == world_ && h.band == band_ && h.local_rows == local_rows_ &&
                       h.samples_per_frame == cfg_.SamplesPerFrame && h.chunk_count == cfg_.ScreenChunkCount;
     if (fits) { img.resize((size_t)W_ * local_rows_ * 4); ok = fread(img.data(), sizeof(float), img.size(), f) == img.size(); }
-    // version 2 (adaptive sampling): the adaptive block must equal this handle's; version 1 cannot resume an adaptive render
+    // version 2 (adaptive sampling or statistics): the adaptive block must equal this handle's; version 1 cannot resume a render with records
     b200pt_adaptive blk{}; std::vector<uint4> px;
-    bool same_mode = h.version == (adaptive_.Enable ? 2u : 1u);
+    bool same_mode = h.version == (records() ? 2u : 1u);
     if (fits && ok && same_mode && h.version == 2) {
         ok = fread(&blk, sizeof blk, 1, f) == 1;
         same_mode = ok && memcmp(&blk, &adaptive_, sizeof blk) == 0;
@@ -830,9 +838,9 @@ void Engine::load_checkpoint(const char *path) {
     fclose(f);
     if (!ok) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "not a b200pt checkpoint (bad magic / version / truncated)" };
     if (!fits) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "checkpoint was taken with another image size, partition, SamplesPerFrame or ScreenChunkCount" };
-    if (!same_mode) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "checkpoint was taken with other adaptive-sampling settings" };
+    if (!same_mode) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "checkpoint was taken with other adaptive-sampling or statistics settings" };
     set_hdr(img.data(), false);
-    if (adaptive_.Enable) {                                   // the records, then the active list rebuilt from their flags
+    if (records()) {                                   // the records, then the active list rebuilt from their flags
         reset(); prepare_adaptive();
         CK(cudaMemcpy(d_px_state_, px.data(), px.size() * sizeof(uint4), cudaMemcpyHostToDevice));
         update_active(false, stream_);
@@ -883,6 +891,10 @@ void Engine::post_process() { post_process_rows(0, H_); }
 void Engine::post_process_rows(uint32_t y0, uint32_t y1) {
     CK(cudaSetDevice(device_));
     if (!d_image_ || !W_ || !H_) throw CudaError{ B200PT_ERR_NO_SCENE, "PostProcess without an input image" };
+    post_chain(d_image_, y0, y1);
+    post_denoised_ = false;
+}
+void Engine::post_chain(const float4 *src, uint32_t y0, uint32_t y1) {
     if (world_ != 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process needs the full image: gather the bands first (world must be 1)" };
     if (y0 >= y1 || y1 > H_) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process_rows: bad row range" };
     ensure_post();
@@ -914,17 +926,17 @@ void Engine::post_process_rows(uint32_t y0, uint32_t y1) {
         auto rows_of = [&](const int r[2], int out[2]) { out[0] = r[0]; out[1] = r[1] + 1; };
         int r[2];
         rows_of(D[1], r);
-        launch_bloom_down_first(d_image_, W_, H_, d_mips_[1], mip_wh_[2], mip_wh_[3], p, stream_, whole ? nullptr : r);                               // :200-226, i == 0 and i == 1
+        launch_bloom_down_first(src, W_, H_, d_mips_[1], mip_wh_[2], mip_wh_[3], p, stream_, whole ? nullptr : r);                               // :200-226, i == 0 and i == 1
         for (uint32_t i = 2; i < mips; i++) { rows_of(D[i], r); launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_, whole ? nullptr : r); }
         for (uint32_t i = mips - 1; i > 1; i--) { rows_of(U[i - 1], r); launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_, whole ? nullptr : r); }   // :229-235
         r[0] = (int)y0; r[1] = (int)y1;
-        launch_bloom_final(d_image_, d_mips_[1], mip_wh_[2], mip_wh_[3], d_ldr_, (keep_bloom_ && whole) ? d_mips_[0] : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
+        launch_bloom_final(src, d_mips_[1], mip_wh_[2], mip_wh_[3], d_ldr_, (keep_bloom_ && whole) ? d_mips_[0] : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
         bloom_valid_ = keep_bloom_ && whole;
     } else {
-        launch_bloom_threshold(d_image_, d_mips_[0], W_ * H_, p, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);            // :200-226, i == 0
+        launch_bloom_threshold(src, d_mips_[0], W_ * H_, p, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);            // :200-226, i == 0
         for (uint32_t i = 1; i < mips; i++) launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_);
         for (uint32_t i = mips - 1; i > 0; i--) launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_);   // :229-235
-        launch_tonemap(d_image_, d_mips_[0], d_ldr_, W_, H_, p, stream_);                           // :238-245
+        launch_tonemap(src, d_mips_[0], d_ldr_, W_, H_, p, stream_);                           // :238-245
         bloom_valid_ = true;
     }
     CK(cudaGetLastError());
@@ -944,7 +956,10 @@ void Engine::get_ldr(uint8_t *dst, bool dev) {
 void Engine::get_bloom(float *dst) {
     CK(cudaSetDevice(device_));
     if (d_mips_.empty() || !dst) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process has not run" };
-    if (!bloom_valid_) { keep_bloom_ = true; post_process(); }              // the fused chain skips mip 0 until somebody asks for it
+    if (!bloom_valid_) {                                                     // the fused chain skips mip 0 until somebody asks for it: re-run it on the same input
+        keep_bloom_ = true;
+        if (post_denoised_ && has_denoised()) post_chain(d_dn_ + 2 * dn_pixels_, 0, H_); else post_process();
+    }
     CK(cudaMemcpyAsync(dst, d_mips_[0], (size_t)W_ * H_ * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
 }
@@ -1008,6 +1023,117 @@ void Engine::bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t 
     if (elapsed_ms) *elapsed_ms = ms;
     cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(d_part); cudaFree(d_tab);
     CK(e);
+}
+// ---------------------------------------------------------------- denoiser (denoise_kernels.cu, DESIGN.md section 12)
+static void check_denoise_params(const b200pt_denoise_params &p) {
+    if (p.Iterations > 10) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise Iterations must be <= 10" };
+    if (p.FeatureSamples == 0 || p.FeatureSamples > 256) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise FeatureSamples must be 1 .. 256" };
+    for (float v : { p.SigmaLuminance, p.SigmaNormal, p.SigmaDepth })
+        if (!std::isfinite(v) || v < 0.0f) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise sigmas must be finite and >= 0" };
+}
+static uint32_t pcg_host(uint32_t in) { const uint32_t st = in * 747796405u + 2891336453u; const uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; }
+void Engine::free_denoise() { dfree(d_dn_); dn_pixels_ = 0; dn_w_ = dn_h_ = 0; }   // (d_dn_img_ is sized by the caller's images: freed with the engine)
+void Engine::ensure_denoise() {
+    const size_t n = (size_t)W_ * local_rows_;
+    if (d_dn_ && n == dn_pixels_) return;
+    sync_all();
+    free_denoise();
+    CK(cudaMalloc(&d_dn_, std::max<size_t>(n, 1) * (6 * sizeof(float4) + sizeof(float))));
+    dn_pixels_ = n;
+}
+void Engine::run_features(const b200pt_denoise_params &p) {
+    if (!has_scene_ || !d_image_) throw CudaError{ B200PT_ERR_NO_SCENE, "denoise needs a scene and an image" };
+    if (!records()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise needs per-pixel statistics (b200pt_set_track_variance) or adaptive sampling" };
+    ensure_denoise();
+    prepare_adaptive();
+    join_waves();
+    const size_t n = dn_pixels_;
+    if (!n) return;
+    // forward: the view direction of the image centre (camera_ray with dx = dy = 0, no jitter), the axis of the view depth
+    const float *PI = proj_inv_, *VI = view_inv_;
+    double t[3] = { (double)PI[8] + PI[12], (double)PI[9] + PI[13], (double)PI[10] + PI[14] }, d[3];
+    const double tl = std::sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
+    for (int k = 0; k < 3; k++) d[k] = (VI[k] * t[0] + VI[4 + k] * t[1] + VI[8 + k] * t[2]) / tl;
+    const double dl = std::sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    const float3 fwd = make_float3((float)(d[0] / dl), (float)(d[1] / dl), (float)(d[2] / dl));
+    CK((cudaError_t)launch_features(lc_, ds_, make_dev_config(), fwd, p.FeatureSamples, pcg_host(0x46454154u), d_dn_, d_dn_ + n, stream_));
+    launch_record_variance(d_px_state_, (uint32_t)n, reinterpret_cast<float *>(d_dn_ + 6 * n), stream_);
+    CK(cudaGetLastError());
+}
+void Engine::denoise(const b200pt_denoise_params &p, float *elapsed_ms) {
+    CK(cudaSetDevice(device_));
+    check_denoise_params(p);
+    if (world_ != 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise needs the full image (world 1): gather b200pt_get_denoise_inputs and use b200pt_denoise_image" };
+    cudaEvent_t e[2] = { nullptr, nullptr };
+    CK(cudaEventCreate(&e[0])); CK(cudaEventCreate(&e[1]));
+    try {
+        join_waves();                                         // the timed window starts behind the render's waves
+        CK(cudaEventRecord(e[0], stream_));
+        run_features(p);
+        const size_t n = dn_pixels_;
+        launch_denoise_filter(W_, H_, d_image_, d_dn_, d_dn_ + n, reinterpret_cast<const float *>(d_dn_ + 6 * n), p.Iterations, p.SigmaLuminance, p.SigmaNormal,
+                              p.SigmaDepth, d_dn_ + 3 * n, d_dn_ + 2 * n, stream_);
+        CK(cudaEventRecord(e[1], stream_));
+        CK(cudaStreamSynchronize(stream_));
+        CK(cudaGetLastError());
+        float ms = 0.0f; CK(cudaEventElapsedTime(&ms, e[0], e[1]));
+        if (elapsed_ms) *elapsed_ms = ms;
+        dn_w_ = W_; dn_h_ = H_;
+    } catch (...) { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); throw; }
+    cudaEventDestroy(e[0]); cudaEventDestroy(e[1]);
+}
+void Engine::get_denoised(float *dst, bool dev) {
+    CK(cudaSetDevice(device_));
+    if (!dst || !has_denoised()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no denoised image of the current size (b200pt_denoise first)" };
+    CK(cudaMemcpyAsync(dst, d_dn_ + 2 * dn_pixels_, (size_t)W_ * H_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+}
+void Engine::denoise_inputs(const b200pt_denoise_params &p, float *albedo_cov, float *normal_depth, float *variance) {
+    CK(cudaSetDevice(device_));
+    check_denoise_params(p);
+    run_features(p);
+    const size_t n = dn_pixels_;
+    if (albedo_cov) CK(cudaMemcpyAsync(albedo_cov, d_dn_, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+    if (normal_depth) CK(cudaMemcpyAsync(normal_depth, d_dn_ + n, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+    if (variance) CK(cudaMemcpyAsync(variance, d_dn_ + 6 * n, n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+}
+void Engine::denoise_image(uint32_t w, uint32_t h, const float *color, const float *albedo_cov, const float *normal_depth, const float *variance,
+                           const b200pt_denoise_params &p, float *out, bool dev) {
+    CK(cudaSetDevice(device_));
+    check_denoise_params(p);
+    if (!w || !h || w > 65535 || h > 65535) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bad image size" };
+    const size_t n = (size_t)w * h, bytes = n * (dev ? 3 : 7) * sizeof(float4) + (dev ? 0 : n * sizeof(float));
+    if (bytes > dn_img_bytes_) {                              // kept for the next call: repeated calls allocate nothing
+        sync_all(); dfree(d_dn_img_); dn_img_bytes_ = 0;
+        CK(cudaMalloc(&d_dn_img_, bytes)); dn_img_bytes_ = bytes;
+    }
+    float4 *const buf = d_dn_img_;                            // [scratch 3n | device copies of the inputs and the output when they are host memory]
+    const float4 *c = reinterpret_cast<const float4 *>(color), *a = reinterpret_cast<const float4 *>(albedo_cov), *nd = reinterpret_cast<const float4 *>(normal_depth);
+    const float *v = variance; float4 *o = reinterpret_cast<float4 *>(out);
+    cudaError_t e = cudaSuccess;
+    if (!dev) {
+        float4 *hc = buf + 3 * n, *ha = buf + 4 * n, *hn = buf + 5 * n; float *hv = reinterpret_cast<float *>(buf + 7 * n);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hc, color, n * sizeof(float4), cudaMemcpyHostToDevice, stream_);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ha, albedo_cov, n * sizeof(float4), cudaMemcpyHostToDevice, stream_);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hn, normal_depth, n * sizeof(float4), cudaMemcpyHostToDevice, stream_);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hv, variance, n * sizeof(float), cudaMemcpyHostToDevice, stream_);
+        c = hc; a = ha; nd = hn; v = hv; o = buf + 6 * n;
+    }
+    if (e == cudaSuccess) {
+        launch_denoise_filter(w, h, c, a, nd, v, p.Iterations, p.SigmaLuminance, p.SigmaNormal, p.SigmaDepth, buf, o, stream_);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && !dev) e = cudaMemcpyAsync(out, o, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_);
+    const cudaError_t es = cudaStreamSynchronize(stream_);
+    CK(e); CK(es);
+}
+void Engine::post_process_denoised() {
+    CK(cudaSetDevice(device_));
+    if (!has_denoised()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no denoised image of the current size (b200pt_denoise first)" };
+    post_chain(d_dn_ + 2 * dn_pixels_, 0, H_);
+    post_denoised_ = true;
 }
 void Engine::scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const {
     if (tris) *tris = n_tris_; if (nodes) *nodes = bvh_.n_nodes; if (emissive) *emissive = n_emissive_; if (textures) *textures = (uint32_t)scene_.textures.size();

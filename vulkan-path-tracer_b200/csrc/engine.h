@@ -48,6 +48,17 @@ public:
     const b200pt_adaptive &adaptive() const { return adaptive_; }
     void pixel_stats(uint32_t *counts, float *rel_error);   // local pixels: frames accumulated, relative standard error of the mean luminance
     uint32_t active_pixels();                               // local pixels still traced
+    // per-pixel statistics without adaptive sampling: the same records, kept by k_resolve_adaptive over the identity list; any set resets the accumulation
+    void set_track_variance(bool on);
+    bool track_variance() const { return track_variance_; }
+
+    // denoiser (no reference equivalent, denoise_kernels.cu): feature pass + a-trous filter into a buffer of its own; the accumulation is not touched
+    void denoise(const b200pt_denoise_params &p, float *elapsed_ms);
+    void get_denoised(float *dst, bool dst_is_device);
+    void denoise_inputs(const b200pt_denoise_params &p, float *albedo_cov, float *normal_depth, float *variance);   // local rows, host memory
+    void denoise_image(uint32_t w, uint32_t h, const float *color, const float *albedo_cov, const float *normal_depth, const float *variance,
+                       const b200pt_denoise_params &p, float *out, bool is_device);
+    void post_process_denoised();                           // the post chain on the denoised image
 
     // PathTracer::PathTrace x dispatches; returns true when all samples are accumulated (or, adaptive, no local pixel is active)
     bool path_trace(uint32_t dispatches, uint32_t base_seed);
@@ -163,6 +174,19 @@ private:
     void prepare_adaptive();
     void free_adaptive();
     void update_active(bool decide, cudaStream_t st);   // decision / list rebuild on st, then A read back (blocks the host)
+    bool track_variance_ = false;                   // the records without adaptive sampling (set_track_variance)
+    bool records() const { return adaptive_.Enable != 0u || track_variance_; }
+
+    // denoiser: one allocation of W * local_rows pixels = [features 2n float4 | denoised n float4 | filter scratch 3n float4 | variance n float]
+    float4 *d_dn_ = nullptr; size_t dn_pixels_ = 0;
+    uint32_t dn_w_ = 0, dn_h_ = 0;                  // size of the image the denoised buffer holds (0: none)
+    float4 *d_dn_img_ = nullptr; size_t dn_img_bytes_ = 0;   // denoise_image: filter scratch (+ device copies of host arrays)
+    bool post_denoised_ = false;                    // the last post pass read the denoised image (get_bloom re-runs it on the same input)
+    void ensure_denoise();
+    void free_denoise();
+    bool has_denoised() const { return d_dn_ && dn_w_ == W_ && dn_h_ == H_; }
+    void run_features(const b200pt_denoise_params &p);   // features + variance of the local rows into d_dn_
+    void post_chain(const float4 *src, uint32_t y0, uint32_t y1);
 };
 
 } // namespace b200pt

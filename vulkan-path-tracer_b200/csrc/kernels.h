@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers of the sm_90a kernels (wavefront_kernels.cu, lbvh.cu, post_kernels.cu)
+// kernels.h -- host-callable launchers of the sm_90a kernels (wavefront_kernels.cu, lbvh.cu, post_kernels.cu, denoise_kernels.cu)
 #pragma once
 #include "device_types.h"
 #include <cuda_runtime.h>
@@ -44,6 +44,16 @@ void launch_resolve_adaptive(const LaunchCfg &lc, const DevConfig &cfg, uint32_t
 // active pixels into `active` and their count into *active_count (device).  tile_count: ceil(npix / ADAPTIVE_TILE) words of scratch.
 void launch_adaptive_update(uint4 *state, uint32_t npix, float threshold, uint32_t min_samples, bool decide, uint32_t *tile_count,
                             uint32_t *active, uint32_t *active_count, cudaStream_t st);
+// ---- denoiser (denoise_kernels.cu) ----
+constexpr float DN_UNKNOWN_VARIANCE = 1e30f;  // variance of a pixel with fewer than two frames
+// k_features over the local rows: albedo_cov = (mean albedo, hit fraction), normal_depth = (mean shading normal, mean view depth of the hits).
+// forward: unit view direction of the image centre; seed0 = PCG_HASH(0x46454154).  Returns cudaError_t as int.
+int launch_features(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, float3 forward, uint32_t samples, uint32_t seed0,
+                    float4 *albedo_cov, float4 *normal_depth, cudaStream_t st);
+void launch_record_variance(const uint4 *state, uint32_t npix, float *variance, cudaStream_t st);   // M2 / (n - 1) / n per record
+// the a-trous filter on a W x H image (device buffers); scratch: 3 * W * H float4.  iterations == 0 copies color to out.
+void launch_denoise_filter(uint32_t W, uint32_t H, const float4 *color, const float4 *albedo_cov, const float4 *normal_depth, const float *variance,
+                           uint32_t iterations, float sigma_l, float sigma_n, float sigma_z, float4 *scratch, float4 *out, cudaStream_t st);
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st);
 // k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.

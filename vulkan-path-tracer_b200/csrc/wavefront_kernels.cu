@@ -25,6 +25,7 @@
 // All per-path state is SoA float4 (coalesced 16-B lanes); live paths are kept dense by compaction.
 #include "bvh_traverse.cuh"
 #include "bvh_dynfetch.cuh"
+#include "camera.cuh"
 #include "atmosphere.cuh"
 #include "kernels.h"
 #include <cstdio>
@@ -33,23 +34,8 @@
 
 namespace b200pt {
 
-// ------------------------------------------------------------------------------------------------
-// partition helpers (rank r owns rows y with ((y / band) % world) == r)
-// ------------------------------------------------------------------------------------------------
-__host__ __device__ inline uint32_t part_global_row(uint32_t local_row, uint32_t rank, uint32_t world, uint32_t band) {
-    uint32_t blk = local_row / band, in = local_row % band;
-    return (blk * world + rank) * band + in;
-}
-
+// partition helper part_global_row, camera_eye and camera_ray: camera.cuh
 // control block (device memory, u32): device_types.h (CTRL_Q)
-
-// camera position before the depth-of-field offset (SH/RayGen.slang:41): the origin of every camera ray when DepthOfFieldStrength == 0
-__device__ __forceinline__ float3 camera_eye(const DevConfig &cfg) {
-    const float *VI = cfg.VI;
-    return f3(VI[0] * 0.0f + VI[4] * 0.0f + VI[8] * 0.0f + VI[12] * 1.0f,
-              VI[1] * 0.0f + VI[5] * 0.0f + VI[9] * 0.0f + VI[13] * 1.0f,
-              VI[2] * 0.0f + VI[6] * 0.0f + VI[10] * 0.0f + VI[14] * 1.0f);
-}
 
 // ------------------------------------------------------------------------------------------------
 // camera_path : camera sample + payload init of path j of a wave (k_raygen, k_camera); returns the camera ray
@@ -78,23 +64,8 @@ __device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispa
         Rng rng;
         if (first_sample) { rng.s = y + cfg.W * x + dd.Seed; sample_buf[j] = make_float4(0, 0, 0, 0); }   // :28 (Q13)
         else rng.s = rng_carry[j];
-        // :35-50
-        const float jx = rng.next() * (0.5f - -0.5f) + -0.5f;
-        const float jy = rng.next() * (0.5f - -0.5f) + -0.5f;
-        const float pcx = (float)x + 0.5f + jx, pcy = (float)y + 0.5f + jy;
-        const float dx = (pcx / (float)cfg.W) * 2.0f - 1.0f, dy = (pcy / (float)cfg.H) * 2.0f - 1.0f;
-        const float *VI = cfg.VI, *PI = cfg.PI;
-        float3 origin = camera_eye(cfg);
-        float3 target = f3(PI[0] * dx + PI[4] * dy + PI[8] * 1.0f + PI[12] * 1.0f,
-                           PI[1] * dx + PI[5] * dy + PI[9] * 1.0f + PI[13] * 1.0f,
-                           PI[2] * dx + PI[6] * dy + PI[10] * 1.0f + PI[14] * 1.0f);
-        float3 direction = mat4_dir(VI, normalize(target));
-        const float3 focus = origin + direction * fmaxf(cfg.FocusDistance, 0.001f);
-        const float u1 = rng.next(), u2 = rng.next();                       // RandomCircleVec, SH/Sampler.slang:103-112
-        const float theta = 2.0f * PT_PI * u1, rad = sqrtf(u2);
-        const float ox = (rad * cosf(theta)) * 0.5f * cfg.DepthOfFieldStrength, oy = (rad * sinf(theta)) * 0.5f * cfg.DepthOfFieldStrength;
-        origin = origin + (f3(VI[0], VI[1], VI[2]) * ox + f3(VI[4], VI[5], VI[6]) * oy);
-        direction = normalize(focus - origin);
+        float3 origin, direction;
+        camera_ray(cfg, x, y, rng, origin, direction);                      // :35-50
         // payload init :52-63.  Pixels outside the image (chunked dispatch overhang) are born dead (Depth = MAX).
         ps.org_pdf[j] = make_float4(origin.x, origin.y, origin.z, 1.0f);
         ps.dir_rng[j] = make_float4(direction.x, direction.y, direction.z, __uint_as_float(rng.s));
