@@ -649,6 +649,12 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     const uint32_t cmask = pre ? (class_mask_ | (1u << MC_GENERAL)) : class_mask_;   // volume / atmosphere events ride in the general queue
     const uint32_t qcap = (uint32_t)wave_cap_;
     const int qsel[2] = { 0, fuse == 2 ? 1 : 0 };
+    // Per-launch flags (kernels.h).  WAVE_IMPLIED: k_camera's paths are all inside the image only without chunked dispatch (overhang paths are
+    // born dead and keep their full state), and only the fused shading kernels infer the state.  WAVE_STORE: sub-wave 0 ends every path exactly once when the bounce loop provably runs dry -- not
+    // with a pre-pass (DEAD_EVENT ends, channel-split paths), not with medium walks (the runaway guard may stop them), not at MaxDepth 0 (no
+    // bounce runs, the slots must read zero).
+    const uint32_t implied_flag = (camera && S == 1 && fuse != 0) ? WAVE_IMPLIED : 0u;
+    const bool store_ok = !pre && !medium && cfg_.MaxDepth > 0;
 
     uint64_t launches = 0; uint32_t waves = 0, bounces_total = 0;
     std::vector<int> prof_kind; size_t prof_n = 0;            // kind: 0 raygen 1 extend 2 shade 3 connect 4 resolve
@@ -687,10 +693,12 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
             float4 *const hitb[2] = { B.so.hit, fuse == 2 ? B.so.bxdf_pdf : B.so.hit };
             for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
+                const uint32_t wflags = (s == 0 && store_ok ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
                 if (camera) {
                     const Queues q0{ B.q_miss[0], B.q_hit[0], qcap };
-                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, hitb[0], B.counts, q0, d_ctr_, st, act));
-                } else launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
+                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, hitb[0],
+                                                  B.counts, q0, d_ctr_, st, act));
+                } else launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
                 launches++; mark(0);
                 int cur = 0; uint32_t k = 0;
                 for (;;) {
@@ -698,13 +706,13 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     if (!medium && cfg_.MaxDepth - std::min(cfg_.MaxDepth, k) < chunk) chunk = cfg_.MaxDepth - std::min(cfg_.MaxDepth, k);
                     if (chunk == 0) break;
                     for (uint32_t b = 0; b < chunk; b++, k++) {
-                        const uint32_t par = k & 1u;
+                        const uint32_t par = k & 1u, bflags = wflags | (k == 0 ? implied_flag : 0u);
                         const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
                         if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
                         if ((fuse != 2 || k == 0) && !(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
                         launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
-                                                 fuse, cmask, st); mark(2);
-                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
+                                                 fuse, cmask, bflags, st); mark(2);
+                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty

@@ -26,14 +26,22 @@ struct LaunchCfg {
 };
 
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc);
+// ---- per-launch flags of the ray-generation and shading launchers (Engine::path_trace sets them per sub-wave and bounce) ----
+// WAVE_IMPLIED: k_camera ran with ScreenSplitCount == 1 in a fused pipeline, so every camera path is inside the image.  k_camera writes
+//               only dir_rng, the hit record and the queue entry; bounce 0's k_shade_miss and fused k_shade_hit take throughput, depth,
+//               radiance, slot and pdf from camera_implied_* instead of loading them (the origin is not read at depth 0 outside a medium).
+// WAVE_STORE:   first sub-wave of a call without pre-pass or medium walks: every path ends exactly once, in a slot nothing else writes, so
+//               a path end stores its radiance instead of adding it to the slot, and ray generation does not clear the slot.
+// WAVE_CARRY:   another sub-wave of the same frames follows: path ends store their RNG state to rng_carry for it.
+constexpr uint32_t WAVE_IMPLIED = 1u, WAVE_STORE = 2u, WAVE_CARRY = 4u;
 // active (adaptive sampling): P is the active count and wave entry i of a dispatch traces local pixel active[i]; nullptr = every pixel
-void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
+void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active = nullptr);
 // launch_raygen + the camera rays' launch_extend in one kernel (LaunchCfg::camera, no pre-pass): clears the control block on `st`, writes the
 // path state, the hit records (hit_out) and the parity-0 queues.  Returns cudaError_t as int.
 int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st,
-                  const uint32_t *active = nullptr);
+                  uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr,
+                  cudaStream_t st, const uint32_t *active = nullptr);
 // ---- adaptive sampling: per local pixel one 16-B record {meanL, M2 (float bits), n_p, flags} (Engine::d_px_state_) ----
 constexpr uint32_t ADAPTIVE_TILE = 2048;      // pixels per block of the two compaction passes
 constexpr uint32_t PX_CONVERGED = 1u;         // flags bit: the pixel is never traced again
@@ -60,11 +68,11 @@ void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4
 // fuse != 0: the bounce is finished inside k_shade_hit (dst, q_next, hit_out are written), launch_connect is not called.
 int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in, float4 *hit_out,
                  uint32_t *ctrl, uint32_t parity, Queues q, Queues q_next, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
-                 int fuse, uint32_t class_mask, cudaStream_t st);
+                 int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st);
 void launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
                           float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st);   // before launch_extend when the scene has volumes or the atmosphere is on (DevScene::pre_pass)
 void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
-                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, cudaStream_t st);
+                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st);
 void launch_resolve(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P,
                     const float4 *sample_buf, float4 *image, cudaStream_t st);
 void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const float *dir, const uint32_t *seeds, float ray_depth,

@@ -41,9 +41,18 @@ namespace b200pt {
 // camera_path : camera sample + payload init of path j of a wave (k_raygen, k_camera); returns the camera ray
 // ADAPTIVE: the wave holds P = A active pixels per dispatch, entry i of a dispatch traces local pixel active[i] (adaptive sampling).  Only the
 // pixel changes: the slot stays j, and the RNG is keyed on the pixel as always, so a pixel's frames are those of the plain renderer.
+// flags (kernels.h): WAVE_STORE skips the clear of the sample slot, WAVE_IMPLIED skips the stores of org_pdf, thr_depth and rad_slot (the
+// bounce-0 kernels infer them from the camera_implied_* helpers below, which are also what this function writes otherwise).
 // ------------------------------------------------------------------------------------------------
+constexpr float CAMERA_IMPLIED_PDF = 1.0f;                                  // payload.PDF of a camera path
+__device__ __forceinline__ float4 camera_implied_thr_depth(bool inside) {   // throughput 1, Depth 0 (born dead: MAX)
+    return make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(inside ? 0u : PT_MAX_DEPTH));
+}
+__device__ __forceinline__ float4 camera_implied_rad_slot(uint32_t j) {     // no radiance yet, sample slot j
+    return make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(j));
+}
 template <bool ADAPTIVE>
-__device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispatch *__restrict__ disp, uint32_t P, uint32_t first_sample,
+__device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispatch *__restrict__ disp, uint32_t P, uint32_t first_sample, uint32_t flags,
                                             const uint32_t *__restrict__ rng_carry, const PathState &ps, float4 *__restrict__ sample_buf,
                                             uint32_t j, float3 &ray_o, float3 &ray_d, const uint32_t *__restrict__ active) {
     const uint32_t S = cfg.ScreenSplitCount;
@@ -62,15 +71,19 @@ __device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispa
         }
         const bool inside = (x < cfg.W && y < cfg.H);                      // :24-25
         Rng rng;
-        if (first_sample) { rng.s = y + cfg.W * x + dd.Seed; sample_buf[j] = make_float4(0, 0, 0, 0); }   // :28 (Q13)
-        else rng.s = rng_carry[j];
+        if (first_sample) {                                                 // :28 (Q13)
+            rng.s = y + cfg.W * x + dd.Seed;
+            if (!(flags & WAVE_STORE)) sample_buf[j] = make_float4(0, 0, 0, 0);
+        } else rng.s = rng_carry[j];
         float3 origin, direction;
         camera_ray(cfg, x, y, rng, origin, direction);                      // :35-50
         // payload init :52-63.  Pixels outside the image (chunked dispatch overhang) are born dead (Depth = MAX).
-        ps.org_pdf[j] = make_float4(origin.x, origin.y, origin.z, 1.0f);
         ps.dir_rng[j] = make_float4(direction.x, direction.y, direction.z, __uint_as_float(rng.s));
-        ps.thr_depth[j] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(inside ? 0u : PT_MAX_DEPTH));
-        ps.rad_slot[j] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(j));
+        if (!(flags & WAVE_IMPLIED)) {
+            ps.org_pdf[j] = make_float4(origin.x, origin.y, origin.z, CAMERA_IMPLIED_PDF);
+            ps.thr_depth[j] = camera_implied_thr_depth(inside);
+            ps.rad_slot[j] = camera_implied_rad_slot(j);
+        }
         if (ps.vol_depth) ps.vol_depth[j] = 0u;                             // payload.VolumeDepth = 0 (SH/RayGen.slang:61)
         ray_o = origin; ray_d = direction;
     }
@@ -82,13 +95,13 @@ __device__ __forceinline__ void camera_path(const DevConfig &cfg, const DevDispa
 // ADAPTIVE: P = the active count, entry i traces pixel active[i] (camera_path); `active` is unused otherwise.
 template <bool ADAPTIVE>
 __global__ void __launch_bounds__(256) k_raygen(DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
-                                                 uint32_t first_sample, const uint32_t *__restrict__ rng_carry,
+                                                 uint32_t first_sample, uint32_t flags, const uint32_t *__restrict__ rng_carry,
                                                  PathState ps, float4 *__restrict__ sample_buf, uint32_t *__restrict__ ctrl,
                                                  WaveCounters *ctr, const uint32_t *__restrict__ active) {
     const uint32_t n = n_disp * P;
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
         float3 o, d;
-        camera_path<ADAPTIVE>(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, j, o, d, active);
+        camera_path<ADAPTIVE>(cfg, disp, P, first_sample, flags, rng_carry, ps, sample_buf, j, o, d, active);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { for (uint32_t w = 0; w < CTRL_WORDS; w++) ctrl[w] = 0; ctrl[0] = n; atomicAdd(&ctr->paths, (unsigned long long)n); }
 }
@@ -267,12 +280,13 @@ __global__ void __launch_bounds__(SMEM ? EXTEND_SMEM_MAX_THREADS : 512) k_extend
 //            it, but the ray is traced from registers instead of being read back: the closest-hit query of k_extend<true, true, .>
 //            (normalize_ray, exact slabs, tmin 0.01, tmax 1e5).  The hit record goes to hit_out, the path to the queues of parity 0.
 //            The control block is cleared on the stream before the launch (launch_camera): the appends of other CTAs may run before
-//            block 0 does.
+//            block 0 does.  With WAVE_IMPLIED and WAVE_STORE (the default pipeline) a path costs 36 B of stores: dir_rng, the hit record,
+//            the queue entry.
 // ------------------------------------------------------------------------------------------------
 // 64 registers: 4 CTAs of 256 threads per SM (big mode: 2 of 512).  ADAPTIVE: as k_raygen<true> (P = active count, `active_px` unused otherwise).
 template <bool UNIFORM, bool ADAPTIVE>
 __global__ void __launch_bounds__(512, 2) k_camera(DevScene sc, DevConfig cfg, const DevDispatch *__restrict__ disp, uint32_t n_disp, uint32_t P,
-                                                   uint32_t first_sample, const uint32_t *__restrict__ rng_carry, PathState ps,
+                                                   uint32_t first_sample, uint32_t flags, const uint32_t *__restrict__ rng_carry, PathState ps,
                                                    float4 *__restrict__ sample_buf, float4 *__restrict__ hit_out, uint32_t *__restrict__ ctrl,
                                                    Queues q, int max_stack, WaveCounters *ctr, const uint32_t *__restrict__ active_px) {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -310,7 +324,7 @@ __global__ void __launch_bounds__(512, 2) k_camera(DevScene sc, DevConfig cfg, c
             bool hit = false;
             uint32_t code = Q_NONE;
             float3 o = f3(0.0f), d = o;
-            if (active) camera_path<ADAPTIVE>(cfg, disp, P, first_sample, rng_carry, ps, sample_buf, i, o, d, active_px);
+            if (active) camera_path<ADAPTIVE>(cfg, disp, P, first_sample, flags, rng_carry, ps, sample_buf, i, o, d, active_px);
             bool at_eye = false;
             if (fixed) {
                 const float4 e = fixed_eye;
@@ -336,9 +350,21 @@ __device__ __forceinline__ void add_path_light(float4 &acc, float3 rad, int chan
     if (channel < 0) { acc.x += rad.x; acc.y += rad.y; acc.z += rad.z; }
     else if (channel == 0) acc.x += rad.x; else if (channel == 1) acc.y += rad.y; else acc.z += rad.z;
 }
+// A finished path (SH/RayGen.slang:116-128): its radiance is folded into its sample slot, its RNG state carried to the next sub-wave.
+// WAVE_STORE: the slot holds nothing yet (a cleared slot holds zeros), so the sum starts from zeros instead of a load -- the same bits.
+// Without WAVE_CARRY no later sub-wave reads rng_carry.
+__device__ __forceinline__ void finish_path_slot(uint32_t flags, uint32_t slot, float3 rad, int channel, uint32_t rng_state,
+                                                 float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
+    const bool ok = !isinf(rad.x) && !isinf(rad.y) && !isinf(rad.z) && !isnan(rad.x) && !isnan(rad.y) && !isnan(rad.z);   // :116
+    float4 acc = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    if (!(flags & WAVE_STORE)) acc = sample_buf[slot];
+    if (ok) add_path_light(acc, rad, channel);
+    sample_buf[slot] = acc;
+    if (flags & WAVE_CARRY) rng_carry[slot] = rng_state;
+}
 // SH/Miss.slang:8-76 + the ray-gen epilogue for a path whose segment missed (shared by k_shade_miss and the fused bounce kernel's tail)
 __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const DevConfig &cfg, float3 dir, uint32_t rng_state, float4 t4, float4 r4, float payPDF,
-                                                   float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
+                                                   uint32_t flags, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
     const uint32_t depth = __float_as_uint(t4.w) & DEPTH_MASK;
     const int channel = dflags_channel(__float_as_uint(t4.w));
     float4 c;
@@ -359,12 +385,7 @@ __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const Dev
     const float3 rad = f3(r4) + contribution;
     Rng rng; rng.s = rng_state;
     (void)rng.next();                                                       // the Russian-roulette draw of this segment (:111) still advances the stream
-    const uint32_t slot = __float_as_uint(r4.w);
-    const bool ok = !isinf(rad.x) && !isinf(rad.y) && !isinf(rad.z) && !isnan(rad.x) && !isnan(rad.y) && !isnan(rad.z);   // :116
-    float4 acc = sample_buf[slot];
-    if (ok) add_path_light(acc, rad, channel);
-    sample_buf[slot] = acc;
-    rng_carry[slot] = rng.s;
+    finish_path_slot(flags, __float_as_uint(r4.w), rad, channel, rng.s, sample_buf, rng_carry);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -373,14 +394,18 @@ __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const Dev
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_shade_miss(DevScene sc, DevConfig cfg, PathState ps, uint32_t *__restrict__ ctrl, uint32_t parity, uint32_t reset_next,
                                                      const uint32_t *__restrict__ q_miss, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry,
-                                                     WaveCounters *ctr) {
+                                                     WaveCounters *ctr, uint32_t flags) {
     const uint32_t n = ctrl[CTRL_Q + 8u * parity];
     // fused pipeline (k_bounce): this is the first kernel of the bounce, so it clears the counters the bounce kernels are about to fill
     if (reset_next && blockIdx.x == 0 && threadIdx.x == 0) ctrl_reset_parity(ctrl, parity ^ 1u);
+    const bool implied = (flags & WAVE_IMPLIED) != 0u;
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
         const uint32_t i = q_miss[j];
-        const float4 d4 = ps.dir_rng[i], t4 = ps.thr_depth[i], r4 = ps.rad_slot[i];
-        finish_missed_path(sc, cfg, f3(d4), __float_as_uint(d4.w), t4, r4, ps.org_pdf[i].w, sample_buf, rng_carry);
+        const float4 d4 = ps.dir_rng[i];
+        float4 t4, r4; float pdf;
+        if (implied) { t4 = camera_implied_thr_depth(true); r4 = camera_implied_rad_slot(i); pdf = CAMERA_IMPLIED_PDF; }
+        else { t4 = ps.thr_depth[i]; r4 = ps.rad_slot[i]; pdf = ps.org_pdf[i].w; }
+        finish_missed_path(sc, cfg, f3(d4), __float_as_uint(d4.w), t4, r4, pdf, flags, sample_buf, rng_carry);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&ctr->misses, (unsigned long long)n); atomicAdd(&ctr->shade_invocations, (unsigned long long)n); }
 }
@@ -405,7 +430,7 @@ __device__ __forceinline__ bool path_roulette(const DevConfig &cfg, float4 b4, u
     return alive && (newDepth < cfg.MaxDepth);                              // loop condition :66
 }
 __device__ __forceinline__ float3 path_radiance(const DevConfig &cfg, float3 emitted, uint32_t newDepth, int channel, float4 thr4, float4 r4, bool alive, uint32_t rng_state,
-                                                float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
+                                                uint32_t flags, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
     float3 contribution = mul_rn(emitted, f3(thr4));
     if (newDepth != 1u) {                                                   // Q3: dot(contribution, luminance weights)
         const float lum = __fmaf_rn(contribution.z, 0.072169f, __fmaf_rn(contribution.x, 0.212671f, __fmul_rn(contribution.y, 0.715160f)));
@@ -413,14 +438,7 @@ __device__ __forceinline__ float3 path_radiance(const DevConfig &cfg, float3 emi
         contribution = mul_rn(contribution, f3(scale));
     }
     const float3 rad = add_rn(f3(r4), contribution);
-    if (!alive) {                                                           // path finished: :116-128 (+ carry RNG for SampleCount > 1)
-        const uint32_t slot = __float_as_uint(r4.w);
-        const bool ok = !isinf(rad.x) && !isinf(rad.y) && !isinf(rad.z) && !isnan(rad.x) && !isnan(rad.y) && !isnan(rad.z);
-        float4 acc = sample_buf[slot];
-        if (ok) add_path_light(acc, rad, channel);
-        sample_buf[slot] = acc;
-        rng_carry[slot] = rng_state;
-    }
+    if (!alive) finish_path_slot(flags, __float_as_uint(r4.w), rad, channel, rng_state, sample_buf, rng_carry);   // path finished: :116-128
     return rad;
 }
 
@@ -457,8 +475,12 @@ template <uint32_t CLASS, bool VOL, int FUSE, bool BIG = false>   // VOL: the sc
 __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_BLOCKS : SHADE_MIN_BLOCKS)) k_shade_hit(DevScene sc, DevConfig cfg, PathState ps, PathState dst, ShadeOut so,
                                                     const float4 *__restrict__ hit_in, float4 *__restrict__ hit_out,
                                                     uint32_t *__restrict__ ctrl, uint32_t parity, Queues q, Queues q_next,
-                                                    float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry, int max_stack, WaveCounters *ctr) {
+                                                    float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry, int max_stack, WaveCounters *ctr,
+                                                    uint32_t flags) {
     constexpr uint32_t LOBES = class_lobes(CLASS);
+    // bounce 0 behind k_camera: only dir_rng of the path state was written.  Fused forms only: inferring the state in the unfused form (held to
+    // 96 registers, already spilling) costs it spill traffic, so the engine does not set WAVE_IMPLIED for the unfused pipeline.
+    const bool implied = FUSE && (flags & WAVE_IMPLIED) != 0u;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     __shared__ uint32_t list_count[FUSE == 2 ? (BIG ? 16 : 4) : 1];           // entries in each warp's ray list
@@ -501,13 +523,15 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
         const uint32_t i = i_nx;
         if (valid) do {
             const float4 h4 = h4_nx;
-            const float4 o4 = ps.org_pdf[i], d4 = ps.dir_rng[i];
-            const uint32_t dflags = __float_as_uint(ps.thr_depth[i].w);
+            // implied: the origin is never read at Depth 0 outside a medium (the medium branch and the emission MIS need Depth != 0)
+            const float4 o4 = implied ? make_float4(0.0f, 0.0f, 0.0f, CAMERA_IMPLIED_PDF) : ps.org_pdf[i], d4 = ps.dir_rng[i];
+            const uint32_t dflags = implied ? __float_as_uint(camera_implied_thr_depth(true).w) : __float_as_uint(ps.thr_depth[i].w);
             if (j + jstep < n) {
                 i_nx = q_hit[j + jstep]; h4_nx = hit_in[i_nx];
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.org_pdf + i_nx));
+                if (!implied) asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.org_pdf + i_nx));
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.dir_rng + i_nx));
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.thr_depth + i_nx));
+                if (!implied) asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.thr_depth + i_nx));
+                if (FUSE && !implied) asm volatile("prefetch.global.L2 [%0];" ::"l"(ps.rad_slot + i_nx));   // read by the path epilogue
             }
             const uint32_t depth = dflags & DEPTH_MASK;
             const uint32_t chanBits = dflags & CHANNEL_MASK;           // colour channel of a path split by an atmosphere event (0 = unsplit)
@@ -705,7 +729,8 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
             bool alive = false;
             float4 thr4 = zero4, r4 = zero4; float3 thr = f3(0.0f), rad = f3(0.0f);
             if (shaded) {
-                thr4 = ps.thr_depth[i]; r4 = ps.rad_slot[i];
+                if (implied) { thr4 = camera_implied_thr_depth(true); r4 = camera_implied_rad_slot(i); }
+                else { thr4 = ps.thr_depth[i]; r4 = ps.rad_slot[i]; }
                 alive = path_roulette(cfg, b4, newDflags & DEPTH_MASK, thr4, rng, thr);
             }
             uint32_t code = Q_NONE; float4 h4 = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0xFFFFFFFFu));
@@ -740,7 +765,7 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                     code = __float_as_uint(h4.w) != 0xFFFFFFFFu ? hit_code(sc, __float_as_uint(h4.w)) : 0u;
                 }
             }
-            if (shaded) rad = path_radiance(cfg, emitted, newDflags & DEPTH_MASK, dflags_channel(newDflags), thr4, r4, alive, rng.s, sample_buf, rng_carry);
+            if (shaded) rad = path_radiance(cfg, emitted, newDflags & DEPTH_MASK, dflags_channel(newDflags), thr4, r4, alive, rng.s, flags, sample_buf, rng_carry);
             const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alive);
             if (ballot) {
                 uint32_t base = 0;
@@ -783,7 +808,7 @@ template <bool SMEM, bool TRACE, bool WALKS = false>   // TRACE = false: k_shado
 __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, PathState src, PathState dst, ShadeOut so,
                                                   uint32_t *__restrict__ ctrl, uint32_t parity, Queues q,
                                                   float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry,
-                                                  int max_stack, WaveCounters *ctr) {
+                                                  int max_stack, WaveCounters *ctr, uint32_t flags) {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
@@ -877,7 +902,7 @@ __global__ void __launch_bounds__(512) k_connect(DevScene sc, DevConfig cfg, Pat
             if (!walks) { o4 = src.org_pdf[i]; d4 = src.dir_rng[i]; rng.s = __float_as_uint(d4.w); }
             const float4 b4 = so.bxdf_pdf[i];
             alive = path_roulette(cfg, b4, newDepth, thr4, rng, thr);
-            rad = path_radiance(cfg, emitted, newDepth, channel, thr4, r4, alive, rng.s, sample_buf, rng_carry);
+            rad = path_radiance(cfg, emitted, newDepth, channel, thr4, r4, alive, rng.s, flags, sample_buf, rng_carry);
         }
         // ---- warp ballot + prefix-sum compaction of the live paths
         const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alive);
@@ -1565,19 +1590,19 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     return 0;
 }
 
-void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
+void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
                    const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active) {
-    if (active) k_raygen<true><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr, active);
-    else k_raygen<false><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, ctrl, ctr, nullptr);
+    if (active) k_raygen<true><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, ctrl, ctr, active);
+    else k_raygen<false><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, ctrl, ctr, nullptr);
 }
 int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr, cudaStream_t st,
-                  const uint32_t *active) {
+                  uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr,
+                  cudaStream_t st, const uint32_t *active) {
     set_attrs_for_current_device();
     const cudaError_t e = cudaMemsetAsync(ctrl, 0, CTRL_WORDS * sizeof(uint32_t), st);   // before any CTA appends to the parity-0 queues
     if (e != cudaSuccess) return (int)e;
     const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, true);
-#define B200PT_CAM(U, A) k_camera<U, A><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr, active)
+#define B200PT_CAM(U, A) k_camera<U, A><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr, active)
     if (sc.uniform_class != 0xFFu) { if (active) B200PT_CAM(true, true); else B200PT_CAM(true, false); }
     else { if (active) B200PT_CAM(false, true); else B200PT_CAM(false, false); }
 #undef B200PT_CAM
@@ -1620,17 +1645,17 @@ void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4
 // Returns the number of kernels launched.
 int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in, float4 *hit_out,
                  uint32_t *ctrl, uint32_t parity, Queues q, Queues q_next, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
-                 int fuse, uint32_t class_mask, cudaStream_t st) {
+                 int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st) {
     set_attrs_for_current_device();
     int launched = 1;
-    k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, fuse == 2 ? 1u : 0u, q.miss, sample_buf, rng_carry, ctr);
+    k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, fuse == 2 ? 1u : 0u, q.miss, sample_buf, rng_carry, ctr, flags);
     const size_t shb = fuse == 2 ? bounce_smem_bytes(sc, lc.max_stack, lc.big ? 512 : 128) : trace_smem_bytes(sc, lc.max_stack, 128, true);
 #define B200PT_SHADE(C) do { if (class_mask & (1u << C)) { launched++;                                                                                              \
-        if (fuse == 2 && lc.big) k_shade_hit<C, false, 2, true><<<lc.grid_bounce, 512, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr); \
-        else if (fuse == 2) k_shade_hit<C, false, 2><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr);      \
-        else if (fuse == 1) k_shade_hit<C, false, 1><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr); \
-        else if (sc.pre_pass) k_shade_hit<C, true, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr);   \
-        else k_shade_hit<C, false, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr); } } while (0)
+        if (fuse == 2 && lc.big) k_shade_hit<C, false, 2, true><<<lc.grid_bounce, 512, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
+        else if (fuse == 2) k_shade_hit<C, false, 2><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags);      \
+        else if (fuse == 1) k_shade_hit<C, false, 1><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
+        else if (sc.pre_pass) k_shade_hit<C, true, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags);   \
+        else k_shade_hit<C, false, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); } } while (0)
     B200PT_SHADE(MC_DIFFUSE); B200PT_SHADE(MC_METAL); B200PT_SHADE(MC_GLASS); B200PT_SHADE(MC_GENERAL);
 #undef B200PT_SHADE
     if (sc.pre_pass) { launched++; k_shade_volume<<<lc.grid_light, 128, 0, st>>>(sc, cfg, ps, so, ctrl, parity, q, ctr); }
@@ -1645,7 +1670,7 @@ void launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConf
     else k_volume_decide<false><<<lc.grid_trace, 256, sh, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
 }
 void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
-                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, cudaStream_t st) {
+                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st) {
     set_attrs_for_current_device();
     const bool smem = lc.bvh_in_smem;
     const bool walks = cfg.EnableAtmosphere != 0u || sc.n_grids != 0u;      // k_connect<.., WALKS>
@@ -1654,12 +1679,12 @@ void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cf
 #define B200PT_SH_DYN(S, W) k_shadow_dyn<S, W><<<lc.grid_shadow, 256, shd, st>>>(sc, so, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr)
         if (lc.wide) B200PT_SH_DYN(false, true); else if (smem) B200PT_SH_DYN(true, false); else B200PT_SH_DYN(false, false);
 #undef B200PT_SH_DYN
-        if (walks) k_connect<false, false, true><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr);
-        else k_connect<false, false><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr);
+        if (walks) k_connect<false, false, true><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
+        else k_connect<false, false><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
         return;
     }
     const size_t sh = trace_smem_bytes(sc, lc.max_stack, smem ? lc.extend_threads : 256, smem);
-#define B200PT_CONNECT(S, W, T) k_connect<S, true, W><<<lc.grid_connect, T, sh, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr)
+#define B200PT_CONNECT(S, W, T) k_connect<S, true, W><<<lc.grid_connect, T, sh, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags)
     if (smem) { if (walks) B200PT_CONNECT(true, true, lc.extend_threads); else B200PT_CONNECT(true, false, lc.extend_threads); }
     else { if (walks) B200PT_CONNECT(false, true, 256); else B200PT_CONNECT(false, false, 256); }
 #undef B200PT_CONNECT
