@@ -15,10 +15,10 @@ def run(name, W, H, frames, depth, **kw):
     T.post_process_rows(8, min(H, 24)); T.get_ldr_rows(8, min(H, 24))
     print(name, kw.get("Volumes") is not None, os.environ.get("B200PT_FUSE"), os.environ.get("B200PT_TRAV"), "ok", float(img[..., :3].mean()))
 
-run("cornell_box", 64, 36, 2, 6)                                   # BVH in shared memory (TMA), flat traversal, uniform class, k_camera, k_shade_hit<., ., 1> + k_extend
+run("cornell_box", 64, 36, 2, 6)                                   # BVH in shared memory (TMA), flat traversal, uniform class, k_camera, k_shade_hit<., ., true> + k_extend
 os.environ["B200PT_FLAT_MAX"] = "0"; run("cornell_box", 48, 32, 1, 4); del os.environ["B200PT_FLAT_MAX"]      # BVH2 stack traversal in shared memory (k_camera too)
-os.environ["B200PT_FUSE"] = "2"; os.environ["B200PT_CAMERA"] = "0"; run("cornell_box", 48, 32, 2, 6)         # k_raygen + k_extend, bounce kernel k_shade_hit<., ., 2>
-del os.environ["B200PT_FUSE"]; del os.environ["B200PT_CAMERA"]
+os.environ["B200PT_CAMERA"] = "0"; run("cornell_box", 48, 32, 2, 6); del os.environ["B200PT_CAMERA"]          # k_raygen + k_extend<., true, .>
+os.environ["B200PT_SMEM_BIG"] = "1"; run("cornell_box_glass", 48, 48, 2, 8); del os.environ["B200PT_SMEM_BIG"]  # big mode: 512-thread k_camera, k_extend, fused k_shade_hit
 run("cornell_box", 48, 32, 1, 5, Volumes=[FOG])                     # k_volume_decide / k_shade_volume
 run("cornell_box", 48, 32, 2, 5, EnableAtmosphere=1, SkyRotationAltitude=-30.0)                       # atmosphere: sun NEE, delta tracking, transmittance walks
 run("cornell_box", 40, 30, 1, 5, EnableAtmosphere=1, SkyRotationAltitude=-20.0, Volumes=[FOG])        # atmosphere + homogeneous volume

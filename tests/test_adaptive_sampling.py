@@ -112,6 +112,7 @@ def test_stopped_pixels_equal_the_plain_render_bit_for_bit(gpu_pt, name):
     assert T.counters()["paths"] == int(counts.sum()) * spf
 
 
+# fuse2: B200PT_FUSE=2 selected the bounce kernel, which is gone; an unsupported value must keep the default pipeline
 ENV_VARIANTS = [("fif1", {}, dict(FramesInFlight=1)), ("overlap0", {"B200PT_OVERLAP": "0"}, {}),
                 ("fuse0", {"B200PT_FUSE": "0"}, {}), ("fuse1", {"B200PT_FUSE": "1"}, {}), ("fuse2", {"B200PT_FUSE": "2"}, {}),
                 ("camera0", {"B200PT_CAMERA": "0"}, {}), ("split", {}, {})]

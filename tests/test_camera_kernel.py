@@ -50,18 +50,28 @@ def _check(monkeypatch, W=96, H=70, frames=4, samples=1, **kw):
     assert np.array_equal(img1.view(np.uint32), img0.view(np.uint32)), int((img1 != img0).any(axis=-1).sum())
     assert {k: c1[k] for k in WORK} == {k: c0[k] for k in WORK}
     assert c0["kernel_launches"] - c1["kernel_launches"] == waves * samples      # k_camera ran: one launch instead of two per wave and sample
+    return img1, c1
+
+
+def _check_fuse(monkeypatch, fuse, **kw):
+    """_check under B200PT_FUSE=fuse.  2 selected the bounce kernel, which is gone: an unsupported value must run the default pipeline, so
+    its image and every counter (kernel_launches included) must equal those of a render without the variable."""
+    monkeypatch.setenv("B200PT_FUSE", fuse)
+    img, c = _check(monkeypatch, **kw)
+    if fuse == "2":
+        monkeypatch.delenv("B200PT_FUSE")
+        img_d, c_d = _check(monkeypatch, **kw)
+        assert np.array_equal(img.view(np.uint32), img_d.view(np.uint32)) and c == c_d, (c, c_d)
 
 
 @pytest.mark.parametrize("fuse", ["0", "1", "2"])
 def test_camera_kernel_matches_raygen_extend_per_pipeline(pt, fuse, monkeypatch):
-    monkeypatch.setenv("B200PT_FUSE", fuse)
-    _check(monkeypatch, depth=8)
+    _check_fuse(monkeypatch, fuse, depth=8)
 
 
 @pytest.mark.parametrize("fuse", ["1", "2"])
 def test_camera_kernel_matches_with_four_material_classes(pt, fuse, monkeypatch):
-    monkeypatch.setenv("B200PT_FUSE", fuse)
-    _check(monkeypatch, W=128, H=96, depth=8, edit=_four_classes)
+    _check_fuse(monkeypatch, fuse, W=128, H=96, depth=8, edit=_four_classes)
 
 
 def test_camera_kernel_matches_with_screen_chunks(pt, monkeypatch):

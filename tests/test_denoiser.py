@@ -327,6 +327,7 @@ def test_the_filter_backs_off_as_the_render_converges(gpu_pt):
 
 # ---------------------------------------------------------------- 7. invariance
 
+# fuse2: B200PT_FUSE=2 selected the bounce kernel, which is gone; an unsupported value must keep the default pipeline
 VARIANTS = [("fif1", {}, dict(FramesInFlight=1)), ("fuse0", {"B200PT_FUSE": "0"}, {}), ("fuse2", {"B200PT_FUSE": "2"}, {}),
             ("camera0", {"B200PT_CAMERA": "0"}, {}), ("split", {}, {})]
 _BASE = {}

@@ -701,18 +701,18 @@ def _mixed_materials_edit(T):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,depth", [("cornell_box", 8), ("cornell_box_glass", 12)])
 def test_fused_bounce_kernel_and_class_queues_return_the_same_image(pt, name, depth, monkeypatch):
-    """The material-class hit queues (k_extend sorts hits by lobe set, k_shade_hit<CLASS> compiles the dead lobes out) and the fused bounce
-    kernel of shared-memory scenes (k_shade_hit<CLASS, ., FUSE>: NEE shadow queries, path epilogue and the next TraceRay in one kernel) are
+    """The material-class hit queues (k_extend sorts hits by lobe set, k_shade_hit<CLASS> compiles the dead lobes out) and the fused shading
+    kernel of shared-memory scenes (k_shade_hit<CLASS, ., true>: NEE shadow queries and the path epilogue inside the shading kernel) are
     re-arrangements of the same estimator: same random numbers per path, same closest hits, same sums.  B200PT_FUSE=0 is the round-1
     pipeline (k_shade_hit + k_connect), B200PT_CLASSES=0 sends every hit through the general (all-lobes) kernel.  A lobe whose probability is
     exactly 0 only ever adds exact zeros, so images agree bit for bit except where the compiler contracts an a*b+c differently in two
     instantiations (a last-bit difference that a path may amplify across a branch; measured 98.6 % identical pixels on the four-class Cornell
     box after 4 frames, 94.4 % with a relative L2 of 1e-9 on the glass scene in big shared-memory mode): >= 90 % of the pixels identical,
-    rel. L2 < 1e-3.  The fused kernels and the big mode are opt-in (measured slower, DESIGN.md)."""
+    rel. L2 < 1e-3.  The glass scene runs in big mode (opt-in, B200PT_SMEM_BIG=1), so the 512-thread fused kernel is compared as well."""
     if name == "cornell_box_glass": monkeypatch.setenv("B200PT_SMEM_BIG", "1")
     W, H, frames = 192, 128, 4
     out = {}
-    for fuse in ("2", "1", "0"):
+    for fuse in ("1", "0"):
         for classes in ("1", "0"):
             monkeypatch.setenv("B200PT_FUSE", fuse); monkeypatch.setenv("B200PT_CLASSES", classes)
             T = util.product_tracer(name, W, H, MaxDepth=depth)

@@ -1,7 +1,7 @@
 """Sample slots are reused across calls without being cleared where every path of a sub-wave is known to end exactly once (WAVE_STORE:
 the path end stores its radiance instead of adding it to the slot).  A handle whose slots still hold another seed's radiance must render
 exactly what a fresh handle renders: the same image bit for bit and the same work.  The cases cover every pipeline that reaches a path end:
-the three bounce pipelines with and without k_camera, a second sample per frame (the slot is accumulated, the RNG state carried), chunked
+the two bounce pipelines (and an unsupported B200PT_FUSE value, which must run the default one) with and without k_camera, a second sample per frame (the slot is accumulated, the RNG state carried), chunked
 dispatch (overhang paths keep their full camera state), a BVH outside shared memory (k_raygen + the dynamic-fetch kernels), a medium
 (the bounce loop can stop on its runaway guard, so the slots are cleared as before) and a volume (pre-pass pipeline, cleared as before).
 """
@@ -64,12 +64,23 @@ def _check(monkeypatch, env=None, scene="cornell_box", W=64, H=48, frames=3, dep
     assert np.isfinite(img_fresh).all() and img_fresh[..., :3].max() > 0
     assert np.array_equal(img_used.view(np.uint32), img_fresh.view(np.uint32)), int((img_used != img_fresh).any(axis=-1).sum())
     assert c_used == c_fresh
+    return img_fresh, c_fresh
+
+
+def _check_fuse(monkeypatch, fuse, env=None, **kw):
+    """_check under B200PT_FUSE=fuse.  2 selected the bounce kernel, which is gone: an unsupported value must run the default pipeline, so
+    its image and every counter (kernel_launches included) must equal those of a render without the variable."""
+    img, c = _check(monkeypatch, dict(env or {}, B200PT_FUSE=fuse), **kw)
+    if fuse == "2":
+        monkeypatch.delenv("B200PT_FUSE")
+        img_d, c_d = _check(monkeypatch, env, **kw)
+        assert np.array_equal(img.view(np.uint32), img_d.view(np.uint32)) and c == c_d, (c, c_d)
 
 
 @pytest.mark.parametrize("camera", ["0", "1"])
 @pytest.mark.parametrize("fuse", ["0", "1", "2"])
 def test_reused_slots_match_a_fresh_handle_per_pipeline(pt, fuse, camera, monkeypatch):
-    _check(monkeypatch, {"B200PT_FUSE": fuse, "B200PT_CAMERA": camera}, depth=8)
+    _check_fuse(monkeypatch, fuse, {"B200PT_CAMERA": camera}, depth=8)
 
 
 @pytest.mark.parametrize("camera", ["0", "1"])
@@ -89,7 +100,7 @@ def test_reused_slots_match_with_bvh_outside_shared_memory(pt, monkeypatch):
 
 @pytest.mark.parametrize("fuse", ["1", "2"])
 def test_reused_slots_match_with_a_medium(pt, fuse, monkeypatch):
-    _check(monkeypatch, {"B200PT_FUSE": fuse}, W=96, H=64, depth=8, edit=_four_classes)
+    _check_fuse(monkeypatch, fuse, W=96, H=64, depth=8, edit=_four_classes)
 
 
 def test_reused_slots_match_with_a_volume(pt, monkeypatch):

@@ -122,17 +122,13 @@ __device__ __forceinline__ bool tri_test(float3 v0, float3 e1, float3 e2, float3
 // on scene surfaces.  Camera rays (origin anywhere) and the test hook use the subtract-then-multiply form (FMA_SLABS = false).
 // TARGET (with ANYHIT): "is anything in front of triangle target_gid, which the ray hits at tmax?"  A triangle occludes when
 // t < tmax, or t == tmax and its id is lower than the target's (the tie rule of the closest-hit query); the target itself never does.
-// MIXED: the query kind is chosen per ray at run time (one inlined copy of the loop serves a list of rays of all kinds, k_shade_hit<.., 2>):
-// shadow = true is the TARGET any-hit query, shadow = false the closest-hit query.  Triangles are tested branch-free (same roundings as the
-// early-out form, see tri_test).
-template <bool SMEM, bool ANYHIT, bool COUNT = false, bool TARGET = false, bool FMA_SLABS = false, bool MIXED = false>
+template <bool SMEM, bool ANYHIT, bool COUNT = false, bool TARGET = false, bool FMA_SLABS = false>
 __device__ __forceinline__ bool bvh_trace(const BvhView &b, float3 o, float3 d, float tmin, float tmax, HitRec &h,
                                           int *stack, int stride, int max_stack, uint32_t *n_nodes = nullptr, uint32_t *n_tris = nullptr,
-                                          uint32_t target_gid = 0xFFFFFFFFu, float tmax_test_in = -1.0f, bool shadow = false) {
-    const bool any = MIXED ? shadow : ANYHIT, tgt = MIXED ? shadow : TARGET;
-    // TARGET: admit t == tmax (tmax > 0).  A caller that serves both query kinds with one copy of this loop (k_shade_hit<.., FUSE>) passes the
+                                          uint32_t target_gid = 0xFFFFFFFFu, float tmax_test_in = -1.0f) {
+    // TARGET: admit t == tmax (tmax > 0).  A caller that serves both NEE queries with one copy of this loop (the fused k_shade_hit) passes the
     // acceptance bound itself: nextafter(tL) for a light ray, tmax for a sky ray (whose target 0xFFFFFFFF makes every t < tmax an occluder).
-    const float tmax_test = tgt ? (tmax_test_in >= 0.0f ? tmax_test_in : __uint_as_float(__float_as_uint(tmax) + 1u)) : tmax;
+    const float tmax_test = TARGET ? (tmax_test_in >= 0.0f ? tmax_test_in : __uint_as_float(__float_as_uint(tmax) + 1u)) : tmax;
     h.slot = 0xFFFFFFFFu; h.gid = 0xFFFFFFFFu; h.t = tmax; h.u = 0.0f; h.v = 0.0f;
     uint32_t best_gid = 0xFFFFFFFFu;
     bool found = false;
@@ -142,12 +138,12 @@ __device__ __forceinline__ bool bvh_trace(const BvhView &b, float3 o, float3 d, 
         const float4 *tp = b.tris + (size_t)slot * 3;
         const float4 ta = ld4<SMEM>(tp), tb = ld4<SMEM>(tp + 1), tc = ld4<SMEM>(tp + 2);
         float t, u, v;
-        if (tri_test<!ANYHIT && !MIXED>(f3(ta), f3(tb), f3(tc), o, d, tmin, tmax_test, t, u, v)) {
+        if (tri_test<!ANYHIT>(f3(ta), f3(tb), f3(tc), o, d, tmin, tmax_test, t, u, v)) {
             const uint32_t gid = __float_as_uint(ta.w);
-            if (tgt && !(t < tmax || gid < target_gid)) return false;
+            if (TARGET && !(t < tmax || gid < target_gid)) return false;
             if (!found || t < h.t || (t == h.t && gid < best_gid)) {
                 found = true; h.t = t; h.u = u; h.v = v; h.slot = slot; h.gid = gid; best_gid = gid;
-                if (any) return true;
+                if (ANYHIT) return true;
             }
         }
         return false;

@@ -531,7 +531,7 @@ void Engine::free_wave() {
     for (auto &B : wb_) {
         for (auto &p : B.ps) { dfree(p.org_pdf); dfree(p.dir_rng); dfree(p.thr_depth); dfree(p.rad_slot); dfree(p.medium); dfree(p.medium_g); dfree(p.vol_depth); }
         dfree(B.so.hit); dfree(B.so.bxdf_pdf); dfree(B.so.e0); dfree(B.so.sky_o); dfree(B.so.sky_d); dfree(B.so.sky_c); dfree(B.so.lit_o); dfree(B.so.lit_d); dfree(B.so.lit_c);
-        dfree(B.sample_buf); dfree(B.rng_carry); dfree(B.q_hit[0]); dfree(B.q_hit[1]); dfree(B.q_miss[0]); dfree(B.q_miss[1]);
+        dfree(B.sample_buf); dfree(B.rng_carry); dfree(B.q_hit); dfree(B.q_miss);
         B.cap = 0;
     }
     wave_cap_ = 0;
@@ -550,7 +550,7 @@ void Engine::ensure_wave(size_t cap, int contexts) {
         a4(B.so.hit); a4(B.so.bxdf_pdf); a4(B.so.e0); a4(B.so.sky_o); a4(B.so.sky_d); a4(B.so.sky_c); a4(B.so.lit_o); a4(B.so.lit_d); a4(B.so.lit_c);
         a4(B.sample_buf);
         CK(cudaMalloc(&B.rng_carry, cap * sizeof(uint32_t)));
-        for (int i = 0; i < 2; i++) { CK(cudaMalloc(&B.q_hit[i], (size_t)MC_COUNT * cap * sizeof(uint32_t))); CK(cudaMalloc(&B.q_miss[i], cap * sizeof(uint32_t))); }   // one hit queue per material class, ping-pong for the fused bounce kernel
+        CK(cudaMalloc(&B.q_hit, (size_t)MC_COUNT * cap * sizeof(uint32_t))); CK(cudaMalloc(&B.q_miss, cap * sizeof(uint32_t)));   // one hit queue per material class
         B.cap = cap;
     }
     wave_cap_ = cap;
@@ -610,7 +610,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     if (const char *e = getenv("B200PT_OVERLAP")) { if (atoi(e) == 0) overlap = false; }
     uint64_t target = 0;                                      // auto wave size (paths per context), when FramesInFlight == 0
     if (cfg_.FramesInFlight == 0) {
-        // Auto wave size: up to 64 M paths per context (~24 GB of wavefront state at ~380 B per path; all contexts capped to a quarter of the free HBM): large enough
+        // Auto wave size: up to 64 M paths per context (~24 GB of wavefront state at ~360 B per path; all contexts capped to a quarter of the free HBM): large enough
         // to amortise the floors above.  On an 80 GB H100 the quarter of free HBM, not the 64 M cap, sets the size.
         target = 64ull << 20;
         size_t free_b = 0, total_b = 0;
@@ -642,13 +642,11 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     // density (not validated by the reference either) scatters on every segment.  A false positive only costs a 4-byte read-back per 16 bounces.
     for (const auto &m : scene_.materials) if (m.Transmission > 0.0f && m.MediumDensity != 0.0f && m.MediumAnisotropy != 1.0f) medium = true;
 
-    // Fused bounce kernels (LaunchCfg::fuse) need the BVH in shared memory and no volumes; they ping-pong the queues and the hit records
-    // (the kernel that consumes bounce k's queue fills bounce k+1's), the unfused pipeline uses buffer 0 only.
+    // The fused shading kernels (LaunchCfg::fuse) need the BVH in shared memory and no volumes.
     const int fuse = pre ? 0 : lc_.fuse;
     const bool camera = lc_.camera && !pre;                   // k_camera: camera rays generated and traced in one kernel (bounce 0's k_extend is skipped)
     const uint32_t cmask = pre ? (class_mask_ | (1u << MC_GENERAL)) : class_mask_;   // volume / atmosphere events ride in the general queue
     const uint32_t qcap = (uint32_t)wave_cap_;
-    const int qsel[2] = { 0, fuse == 2 ? 1 : 0 };
     // Per-launch flags (kernels.h).  WAVE_IMPLIED: k_camera's paths are all inside the image only without chunked dispatch (overhang paths are
     // born dead and keep their full state), and only the fused shading kernels infer the state.  WAVE_STORE: sub-wave 0 ends every path exactly once when the bounce loop provably runs dry -- not
     // with a pre-pass (DEAD_EVENT ends, channel-split paths), not with medium walks (the runaway guard may stop them), not at MaxDepth 0 (no
@@ -691,13 +689,12 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             CK(cudaEventRecord(B.disp_ev, st));
             PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
             if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
-            float4 *const hitb[2] = { B.so.hit, fuse == 2 ? B.so.bxdf_pdf : B.so.hit };
+            const Queues q{ B.q_miss, B.q_hit, qcap };
             for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
                 const uint32_t wflags = (s == 0 && store_ok ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
                 if (camera) {
-                    const Queues q0{ B.q_miss[0], B.q_hit[0], qcap };
-                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, hitb[0],
-                                                  B.counts, q0, d_ctr_, st, act));
+                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
+                                                  B.counts, q, d_ctr_, st, act));
                 } else launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
                 launches++; mark(0);
                 int cur = 0; uint32_t k = 0;
@@ -707,12 +704,11 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     if (chunk == 0) break;
                     for (uint32_t b = 0; b < chunk; b++, k++) {
                         const uint32_t par = k & 1u, bflags = wflags | (k == 0 ? implied_flag : 0u);
-                        const Queues qc{ B.q_miss[qsel[par]], B.q_hit[qsel[par]], qcap }, qn{ B.q_miss[qsel[par ^ 1u]], B.q_hit[qsel[par ^ 1u]], qcap };
                         if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
-                        if ((fuse != 2 || k == 0) && !(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], hitb[par], B.counts, par, qc, d_ctr_, k == 0, st); launches++; } mark(1);
-                        launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, hitb[par], hitb[par ^ 1u], B.counts, par, qc, qn, B.sample_buf, B.rng_carry, d_ctr_,
+                        if (!(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); launches++; } mark(1);
+                        launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_,
                                                  fuse, cmask, bflags, st); mark(2);
-                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, qc, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
+                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty

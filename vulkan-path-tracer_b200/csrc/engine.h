@@ -150,7 +150,7 @@ private:
     // overlap the full-machine head of wave w+1; k_resolve runs in dispatch order (events), so the image does not depend on it.
     struct WaveBuf {
         PathState ps[2]{}; ShadeOut so{};
-        float4 *sample_buf = nullptr; uint32_t *rng_carry = nullptr; uint32_t *q_hit[2] = { nullptr, nullptr }, *q_miss[2] = { nullptr, nullptr };
+        float4 *sample_buf = nullptr; uint32_t *rng_carry = nullptr; uint32_t *q_hit = nullptr, *q_miss = nullptr;
         uint32_t *counts = nullptr, *h_count = nullptr;
         DevDispatch *d_disp = nullptr, *h_disp = nullptr; cudaEvent_t disp_ev = nullptr;   // this context's slice of the dispatch table (pinned host copy reusable once disp_ev has fired)
         size_t cap = 0;

@@ -17,10 +17,11 @@ struct LaunchCfg {
     int grid_shadow;    // persistent grid of k_shadow_dyn
     bool wide;          // the dynamic-fetch kernels walk the BVH4 (DevScene::nodes4)
     int dyn_stack;      // shared-memory stack entries per thread of the dynamic-fetch kernels (BVH4: overflow goes to local memory)
-    bool big;           // bvh_in_smem with a BVH > 64 KiB: one 512-thread CTA per SM for k_extend and the fused bounce kernels
+    bool big;           // bvh_in_smem with a BVH > 64 KiB: one 512-thread CTA per SM for k_extend, k_camera, k_connect and the fused k_shade_hit
     int extend_threads; // CTA size of k_extend (256, big: 512)
-    int fuse;           // 0: k_shade_hit + k_connect; 1: NEE queries + path epilogue inside k_shade_hit; 2: + the next segment's TraceRay (one kernel per bounce and class)
-    int grid_bounce;    // persistent grid of the fused k_shade_hit instantiations (BVH + stacks in shared memory)
+    int bounce_threads; // CTA size of the fused k_shade_hit (128, big: 512)
+    int fuse;           // 0: k_shade_hit + k_connect; 1: NEE queries + path epilogue inside k_shade_hit (no k_connect)
+    int grid_bounce;    // persistent grid of the fused k_shade_hit (BVH + stacks in shared memory)
     bool camera;        // camera rays generated and traced by k_camera (shared-memory BVH, one ray per thread) when the call has no pre-pass
     int grid_camera;    // persistent grid of k_camera (extend_threads per CTA)
 };
@@ -65,9 +66,9 @@ void launch_denoise_filter(uint32_t W, uint32_t H, const float4 *color, const fl
 void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
                    WaveCounters *ctr, bool primary, cudaStream_t st);
 // k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.
-// fuse != 0: the bounce is finished inside k_shade_hit (dst, q_next, hit_out are written), launch_connect is not called.
-int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in, float4 *hit_out,
-                 uint32_t *ctrl, uint32_t parity, Queues q, Queues q_next, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
+// fuse != 0: the bounce is finished inside k_shade_hit (the survivors are written compacted to dst), launch_connect is not called.
+int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
+                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
                  int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st);
 void launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
                           float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st);   // before launch_extend when the scene has volumes or the atmosphere is on (DevScene::pre_pass)

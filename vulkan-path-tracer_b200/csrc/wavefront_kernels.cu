@@ -14,9 +14,7 @@
 //     k_connect  shadow rays, payload.Emitted assembly,        SH/ClosestHit.slang:139,171-176,326-372
 //                luminance clamp, throughput, Russian          SH/RayGen.slang:92-113
 //                roulette, ballot/prefix-sum compaction
-//   scenes whose BVH is staged in shared memory by TMA fuse the shadow queries and the roulette into k_shade_hit<CLASS, ., 1> (default), or
-//   run the bounce as ONE kernel per class (k_shade_hit<CLASS, ., 2>): shading + both NEE shadow queries + roulette + the next segment's
-//   closest-hit query + queue append.
+//   scenes whose BVH is staged in shared memory by TMA fuse the shadow queries and the roulette into k_shade_hit<CLASS, ., true> (default).
 //   k_resolve  NaN/Inf rejection + running mean                SH/RayGen.slang:116-159
 //   (adaptive sampling, no reference equivalent: k_raygen / k_camera over a list of active pixels, k_resolve_adaptive, and
 //    k_adaptive_update + k_adaptive_compact at interval boundaries)
@@ -362,7 +360,7 @@ __device__ __forceinline__ void finish_path_slot(uint32_t flags, uint32_t slot, 
     sample_buf[slot] = acc;
     if (flags & WAVE_CARRY) rng_carry[slot] = rng_state;
 }
-// SH/Miss.slang:8-76 + the ray-gen epilogue for a path whose segment missed (shared by k_shade_miss and the fused bounce kernel's tail)
+// SH/Miss.slang:8-76 + the ray-gen epilogue for a path whose segment missed (k_shade_miss)
 __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const DevConfig &cfg, float3 dir, uint32_t rng_state, float4 t4, float4 r4, float payPDF,
                                                    uint32_t flags, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
     const uint32_t depth = __float_as_uint(t4.w) & DEPTH_MASK;
@@ -392,12 +390,10 @@ __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const Dev
 // k_shade_miss : SH/Miss.slang:8-76 for the miss queue.  A miss always ends the path (Depth = MAX_DEPTH), so the
 //                ray-gen epilogue (SH/RayGen.slang:92-128) is applied here and the path never reaches k_connect.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_shade_miss(DevScene sc, DevConfig cfg, PathState ps, uint32_t *__restrict__ ctrl, uint32_t parity, uint32_t reset_next,
+__global__ void __launch_bounds__(256) k_shade_miss(DevScene sc, DevConfig cfg, PathState ps, uint32_t *__restrict__ ctrl, uint32_t parity,
                                                      const uint32_t *__restrict__ q_miss, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry,
                                                      WaveCounters *ctr, uint32_t flags) {
     const uint32_t n = ctrl[CTRL_Q + 8u * parity];
-    // fused pipeline (k_bounce): this is the first kernel of the bounce, so it clears the counters the bounce kernels are about to fill
-    if (reset_next && blockIdx.x == 0 && threadIdx.x == 0) ctrl_reset_parity(ctrl, parity ^ 1u);
     const bool implied = (flags & WAVE_IMPLIED) != 0u;
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
         const uint32_t i = q_miss[j];
@@ -411,8 +407,7 @@ __global__ void __launch_bounds__(256) k_shade_miss(DevScene sc, DevConfig cfg, 
 }
 
 // SH/RayGen.slang:92-113 for a path that was shaded at a hit, in two parts: path_roulette (throughput update, Russian roulette (Q4), loop
-// condition) does not depend on the NEE terms, so the fused bounce kernel decides a path's next segment before its shadow queries are traced;
-// path_radiance (contribution, luminance clamp unless Depth == 1 (Q3), radiance; a finished path is folded into its sample slot, :116-128)
+// condition) does not depend on the NEE terms; path_radiance (contribution, luminance clamp unless Depth == 1 (Q3), radiance; a finished path is folded into its sample slot, :116-128)
 // runs once they are joined.  k_connect calls both in sequence.
 // The join and every product / sum of the epilogue are written with explicitly rounded operations, in the form k_connect compiled to when
 // its inputs came from memory: a value that stays in registers (the fused kernels) must not be contracted into an FMA that the unfused
@@ -444,37 +439,20 @@ __device__ __forceinline__ float3 path_radiance(const DevConfig &cfg, float3 emi
 
 // ------------------------------------------------------------------------------------------------
 // k_shade_hit<CLASS, VOL, FUSE> : SH/ClosestHit.slang:20-378 for the hit queue of one material class.
-//   FUSE == 0  writes the new ray + payload in place and <= 2 NEE shadow requests; k_connect (or k_shadow_dyn + k_connect) finishes the bounce.
-//   FUSE == 1  for scenes whose BVH is staged in shared memory (no volumes): each NEE request is traced the moment it is built (one copy of
-//              the any-hit traversal inside the rolled NEE loop), then SH/RayGen.slang:92-113 runs in the same thread and the survivor is
-//              written compacted to the other PathState buffer -- no request / payload round trip through HBM, no k_connect.
-//   FUSE == 2  the bounce kernel of shared-memory scenes (the default there): one kernel per (bounce, class) that also traces the survivor's
-//              NEXT segment (the next bounce's k_extend) and appends it to the next bounce's miss / class queues.  A warp iteration (32 queue
-//              entries) runs in three phases:
-//                shade     up to the NEE requests, which are written to the warp's ray list in shared memory instead of being traced;
-//                roulette  path_roulette decides the path's fate (shadow queries consume no random numbers when this kernel runs: no
-//                          volumes, no atmosphere), a survivor appends its next segment to the same list;
-//                trace     the warp traces the list densely, one entry per lane and round (one copy of the traversal, query kind chosen
-//                          per ray), then each owner joins its visible NEE terms, finishes or compacts its path and queues the next segment.
-//              Per continuing path: 80 B read + 84 B written.
+//   !FUSE  writes the new ray + payload in place and <= 2 NEE shadow requests; k_connect (or k_shadow_dyn + k_connect) finishes the bounce.
+//   FUSE   for scenes whose BVH is staged in shared memory (no volumes): each NEE request is traced the moment it is built (one copy of
+//          the any-hit traversal inside the rolled NEE loop), then SH/RayGen.slang:92-113 runs in the same thread and the survivor is
+//          written compacted to the other PathState buffer -- no request / payload round trip through HBM, no k_connect.
 // ------------------------------------------------------------------------------------------------
 #ifndef SHADE_MIN_BLOCKS
 #define SHADE_MIN_BLOCKS 5
 #endif
-#ifndef BOUNCE_MIN_BLOCKS                                                   // 4 x 128 threads: 128 registers, no spills (at 5 the 96-register cap spills 84-140 B)
-#define BOUNCE_MIN_BLOCKS 4
-#endif
-// Ray list of k_shade_hit<., ., 2> (dynamic shared memory after the stacks and the BVH): per warp up to 3 rays per lane -- sky, light,
-// next segment.  Entry e = two float4: [2e] origin + tmax, [2e+1] direction + target word (0xFFFFFFFF: sky, RAY_NEXT: the next segment's
-// closest-hit query, otherwise the sampled light triangle).  The traversal writes its hit record (t, u, v, gid) over [2e].
-constexpr uint32_t RAY_LIST_PER_WARP = 96;
-constexpr size_t RAY_LIST_BYTES_PER_WARP = (size_t)RAY_LIST_PER_WARP * 2 * sizeof(float4);
-constexpr uint32_t RAY_NEXT = 0xFFFFFFFEu;
-// BIG: 512-thread CTAs, one per SM -- for BVHs of 64..~170 KiB, which fit shared memory only once per SM (config 4's glass scene: 108 KiB).
-template <uint32_t CLASS, bool VOL, int FUSE, bool BIG = false>   // VOL: the scene has AABB volumes (volumes.cuh) -- volume events in the hit queue are skipped, NEE terms get the transmittance
-__global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_BLOCKS : SHADE_MIN_BLOCKS)) k_shade_hit(DevScene sc, DevConfig cfg, PathState ps, PathState dst, ShadeOut so,
-                                                    const float4 *__restrict__ hit_in, float4 *__restrict__ hit_out,
-                                                    uint32_t *__restrict__ ctrl, uint32_t parity, Queues q, Queues q_next,
+// The fused form runs 128-thread CTAs (4 per SM) or, in big mode, one 512-thread CTA per SM (BVHs of 64 KiB and more, which fit shared memory
+// only once per SM).  Both bounds cap it at 128 registers, without spills (a 5 x 128 bound's 96-register cap spills 84-140 B).
+template <uint32_t CLASS, bool VOL, bool FUSE>   // VOL: the scene has AABB volumes (volumes.cuh) -- volume events in the hit queue are skipped, NEE terms get the transmittance
+__global__ void __launch_bounds__(FUSE ? 512 : 128, FUSE ? 1 : SHADE_MIN_BLOCKS) k_shade_hit(DevScene sc, DevConfig cfg, PathState ps, PathState dst, ShadeOut so,
+                                                    const float4 *__restrict__ hit_in,
+                                                    uint32_t *__restrict__ ctrl, uint32_t parity, Queues q,
                                                     float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry, int max_stack, WaveCounters *ctr,
                                                     uint32_t flags) {
     constexpr uint32_t LOBES = class_lobes(CLASS);
@@ -483,24 +461,15 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
     const bool implied = FUSE && (flags & WAVE_IMPLIED) != 0u;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
-    __shared__ uint32_t list_count[FUSE == 2 ? (BIG ? 16 : 4) : 1];           // entries in each warp's ray list
     int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
     const int stride = blockDim.x;
     BvhView bv;
     if (FUSE) bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
-    float4 *list = nullptr; uint32_t *list_n = nullptr;
-    if (FUSE == 2) {
-        list = reinterpret_cast<float4 *>(smem + (size_t)max_stack * blockDim.x * sizeof(int) + sc.bvh_bytes) + (threadIdx.x >> 5) * (2u * RAY_LIST_PER_WARP);
-        list_n = list_count + (threadIdx.x >> 5);
-        if ((threadIdx.x & 31u) == 0u) *list_n = 0u;
-        __syncwarp();
-    }
     const uint32_t n = ctrl[CTRL_Q + 8u * parity + 1u + CLASS];
     const uint32_t *__restrict__ q_hit = q.hit + (size_t)CLASS * q.cap;
-    uint32_t *qc_next = ctrl + CTRL_Q + 8u * (parity ^ 1u);
     uint32_t *n_next_ptr = ctrl + (parity ^ 1u);
     const uint32_t lane = threadIdx.x & 31u;
-    uint32_t n_med = 0, n_shadow = 0, n_ext = 0;
+    uint32_t n_med = 0, n_shadow = 0;
     const float4 zero4 = make_float4(0, 0, 0, 0);
     // The queue entry and the hit record of the NEXT path of this thread are fetched one iteration ahead (two dependent DRAM
     // round trips off the critical path for 5 registers); its path-state lines are pulled towards L2 meanwhile.
@@ -510,7 +479,6 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
     if (j < n) { i_nx = q_hit[j]; h4_nx = hit_in[i_nx]; }
     const uint32_t n_loop = FUSE ? ((n + 31u) & ~31u) : n;                  // fused: warps stay converged for the compaction collectives
     for (; j < n_loop; j += jstep) {
-        if (FUSE == 2) __syncwarp();                                        // the previous iteration's list reads and counter reset are done
         const bool valid = j < n;
         // ---- results of the shading part, consumed by the fused tail
         bool shaded = false;                                                // this lane holds a path whose bounce must be finished (fused)
@@ -518,8 +486,6 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
         float4 b4 = zero4; uint32_t newDflags = 0u; Rng rng; rng.s = 0u;
         bool entered = false;
         const DevMaterial *cmp = nullptr;
-        uint32_t ents = 0xFFFFFFu;                                          // FUSE == 2: list entries of this lane's sky / light / next-segment rays (8 bits each, 0xFF: none)
-        float3 c_sky = f3(0.0f), c_lit = f3(0.0f);                          // FUSE == 2: their NEE terms, joined once the visibility is known
         const uint32_t i = i_nx;
         if (valid) do {
             const float4 h4 = h4_nx;
@@ -668,13 +634,7 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                             tmax = tL; tmax_test = __uint_as_float(__float_as_uint(tL) + 1u);
                         }
                         n_shadow++;
-                        if (go && FUSE == 2) {                                  // queued; traced with the warp's other rays after the roulette
-                            const uint32_t e = atomicAdd(list_n, 1u);
-                            list[2u * e] = make_float4(ro.x, ro.y, ro.z, tmax);
-                            list[2u * e + 1u] = make_float4(toW.x, toW.y, toW.z, __uint_as_float(k == 0 ? 0xFFFFFFFFu : lgid));
-                            ents = (ents & ~(0xFFu << (8 * k))) | (e << (8 * k));
-                            if (k == 0) c_sky = c; else c_lit = c;
-                        } else if (go) {
+                        if (go) {
                             HitRec hs;
                             const bool occluded = bvh_trace<true, true, false, true, true>(bv, ro, toW, 0.0001f, tmax, hs, stack, stride, max_stack, nullptr, nullptr, lgid, tmax_test);
                             if (!occluded) emitted = nee_join(emitted, c);
@@ -725,45 +685,13 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
         } while (false);
 
         if (FUSE) {
-            // ---- SH/RayGen.slang:92-113, then (FUSE == 2) the next segment's TraceRay, then compaction into the other PathState buffer
+            // ---- SH/RayGen.slang:92-113, then compaction into the other PathState buffer
             bool alive = false;
             float4 thr4 = zero4, r4 = zero4; float3 thr = f3(0.0f), rad = f3(0.0f);
             if (shaded) {
                 if (implied) { thr4 = camera_implied_thr_depth(true); r4 = camera_implied_rad_slot(i); }
                 else { thr4 = ps.thr_depth[i]; r4 = ps.rad_slot[i]; }
                 alive = path_roulette(cfg, b4, newDflags & DEPTH_MASK, thr4, rng, thr);
-            }
-            uint32_t code = Q_NONE; float4 h4 = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0xFFFFFFFFu));
-            if (FUSE == 2) {
-                if (alive) {                                                // SH/RayGen.slang:70-72 of the next loop iteration, queued
-                    const uint32_t e = atomicAdd(list_n, 1u);
-                    list[2u * e] = make_float4(newO.x, newO.y, newO.z, 100000.0f);
-                    list[2u * e + 1u] = make_float4(newD.x, newD.y, newD.z, __uint_as_float(RAY_NEXT));
-                    ents = (ents & 0x00FFFFu) | (e << 16);
-                    n_ext++;
-                }
-                __syncwarp();
-                // trace the warp's list densely: round r hands entry 32 r + lane to this lane
-                const uint32_t n_rays = *list_n;
-                for (uint32_t e = lane; e < n_rays; e += 32u) {
-                    const float4 a = list[2u * e], b = list[2u * e + 1u];
-                    const uint32_t target = __float_as_uint(b.w);
-                    const bool shadow = target != RAY_NEXT;
-                    HitRec h;
-                    bvh_trace<true, false, false, false, true, true>(bv, f3(a), shadow ? f3(b) : normalize_ray(f3(b)), shadow ? 0.0001f : 0.01f, a.w, h, stack, stride, max_stack,
-                                                                       nullptr, nullptr, target, target == 0xFFFFFFFFu ? a.w : -1.0f, shadow);
-                    list[2u * e] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
-                }
-                __syncwarp();
-                if (lane == 0u) *list_n = 0u;                               // ordered before the next iteration's appends by the __syncwarp there
-                // join in the reference's order: e0, then the sky term, then the light term, each iff its ray came out unoccluded
-                const uint32_t e_sky = ents & 0xFFu, e_lit = (ents >> 8) & 0xFFu, e_ext = ents >> 16;
-                if (e_sky != 0xFFu && __float_as_uint(list[2u * e_sky].w) == 0xFFFFFFFFu) emitted = nee_join(emitted, c_sky);
-                if (e_lit != 0xFFu && __float_as_uint(list[2u * e_lit].w) == 0xFFFFFFFFu) emitted = nee_join(emitted, c_lit);
-                if (alive) {
-                    h4 = list[2u * e_ext];
-                    code = __float_as_uint(h4.w) != 0xFFFFFFFFu ? hit_code(sc, __float_as_uint(h4.w)) : 0u;
-                }
             }
             if (shaded) rad = path_radiance(cfg, emitted, newDflags & DEPTH_MASK, dflags_channel(newDflags), thr4, r4, alive, rng.s, flags, sample_buf, rng_carry);
             const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alive);
@@ -786,16 +714,13 @@ __global__ void __launch_bounds__(BIG ? 512 : 128, BIG ? 1 : (FUSE ? BOUNCE_MIN_
                         } else { mv = ps.medium[i]; mg = ps.medium_g[i]; }
                         dst.medium[k] = mv; dst.medium_g[k] = mg;
                     }
-                    if (FUSE == 2) hit_out[k] = h4;
                 }
-                if (FUSE == 2) queue_append(code, k, qc_next, q_next, lane);
             }
         }
     }
-    for (int o = 16; o > 0; o >>= 1) { n_med += __shfl_down_sync(0xFFFFFFFFu, n_med, o); n_shadow += __shfl_down_sync(0xFFFFFFFFu, n_shadow, o); n_ext += __shfl_down_sync(0xFFFFFFFFu, n_ext, o); }
+    for (int o = 16; o > 0; o >>= 1) { n_med += __shfl_down_sync(0xFFFFFFFFu, n_med, o); n_shadow += __shfl_down_sync(0xFFFFFFFFu, n_shadow, o); }
     if (lane == 0 && n_med) atomicAdd(&ctr->medium_events, (unsigned long long)n_med);
     if (FUSE && lane == 0 && n_shadow) atomicAdd(&ctr->shadow_rays, (unsigned long long)n_shadow);
-    if (FUSE == 2 && lane == 0 && n_ext) atomicAdd(&ctr->extend_rays, (unsigned long long)n_ext);
     if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&ctr->shade_invocations, (unsigned long long)n); atomicAdd(&ctr->surface_hits, (unsigned long long)n); }
 }
 
@@ -1445,10 +1370,6 @@ static constexpr size_t DYN_RING_BYTES_HOST = 8 * 128 * sizeof(uint32_t);
 static size_t trace_smem_bytes(const DevScene &sc, int max_stack, int threads, bool smem) {
     return (size_t)max_stack * threads * sizeof(int) + (smem ? sc.bvh_bytes : 0);
 }
-// k_shade_hit<., ., 2>: stacks + BVH + one ray list per warp
-static size_t bounce_smem_bytes(const DevScene &sc, int max_stack, int threads) {
-    return trace_smem_bytes(sc, max_stack, threads, true) + (size_t)(threads / 32) * RAY_LIST_BYTES_PER_WARP;
-}
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) applies to the CURRENT device only, and the C-ABI lets one process drive several GPUs
 // (b200pt_create(device, ..)): the opt-in is tracked per device ordinal.
@@ -1479,9 +1400,8 @@ static int set_attrs_for_current_device() {
     optin((const void *)k_shadow_dyn<true, false>); optin((const void *)k_shadow_dyn<false, false>); optin((const void *)k_shadow_dyn<false, true>);
     optin((const void *)k_trace_rays<true>); optin((const void *)k_trace_rays<false>);
     optin((const void *)k_volume_decide<true>); optin((const void *)k_volume_decide<false>);
-#define B200PT_OPTIN_BOUNCE(C) optin((const void *)k_shade_hit<C, false, 1>); optin((const void *)k_shade_hit<C, false, 2>); optin((const void *)k_shade_hit<C, false, 2, true>);
-    B200PT_OPTIN_BOUNCE(MC_DIFFUSE) B200PT_OPTIN_BOUNCE(MC_METAL) B200PT_OPTIN_BOUNCE(MC_GLASS) B200PT_OPTIN_BOUNCE(MC_GENERAL)
-#undef B200PT_OPTIN_BOUNCE
+    optin((const void *)k_shade_hit<MC_DIFFUSE, false, true>); optin((const void *)k_shade_hit<MC_METAL, false, true>);
+    optin((const void *)k_shade_hit<MC_GLASS, false, true>); optin((const void *)k_shade_hit<MC_GENERAL, false, true>);
     cudaGetLastError();
     if (rc == 0 && dev >= 0 && dev < 64) g_attr_done_mask |= 1ull << dev;
     return rc;
@@ -1496,16 +1416,33 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     const int sms = prop.multiProcessorCount;
     lc->max_stack = bvh_max_depth + 2; if (lc->max_stack < 4) lc->max_stack = 4; if (lc->max_stack > 64) lc->max_stack = 64;
     // Whole BVH in shared memory: <= 64 KiB -> several CTAs per SM (Cornell: 1.3 KiB); up to what fits beside the stacks of ONE 512-thread CTA per SM
-    // -> "big" mode (config 4's glass scene: 108 KiB): k_extend, k_connect and the fused bounce kernels run 512-thread CTAs.
+    // -> "big" mode (config 4's glass scene: 108 KiB): k_extend, k_connect, k_camera and the fused k_shade_hit run 512-thread CTAs.
     const bool aligned = sc.bvh_bytes > 0 && (sc.bvh_bytes % 16u) == 0;
     const bool fits_small = aligned && sc.bvh_bytes <= 64u * 1024u;
     // Big mode runs the one-ray-per-thread kernels over the shared-memory BVH at 8-16 warps per SM with divergent LDS; the dynamic-fetch kernels
-    // over L2 are the default there -> big mode is OPT-IN (B200PT_SMEM_BIG=1).
+    // over L2 are the default there -> big mode is OPT-IN (B200PT_SMEM_BIG=1).  Each of those 512-thread kernels must fit the stacks and the BVH
+    // into its opt-in limit: 227 KiB minus its static shared memory (k_camera's flat-walk table, ~4 KiB, is the largest).
     bool fits_big = false;
-    if (const char *e = getenv("B200PT_SMEM_BIG")) { if (atoi(e) == 1) fits_big = aligned && !fits_small && bounce_smem_bytes(sc, lc->max_stack, 512) <= 226u * 1024u; }
+    if (const char *e = getenv("B200PT_SMEM_BIG")) {
+        if (atoi(e) == 1 && aligned && !fits_small) {
+            const size_t need = trace_smem_bytes(sc, lc->max_stack, 512, true);
+            const void *const big_kernels[] = {
+                (const void *)k_extend<true, true, true>, (const void *)k_extend<true, true, false>, (const void *)k_extend<true, false, true>, (const void *)k_extend<true, false, false>,
+                (const void *)k_camera<true, true>, (const void *)k_camera<true, false>, (const void *)k_camera<false, true>, (const void *)k_camera<false, false>,
+                (const void *)k_connect<true, true>, (const void *)k_connect<true, true, true>,
+                (const void *)k_shade_hit<MC_DIFFUSE, false, true>, (const void *)k_shade_hit<MC_METAL, false, true>,
+                (const void *)k_shade_hit<MC_GLASS, false, true>, (const void *)k_shade_hit<MC_GENERAL, false, true> };
+            fits_big = true;
+            for (const void *f : big_kernels) {
+                cudaFuncAttributes a{};
+                if (cudaFuncGetAttributes(&a, f) != cudaSuccess || need + a.sharedSizeBytes > 227u * 1024u) fits_big = false;
+            }
+        }
+    }
     lc->bvh_in_smem = fits_small || fits_big;
     lc->big = fits_big;
     lc->extend_threads = fits_big ? 512 : 256;
+    lc->bounce_threads = fits_big ? 512 : 128;
     const size_t sh = trace_smem_bytes(sc, lc->max_stack, lc->extend_threads, lc->bvh_in_smem);
     const size_t sh256 = trace_smem_bytes(sc, lc->max_stack, 256, lc->bvh_in_smem);
     // traversal shape: dynamic-fetch while-while kernels (bvh_dynfetch.cuh) over the BVH4 when the BVH lives in L2/HBM, one ray per thread
@@ -1527,15 +1464,11 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
         if (need - lc->dyn_stack > DYN_SPILL) lc->wide = false, lc->dyn_stack = lc->max_stack;   // deeper than shared column + overflow array: BVH2
     }
     // Bounce pipeline of scenes whose BVH is staged in shared memory and walked one ray per thread (the default elsewhere is 0):
-    //   1 (default): k_shade_hit<., ., 1> traces each NEE query the moment it is built and finishes the path (roulette, radiance, compaction) in
-    //      the same thread; the next segment's closest hit runs in k_extend<true, false, .> at 24 warps per SM.
-    //   2 (big mode's only fused form): k_shade_hit<., ., 2> also traces the next segment, from a per-warp ray list in shared memory.
-    // On the Cornell box 1 is faster: the bounce kernel runs at 16 warps per SM with 118-128 registers, and handing it the closest-hit query
-    // costs more than the separate k_extend does.  Measured with k_camera and the 24-warp k_extend on an H100 at 400 W (DESIGN.md section 8,
-    // which chose this default); before them, on a 700 W card, FUSE=1 already led by 8.5 % (section 9).  B200PT_FUSE=0|1|2 overrides (0: k_extend + k_shade_hit
-    // + k_connect).
-    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? (lc->big ? 2 : 1) : 0;
-    if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if (v >= 0 && v <= 2 && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = (lc->big && v == 1) ? 2 : v; }
+    //   1 (default): k_shade_hit<., ., true> traces each NEE query the moment it is built and finishes the path (roulette, radiance, compaction)
+    //      in the same thread; the next segment's closest hit runs in k_extend<true, false, .>.
+    // B200PT_FUSE=0 overrides (k_extend + k_shade_hit + k_connect); any other value keeps the default.
+    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? 1 : 0;
+    if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if ((v == 0 || v == 1) && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = v; }
     // Camera rays of those scenes: generated and traced in one kernel (k_camera) instead of k_raygen + k_extend<true, true, .>, unless the scene
     // needs a pre-pass (decided per call: Engine::path_trace).  B200PT_CAMERA=0 keeps the pair.
     lc->camera = lc->bvh_in_smem && !lc->trav_dyn;
@@ -1566,9 +1499,9 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     }
     if (occ_sh < 1) occ_sh = 1;
     lc->grid_shadow = sms * occ_sh;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_shade_hit<MC_GENERAL, false, 0>, 128, 0);
-    if (lc->big) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2, true>, 512, bounce_smem_bytes(sc, lc->max_stack, 512));
-    else if (lc->bvh_in_smem) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, 2>, 128, bounce_smem_bytes(sc, lc->max_stack, 128));
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_shade_hit<MC_GENERAL, false, false>, 128, 0);
+    if (lc->bvh_in_smem) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, true>, lc->bounce_threads,
+                                                                       trace_smem_bytes(sc, lc->max_stack, lc->bounce_threads, true));
     if (occ_e < 1) occ_e = 1; if (occ_c < 1) occ_c = 1; if (occ_s < 1) occ_s = 1; if (occ_b < 1) occ_b = 1;
     lc->grid_extend = sms * occ_e; lc->grid_connect = sms * occ_c;
     { int occ_t = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, lc->bvh_in_smem ? k_trace_rays<true> : k_trace_rays<false>, 256, sh256); lc->grid_trace = sms * (occ_t < 1 ? 1 : occ_t); }
@@ -1641,21 +1574,19 @@ void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4
 #undef B200PT_EXT_U
 #undef B200PT_EXT
 }
-// k_shade_miss + one k_shade_hit<CLASS> per material class present in the scene (+ k_shade_volume).  fuse (0 / 1 / 2): see k_shade_hit.
+// k_shade_miss + one k_shade_hit<CLASS> per material class present in the scene (+ k_shade_volume).  fuse (0 / 1): see k_shade_hit.
 // Returns the number of kernels launched.
-int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in, float4 *hit_out,
-                 uint32_t *ctrl, uint32_t parity, Queues q, Queues q_next, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
+int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
+                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
                  int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st) {
     set_attrs_for_current_device();
     int launched = 1;
-    k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, fuse == 2 ? 1u : 0u, q.miss, sample_buf, rng_carry, ctr, flags);
-    const size_t shb = fuse == 2 ? bounce_smem_bytes(sc, lc.max_stack, lc.big ? 512 : 128) : trace_smem_bytes(sc, lc.max_stack, 128, true);
+    k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, q.miss, sample_buf, rng_carry, ctr, flags);
+    const size_t shb = trace_smem_bytes(sc, lc.max_stack, lc.bounce_threads, true);
 #define B200PT_SHADE(C) do { if (class_mask & (1u << C)) { launched++;                                                                                              \
-        if (fuse == 2 && lc.big) k_shade_hit<C, false, 2, true><<<lc.grid_bounce, 512, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
-        else if (fuse == 2) k_shade_hit<C, false, 2><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags);      \
-        else if (fuse == 1) k_shade_hit<C, false, 1><<<lc.grid_bounce, 128, shb, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
-        else if (sc.pre_pass) k_shade_hit<C, true, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags);   \
-        else k_shade_hit<C, false, 0><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, hit_out, ctrl, parity, q, q_next, sample_buf, rng_carry, lc.max_stack, ctr, flags); } } while (0)
+        if (fuse) k_shade_hit<C, false, true><<<lc.grid_bounce, lc.bounce_threads, shb, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
+        else if (sc.pre_pass) k_shade_hit<C, true, false><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);       \
+        else k_shade_hit<C, false, false><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags); } } while (0)
     B200PT_SHADE(MC_DIFFUSE); B200PT_SHADE(MC_METAL); B200PT_SHADE(MC_GLASS); B200PT_SHADE(MC_GENERAL);
 #undef B200PT_SHADE
     if (sc.pre_pass) { launched++; k_shade_volume<<<lc.grid_light, 128, 0, st>>>(sc, cfg, ps, so, ctrl, parity, q, ctr); }
