@@ -174,21 +174,12 @@ static int streaming_grid(uint32_t n) {
     return (int)(blocks < 1u ? 1u : (blocks < cap ? blocks : cap));
 }
 
+FeaturesKernel features_kernel(bool smem) { return smem ? k_features<true> : k_features<false>; }
+
 int launch_features(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, float3 forward, uint32_t samples, uint32_t seed0,
                     float4 *albedo_cov, float4 *normal_depth, cudaStream_t st) {
-    const bool smem = lc.bvh_in_smem;
-    const void *fn = smem ? (const void *)k_features<true> : (const void *)k_features<false>;
-    const size_t sh = (size_t)lc.max_stack * 256 * sizeof(int) + (smem ? sc.bvh_bytes : 0);
-    // the opt-in is per device and cheap: set it on every launch instead of tracking devices
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh);
-    if (e != cudaSuccess) return (int)e;
-    int dev = 0, sms = 0, occ = 0;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, 256, sh)) != cudaSuccess) return (int)e;
-    const int grid = sms * (occ < 1 ? 1 : occ);                           // persistent: each CTA stages the BVH once
-    if (smem) k_features<true><<<grid, 256, sh, st>>>(sc, cfg, forward, samples, seed0, lc.max_stack, albedo_cov, normal_depth);
-    else k_features<false><<<grid, 256, sh, st>>>(sc, cfg, forward, samples, seed0, lc.max_stack, albedo_cov, normal_depth);
+    // persistent grid (query_launch_cfg): each CTA stages the BVH once
+    features_kernel(lc.bvh_in_smem)<<<lc.grid_features, 256, lc.smem_trace, st>>>(sc, cfg, forward, samples, seed0, lc.max_stack, albedo_cov, normal_depth);
     return (int)cudaGetLastError();
 }
 

@@ -634,25 +634,14 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     const DevConfig dc = make_dev_config();
     auto pcg = [](uint32_t in) { uint32_t st = in * 747796405u + 2891336453u; uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; };
 
-    const uint32_t n_vol = ds_.n_volumes;
-    const bool pre = n_vol != 0u || atmosphere_.Enable != 0u;   // k_volume_decide + k_shade_volume run: volumes and / or the atmosphere (csrc/atmosphere.cuh)
-    ds_.pre_pass = pre ? 1u : 0u;
     bool medium = false;                                      // can a path random-walk inside a mesh without gaining Depth?
     // Conservative: the device-side metallic value is Metallic * texel, so the constant factor alone cannot rule refraction out, and a negative
     // density (not validated by the reference either) scatters on every segment.  A false positive only costs a 4-byte read-back per 16 bounces.
     for (const auto &m : scene_.materials) if (m.Transmission > 0.0f && m.MediumDensity != 0.0f && m.MediumAnisotropy != 1.0f) medium = true;
-
-    // The fused shading kernels (LaunchCfg::fuse) need the BVH in shared memory and no volumes.
-    const int fuse = pre ? 0 : lc_.fuse;
-    const bool camera = lc_.camera && !pre;                   // k_camera: camera rays generated and traced in one kernel (bounce 0's k_extend is skipped)
-    const uint32_t cmask = pre ? (class_mask_ | (1u << MC_GENERAL)) : class_mask_;   // volume / atmosphere events ride in the general queue
+    const CallPlan cp = plan_call(lc_, ds_, dc, medium, class_mask_);
+    ds_.pre_pass = cp.pre ? 1u : 0u;
+    const uint32_t implied_flag = cp.implied ? WAVE_IMPLIED : 0u;   // per-launch flags: kernels.h
     const uint32_t qcap = (uint32_t)wave_cap_;
-    // Per-launch flags (kernels.h).  WAVE_IMPLIED: k_camera's paths are all inside the image only without chunked dispatch (overhang paths are
-    // born dead and keep their full state), and only the fused shading kernels infer the state.  WAVE_STORE: sub-wave 0 ends every path exactly once when the bounce loop provably runs dry -- not
-    // with a pre-pass (DEAD_EVENT ends, channel-split paths), not with medium walks (the runaway guard may stop them), not at MaxDepth 0 (no
-    // bounce runs, the slots must read zero).
-    const uint32_t implied_flag = (camera && S == 1 && fuse != 0) ? WAVE_IMPLIED : 0u;
-    const bool store_ok = !pre && !medium && cfg_.MaxDepth > 0;
 
     uint64_t launches = 0; uint32_t waves = 0, bounces_total = 0;
     std::vector<int> prof_kind; size_t prof_n = 0;            // kind: 0 raygen 1 extend 2 shade 3 connect 4 resolve
@@ -688,15 +677,16 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             CK(cudaMemcpyAsync(B.d_disp, B.h_disp, nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
             CK(cudaEventRecord(B.disp_ev, st));
             PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
-            if (!n_vol) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
+            if (!ds_.n_volumes) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
             const Queues q{ B.q_miss, B.q_hit, qcap };
             for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
-                const uint32_t wflags = (s == 0 && store_ok ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
-                if (camera) {
-                    CK((cudaError_t)launch_camera(lc_, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
-                                                  B.counts, q, d_ctr_, st, act));
-                } else launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
-                launches++; mark(0);
+                const uint32_t wflags = (s == 0 && cp.store ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
+                if (cp.camera) {
+                    CK(cudaMemsetAsync(B.counts, 0, CTRL_WORDS * sizeof(uint32_t), st));   // before any CTA appends to the parity-0 queues
+                    launches += launch_camera(lc_, cp, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
+                                              B.counts, q, d_ctr_, st, act);
+                } else launches += launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
+                mark(0);
                 int cur = 0; uint32_t k = 0;
                 for (;;) {
                     uint32_t chunk = 16;
@@ -704,11 +694,10 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     if (chunk == 0) break;
                     for (uint32_t b = 0; b < chunk; b++, k++) {
                         const uint32_t par = k & 1u, bflags = wflags | (k == 0 ? implied_flag : 0u);
-                        if (pre) { launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st); launches++; }
-                        if (!(camera && k == 0)) { launch_extend(lc_, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); launches++; } mark(1);
-                        launches += launch_shade(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_,
-                                                 fuse, cmask, bflags, st); mark(2);
-                        if (!fuse) { launch_connect(lc_, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); launches += lc_.trav_dyn ? 2 : 1; } mark(3);
+                        if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st);
+                        if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); mark(1);
+                        launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); mark(2);
+                        if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); mark(3);
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty

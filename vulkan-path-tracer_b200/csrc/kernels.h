@@ -18,15 +18,35 @@ struct LaunchCfg {
     bool wide;          // the dynamic-fetch kernels walk the BVH4 (DevScene::nodes4)
     int dyn_stack;      // shared-memory stack entries per thread of the dynamic-fetch kernels (BVH4: overflow goes to local memory)
     bool big;           // bvh_in_smem with a BVH > 64 KiB: one 512-thread CTA per SM for k_extend, k_camera, k_connect and the fused k_shade_hit
-    int extend_threads; // CTA size of k_extend (256, big: 512)
+    int extend_threads; // CTA size of k_extend / k_extend_dyn, k_camera and k_connect (256; big mode's one-ray-per-thread kernels: 512)
     int bounce_threads; // CTA size of the fused k_shade_hit (128, big: 512)
     int fuse;           // 0: k_shade_hit + k_connect; 1: NEE queries + path epilogue inside k_shade_hit (no k_connect)
     int grid_bounce;    // persistent grid of the fused k_shade_hit (BVH + stacks in shared memory)
     bool camera;        // camera rays generated and traced by k_camera (shared-memory BVH, one ray per thread) when the call has no pre-pass
     int grid_camera;    // persistent grid of k_camera (extend_threads per CTA)
+    int grid_features;  // persistent grid of k_features (256 threads per CTA)
+    // dynamic shared memory (traversal stacks + the staged BVH) of each launch shape
+    size_t smem_extend; // k_extend / k_extend_dyn, k_camera and the tracing k_connect (extend_threads per CTA)
+    size_t smem_shadow; // k_shadow_dyn (256 threads, + its ray ring)
+    size_t smem_bounce; // fused k_shade_hit (bounce_threads)
+    size_t smem_trace;  // k_trace_rays, k_volume_decide and k_features (256 threads)
 };
 
+// Grids, CTA sizes and shared memory of every traversal launch for one scene, and the per-device shared-memory opt-in of every kernel the
+// launchers can choose.  Runs on the engine's device before its first launch.
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc);
+// The choices of one Engine::path_trace call (plan_call), passed to the launchers.
+struct CallPlan {
+    bool pre;           // k_volume_decide + k_shade_volume run (volumes or atmosphere): DevScene::pre_pass
+    bool fuse;          // LaunchCfg::fuse without a pre-pass: no launch_connect
+    bool camera;        // LaunchCfg::camera without a pre-pass: launch_camera instead of launch_raygen + bounce 0's launch_extend
+    bool uniform;       // k_extend / k_camera skip the per-hit class lookup: one material class, no pre-pass
+    bool walks;         // k_connect<., ., true>: NEE transmittance walks (atmosphere or grid volumes)
+    uint32_t class_mask;   // k_shade_hit<CLASS> runs for every set bit
+    bool implied;       // bounce 0 may run with WAVE_IMPLIED
+    bool store;         // sub-wave 0 may run with WAVE_STORE
+};
+CallPlan plan_call(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, bool medium, uint32_t class_mask);
 // ---- per-launch flags of the ray-generation and shading launchers (Engine::path_trace sets them per sub-wave and bounce) ----
 // WAVE_IMPLIED: k_camera ran with ScreenSplitCount == 1 in a fused pipeline, so every camera path is inside the image.  k_camera writes
 //               only dir_rng, the hit record and the queue entry; bounce 0's k_shade_miss and fused k_shade_hit take throughput, depth,
@@ -35,14 +55,15 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
 //               a path end stores its radiance instead of adding it to the slot, and ray generation does not clear the slot.
 // WAVE_CARRY:   another sub-wave of the same frames follows: path ends store their RNG state to rng_carry for it.
 constexpr uint32_t WAVE_IMPLIED = 1u, WAVE_STORE = 2u, WAVE_CARRY = 4u;
+// The launchers below return the number of kernels they enqueued.
 // active (adaptive sampling): P is the active count and wave entry i of a dispatch traces local pixel active[i]; nullptr = every pixel
-void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
-                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active = nullptr);
-// launch_raygen + the camera rays' launch_extend in one kernel (LaunchCfg::camera, no pre-pass): clears the control block on `st`, writes the
-// path state, the hit records (hit_out) and the parity-0 queues.  Returns cudaError_t as int.
-int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr,
-                  cudaStream_t st, const uint32_t *active = nullptr);
+int launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active = nullptr);
+// launch_raygen + the camera rays' launch_extend in one kernel (CallPlan::camera): writes the path state, the hit records (hit_out) and the
+// parity-0 queues.  The control block must be zero when it starts.
+int launch_camera(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P,
+                  uint32_t first_sample, uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q,
+                  WaveCounters *ctr, cudaStream_t st, const uint32_t *active = nullptr);
 // ---- adaptive sampling: per local pixel one 16-B record {meanL, M2 (float bits), n_p, flags} (Engine::d_px_state_) ----
 constexpr uint32_t ADAPTIVE_TILE = 2048;      // pixels per block of the two compaction passes
 constexpr uint32_t PX_CONVERGED = 1u;         // flags bit: the pixel is never traced again
@@ -55,6 +76,8 @@ void launch_adaptive_update(uint4 *state, uint32_t npix, float threshold, uint32
                             uint32_t *active, uint32_t *active_count, cudaStream_t st);
 // ---- denoiser (denoise_kernels.cu) ----
 constexpr float DN_UNKNOWN_VARIANCE = 1e30f;  // variance of a pixel with fewer than two frames
+using FeaturesKernel = void (*)(DevScene, DevConfig, float3, uint32_t, uint32_t, int, float4 *, float4 *);
+FeaturesKernel features_kernel(bool smem);   // k_features<smem>
 // k_features over the local rows: albedo_cov = (mean albedo, hit fraction), normal_depth = (mean shading normal, mean view depth of the hits).
 // forward: unit view direction of the image centre; seed0 = PCG_HASH(0x46454154).  Returns cudaError_t as int.
 int launch_features(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, float3 forward, uint32_t samples, uint32_t seed0,
@@ -63,23 +86,22 @@ void launch_record_variance(const uint4 *state, uint32_t npix, float *variance, 
 // the a-trous filter on a W x H image (device buffers); scratch: 3 * W * H float4.  iterations == 0 copies color to out.
 void launch_denoise_filter(uint32_t W, uint32_t H, const float4 *color, const float4 *albedo_cov, const float4 *normal_depth, const float *variance,
                            uint32_t iterations, float sigma_l, float sigma_n, float sigma_z, float4 *scratch, float4 *out, cudaStream_t st);
-void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
-                   WaveCounters *ctr, bool primary, cudaStream_t st);
-// k_shade_miss + k_shade_hit<CLASS> for every class in class_mask (+ k_shade_volume); returns the number of kernels launched.
-// fuse != 0: the bounce is finished inside k_shade_hit (the survivors are written compacted to dst), launch_connect is not called.
-int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
-                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
-                 int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st);
-void launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
-                          float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st);   // before launch_extend when the scene has volumes or the atmosphere is on (DevScene::pre_pass)
-void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
-                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st);
+int launch_extend(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
+                  WaveCounters *ctr, bool primary, cudaStream_t st);
+// k_shade_miss + k_shade_hit<CLASS> for every class in cp.class_mask (+ k_shade_volume).
+// cp.fuse: the bounce is finished inside k_shade_hit (the survivors are written compacted to dst), launch_connect is not called.
+int launch_shade(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
+                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st);
+int launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
+                         float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st);   // before launch_extend when the call has a pre-pass (CallPlan::pre)
+int launch_connect(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
+                   uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st);
 void launch_resolve(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P,
                     const float4 *sample_buf, float4 *image, cudaStream_t st);
 void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const float *dir, const uint32_t *seeds, float ray_depth,
                          float *T_out, float *scatter_out, int32_t *vol_out, uint32_t *rng_out, cudaStream_t st);
-void launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
-                       float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st);
+int launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
+                      float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st);
 
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
 struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;

@@ -26,6 +26,7 @@
 #include "camera.cuh"
 #include "atmosphere.cuh"
 #include "kernels.h"
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1364,7 +1365,44 @@ __global__ void __launch_bounds__(256) k_trace_rays(DevScene sc, uint32_t n, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// host-callable launchers
+// kernel selectors: the instantiation each launch runs for its flags.  The launchers launch through them, and query_launch_cfg sizes the
+// grids of, checks big mode against and opts in the shared memory of exactly what they can return.
+// ------------------------------------------------------------------------------------------------
+static auto extend_kernel(bool smem, bool primary, bool uniform) {
+    const decltype(&k_extend<false, false, false>) fn[2][2][2] = {
+        { { k_extend<false, false, false>, k_extend<false, false, true> }, { k_extend<false, true, false>, k_extend<false, true, true> } },
+        { { k_extend<true, false, false>, k_extend<true, false, true> }, { k_extend<true, true, false>, k_extend<true, true, true> } } };
+    return fn[smem][primary][uniform];
+}
+static auto extend_dyn_kernel(bool smem, bool primary, bool wide) {        // the BVH4 is never staged in shared memory
+    if (wide) return primary ? k_extend_dyn<false, true, true> : k_extend_dyn<false, false, true>;
+    if (smem) return primary ? k_extend_dyn<true, true, false> : k_extend_dyn<true, false, false>;
+    return primary ? k_extend_dyn<false, true, false> : k_extend_dyn<false, false, false>;
+}
+static auto shadow_dyn_kernel(bool smem, bool wide) {
+    return wide ? k_shadow_dyn<false, true> : (smem ? k_shadow_dyn<true, false> : k_shadow_dyn<false, false>);
+}
+static auto camera_kernel(bool uniform, bool adaptive) {
+    return uniform ? (adaptive ? k_camera<true, true> : k_camera<true, false>) : (adaptive ? k_camera<false, true> : k_camera<false, false>);
+}
+static auto shade_kernel(uint32_t cls, bool vol, bool fuse) {              // the fused kernels run only without a pre-pass
+    const decltype(&k_shade_hit<MC_GENERAL, false, false>) fn[MC_COUNT][3] = {
+        { k_shade_hit<MC_DIFFUSE, false, false>, k_shade_hit<MC_DIFFUSE, true, false>, k_shade_hit<MC_DIFFUSE, false, true> },
+        { k_shade_hit<MC_METAL, false, false>, k_shade_hit<MC_METAL, true, false>, k_shade_hit<MC_METAL, false, true> },
+        { k_shade_hit<MC_GLASS, false, false>, k_shade_hit<MC_GLASS, true, false>, k_shade_hit<MC_GLASS, false, true> },
+        { k_shade_hit<MC_GENERAL, false, false>, k_shade_hit<MC_GENERAL, true, false>, k_shade_hit<MC_GENERAL, false, true> } };
+    return fn[cls][fuse ? 2 : (int)vol];
+}
+static auto connect_kernel(bool smem, bool trace, bool walks) {            // without tracing (behind k_shadow_dyn) the BVH is not read
+    if (!trace) return walks ? k_connect<false, false, true> : k_connect<false, false, false>;
+    if (smem) return walks ? k_connect<true, true, true> : k_connect<true, true, false>;
+    return walks ? k_connect<false, true, true> : k_connect<false, true, false>;
+}
+static auto volume_decide_kernel(bool smem) { return smem ? k_volume_decide<true> : k_volume_decide<false>; }
+static auto trace_rays_kernel(bool smem) { return smem ? k_trace_rays<true> : k_trace_rays<false>; }
+
+// ------------------------------------------------------------------------------------------------
+// launch configuration
 // ------------------------------------------------------------------------------------------------
 static constexpr size_t DYN_RING_BYTES_HOST = 8 * 128 * sizeof(uint32_t);
 static size_t trace_smem_bytes(const DevScene &sc, int max_stack, int threads, bool smem) {
@@ -1372,36 +1410,27 @@ static size_t trace_smem_bytes(const DevScene &sc, int max_stack, int threads, b
 }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) applies to the CURRENT device only, and the C-ABI lets one process drive several GPUs
-// (b200pt_create(device, ..)): the opt-in is tracked per device ordinal.
+// (b200pt_create(device, ..)): the opt-in is tracked per device ordinal.  It covers every flag combination of every selector.
 static unsigned long long g_attr_done_mask = 0ull;
-static int set_attrs_for_current_device() {
+static int opt_in_shared_memory() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return (int)cudaGetLastError();
     if (dev >= 0 && dev < 64 && ((g_attr_done_mask >> dev) & 1ull)) return 0;
-    // opt-in dynamic shared memory: the 227 KB per-CTA limit covers static + dynamic, so each kernel gets 227 KB minus its static part
+    // the 227 KB per-CTA limit covers static + dynamic, so each kernel gets 227 KB minus its static part
     int rc = 0;
-    auto optin = [&rc](const void *f) {
+    auto optin = [&rc](auto f) {
         cudaFuncAttributes a{};
         cudaError_t e = cudaFuncGetAttributes(&a, f);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)a.sharedSizeBytes);
         if (e != cudaSuccess && rc == 0) rc = (int)e;
     };
-#define B200PT_OPTIN_EXTEND(U) optin((const void *)k_extend<true, true, U>); optin((const void *)k_extend<true, false, U>); \
-                               optin((const void *)k_extend<false, true, U>); optin((const void *)k_extend<false, false, U>);
-    B200PT_OPTIN_EXTEND(true) B200PT_OPTIN_EXTEND(false)
-#undef B200PT_OPTIN_EXTEND
-    optin((const void *)k_camera<true, false>); optin((const void *)k_camera<false, false>);
-    optin((const void *)k_camera<true, true>); optin((const void *)k_camera<false, true>);
-    optin((const void *)k_connect<true, true>); optin((const void *)k_connect<false, true>); optin((const void *)k_connect<false, false>);
-    optin((const void *)k_connect<true, true, true>); optin((const void *)k_connect<false, true, true>); optin((const void *)k_connect<false, false, true>);
-    optin((const void *)k_extend_dyn<true, true, false>); optin((const void *)k_extend_dyn<true, false, false>);
-    optin((const void *)k_extend_dyn<false, true, false>); optin((const void *)k_extend_dyn<false, false, false>);
-    optin((const void *)k_extend_dyn<false, true, true>); optin((const void *)k_extend_dyn<false, false, true>);
-    optin((const void *)k_shadow_dyn<true, false>); optin((const void *)k_shadow_dyn<false, false>); optin((const void *)k_shadow_dyn<false, true>);
-    optin((const void *)k_trace_rays<true>); optin((const void *)k_trace_rays<false>);
-    optin((const void *)k_volume_decide<true>); optin((const void *)k_volume_decide<false>);
-    optin((const void *)k_shade_hit<MC_DIFFUSE, false, true>); optin((const void *)k_shade_hit<MC_METAL, false, true>);
-    optin((const void *)k_shade_hit<MC_GLASS, false, true>); optin((const void *)k_shade_hit<MC_GENERAL, false, true>);
+    for (int f = 0; f < 8; f++) {
+        const bool a = f & 1, b = f & 2, c = f & 4;
+        optin(extend_kernel(a, b, c)); optin(extend_dyn_kernel(a, b, c)); optin(connect_kernel(a, b, c));
+        optin(shadow_dyn_kernel(a, b)); optin(camera_kernel(a, b));
+        optin(volume_decide_kernel(a)); optin(trace_rays_kernel(a)); optin(features_kernel(a));
+        for (uint32_t cls = 0; cls < MC_COUNT; cls++) optin(shade_kernel(cls, a, b));
+    }
     cudaGetLastError();
     if (rc == 0 && dev >= 0 && dev < 64) g_attr_done_mask |= 1ull << dev;
     return rc;
@@ -1409,7 +1438,7 @@ static int set_attrs_for_current_device() {
 
 // grid sizing: persistent grids = SM count x resident CTAs per SM for the chosen shared-memory footprint
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc) {
-    { const int a = set_attrs_for_current_device(); if (a != 0) return a; }
+    { const int a = opt_in_shared_memory(); if (a != 0) return a; }
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceProp prop; cudaError_t e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) return (int)e;
@@ -1426,34 +1455,26 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     if (const char *e = getenv("B200PT_SMEM_BIG")) {
         if (atoi(e) == 1 && aligned && !fits_small) {
             const size_t need = trace_smem_bytes(sc, lc->max_stack, 512, true);
-            const void *const big_kernels[] = {
-                (const void *)k_extend<true, true, true>, (const void *)k_extend<true, true, false>, (const void *)k_extend<true, false, true>, (const void *)k_extend<true, false, false>,
-                (const void *)k_camera<true, true>, (const void *)k_camera<true, false>, (const void *)k_camera<false, true>, (const void *)k_camera<false, false>,
-                (const void *)k_connect<true, true>, (const void *)k_connect<true, true, true>,
-                (const void *)k_shade_hit<MC_DIFFUSE, false, true>, (const void *)k_shade_hit<MC_METAL, false, true>,
-                (const void *)k_shade_hit<MC_GLASS, false, true>, (const void *)k_shade_hit<MC_GENERAL, false, true> };
             fits_big = true;
-            for (const void *f : big_kernels) {
-                cudaFuncAttributes a{};
-                if (cudaFuncGetAttributes(&a, f) != cudaSuccess || need + a.sharedSizeBytes > 227u * 1024u) fits_big = false;
+            auto fits = [&](auto f) { cudaFuncAttributes a{}; if (cudaFuncGetAttributes(&a, f) != cudaSuccess || need + a.sharedSizeBytes > 227u * 1024u) fits_big = false; };
+            for (int f = 0; f < 4; f++) {                                   // f: two flags, or the material class
+                const bool a = f & 1, b = f & 2;
+                fits(extend_kernel(true, a, b)); fits(camera_kernel(a, b)); fits(connect_kernel(true, true, a)); fits(shade_kernel(f, false, true));
             }
         }
     }
     lc->bvh_in_smem = fits_small || fits_big;
     lc->big = fits_big;
-    lc->extend_threads = fits_big ? 512 : 256;
-    lc->bounce_threads = fits_big ? 512 : 128;
-    const size_t sh = trace_smem_bytes(sc, lc->max_stack, lc->extend_threads, lc->bvh_in_smem);
-    const size_t sh256 = trace_smem_bytes(sc, lc->max_stack, 256, lc->bvh_in_smem);
+    const bool smem = lc->bvh_in_smem;
     // traversal shape: dynamic-fetch while-while kernels (bvh_dynfetch.cuh) over the BVH4 when the BVH lives in L2/HBM, one ray per thread
     // over the BVH2 when the whole BVH sits in shared memory (tiny scenes: no divergence or latency to recover).
     // Overrides: B200PT_TRAV=classic|dyn, B200PT_WIDE=0|1, B200PT_DYN_THRESH=1..32, B200PT_WIDE_STACK=<shared-memory stack entries>.
-    lc->trav_dyn = !lc->bvh_in_smem;
+    lc->trav_dyn = !smem;
     if (const char *e = getenv("B200PT_TRAV")) { if (!strcmp(e, "dyn")) lc->trav_dyn = true; else if (!strcmp(e, "classic")) lc->trav_dyn = false; }
     lc->dyn_thresh = 20;
     if (const char *e = getenv("B200PT_DYN_THRESH")) { int v = atoi(e); if (v >= 1 && v <= 32) lc->dyn_thresh = v; }
-    lc->wide = lc->trav_dyn && !lc->bvh_in_smem && sc.nodes4 != nullptr && sc.bvh_bytes >= (8u << 20);   // small BVHs stay L1/L2-hot: BVH2 is cheaper there
-    if (const char *e = getenv("B200PT_WIDE")) { if (atoi(e) == 1 && lc->trav_dyn && !lc->bvh_in_smem && sc.nodes4 != nullptr) lc->wide = true; }
+    lc->wide = lc->trav_dyn && !smem && sc.nodes4 != nullptr && sc.bvh_bytes >= (8u << 20);   // small BVHs stay L1/L2-hot: BVH2 is cheaper there
+    if (const char *e = getenv("B200PT_WIDE")) { if (atoi(e) == 1 && lc->trav_dyn && !smem && sc.nodes4 != nullptr) lc->wide = true; }
     if (const char *e = getenv("B200PT_WIDE")) { if (atoi(e) == 0) lc->wide = false; }
     lc->dyn_stack = lc->max_stack;                                          // BVH2: depth + 2 entries always suffice
     if (lc->wide) {
@@ -1467,79 +1488,84 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     //   1 (default): k_shade_hit<., ., true> traces each NEE query the moment it is built and finishes the path (roulette, radiance, compaction)
     //      in the same thread; the next segment's closest hit runs in k_extend<true, false, .>.
     // B200PT_FUSE=0 overrides (k_extend + k_shade_hit + k_connect); any other value keeps the default.
-    lc->fuse = (lc->bvh_in_smem && !lc->trav_dyn) ? 1 : 0;
-    if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if ((v == 0 || v == 1) && lc->bvh_in_smem && !lc->trav_dyn) lc->fuse = v; }
+    lc->fuse = (smem && !lc->trav_dyn) ? 1 : 0;
+    if (const char *e = getenv("B200PT_FUSE")) { const int v = atoi(e); if ((v == 0 || v == 1) && smem && !lc->trav_dyn) lc->fuse = v; }
     // Camera rays of those scenes: generated and traced in one kernel (k_camera) instead of k_raygen + k_extend<true, true, .>, unless the scene
-    // needs a pre-pass (decided per call: Engine::path_trace).  B200PT_CAMERA=0 keeps the pair.
-    lc->camera = lc->bvh_in_smem && !lc->trav_dyn;
+    // needs a pre-pass (decided per call: plan_call).  B200PT_CAMERA=0 keeps the pair.
+    lc->camera = smem && !lc->trav_dyn;
     if (const char *e = getenv("B200PT_CAMERA")) { if (atoi(e) == 0) lc->camera = false; }
-    const size_t sh_dyn = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, lc->bvh_in_smem);
-    int occ_e = 0, occ_c = 0, occ_s = 0, occ_sh = 0, occ_b = 0;
+
+    // CTA sizes and dynamic shared memory of each launch shape; the dynamic-fetch kernels always run 256-thread CTAs
+    lc->extend_threads = fits_big && !lc->trav_dyn ? 512 : 256;
+    lc->bounce_threads = fits_big ? 512 : 128;
+    lc->smem_extend = trace_smem_bytes(sc, lc->trav_dyn ? lc->dyn_stack + 1 : lc->max_stack, lc->extend_threads, smem);
+    lc->smem_shadow = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, smem) + DYN_RING_BYTES_HOST;
+    lc->smem_bounce = trace_smem_bytes(sc, lc->max_stack, lc->bounce_threads, true);
+    lc->smem_trace = trace_smem_bytes(sc, lc->max_stack, 256, smem);
+    auto occupancy = [](auto fn, int threads, size_t smem_bytes) { int n = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, threads, smem_bytes); return n; };
+    int occ_e = 0, occ_c = 0, occ_sh = 0;
     if (lc->trav_dyn) {
-        if (lc->wide) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend_dyn<false, false, true>, 256, sh_dyn);
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_sh, k_shadow_dyn<false, true>, 256, sh_dyn + DYN_RING_BYTES_HOST);
-        } else if (lc->bvh_in_smem) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend_dyn<true, false, false>, 256, sh_dyn);
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_sh, k_shadow_dyn<true, false>, 256, sh_dyn + DYN_RING_BYTES_HOST);
-        } else {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend_dyn<false, false, false>, 256, sh_dyn);
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_sh, k_shadow_dyn<false, false>, 256, sh_dyn + DYN_RING_BYTES_HOST);
-        }
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<false, false>, 256, 0);
-    } else if (lc->bvh_in_smem) {
-        int occ_u = 0;                                                      // one grid for both tally forms: the smaller residency
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<true, false, false>, lc->extend_threads, sh);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_extend<true, false, true>, lc->extend_threads, sh);
-        if (occ_u < occ_e) occ_e = occ_u;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<true, true>, lc->extend_threads, sh);
+        occ_e = occupancy(extend_dyn_kernel(smem, false, lc->wide), lc->extend_threads, lc->smem_extend);
+        occ_sh = occupancy(shadow_dyn_kernel(smem, lc->wide), 256, lc->smem_shadow);
+        occ_c = occupancy(connect_kernel(smem, false, false), lc->extend_threads, 0);
     } else {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_extend<false, false, false>, 256, sh);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_connect<false, true>, 256, sh);
+        occ_e = occupancy(extend_kernel(smem, false, false), lc->extend_threads, lc->smem_extend);
+        if (smem) occ_e = std::min(occ_e, occupancy(extend_kernel(true, false, true), lc->extend_threads, lc->smem_extend));   // one grid for both tally forms: the smaller residency
+        occ_c = occupancy(connect_kernel(smem, true, false), lc->extend_threads, lc->smem_extend);
     }
-    if (occ_sh < 1) occ_sh = 1;
-    lc->grid_shadow = sms * occ_sh;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_shade_hit<MC_GENERAL, false, false>, 128, 0);
-    if (lc->bvh_in_smem) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_shade_hit<MC_GENERAL, false, true>, lc->bounce_threads,
-                                                                       trace_smem_bytes(sc, lc->max_stack, lc->bounce_threads, true));
-    if (occ_e < 1) occ_e = 1; if (occ_c < 1) occ_c = 1; if (occ_s < 1) occ_s = 1; if (occ_b < 1) occ_b = 1;
-    lc->grid_extend = sms * occ_e; lc->grid_connect = sms * occ_c;
-    { int occ_t = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, lc->bvh_in_smem ? k_trace_rays<true> : k_trace_rays<false>, 256, sh256); lc->grid_trace = sms * (occ_t < 1 ? 1 : occ_t); }
+    // every unfused k_shade_hit runs on the grid of the general one, every fused one on the grid of the fused general one
+    const int occ_s = std::max(1, occupancy(shade_kernel(MC_GENERAL, false, false), 128, 0));
+    const int occ_b = std::max(1, smem ? occupancy(shade_kernel(MC_GENERAL, false, true), lc->bounce_threads, lc->smem_bounce) : 0);
+    int occ_cam = 0;                                                        // both camera forms on one grid: the smaller residency
+    if (lc->camera) occ_cam = std::min(occupancy(camera_kernel(false, false), lc->extend_threads, lc->smem_extend),
+                                       occupancy(camera_kernel(true, false), lc->extend_threads, lc->smem_extend));
+    occ_e = std::max(1, occ_e); occ_c = std::max(1, occ_c); occ_sh = std::max(1, occ_sh);
+    lc->grid_extend = sms * occ_e; lc->grid_connect = sms * occ_c; lc->grid_shadow = sms * occ_sh;
     lc->grid_shade = sms * occ_s;
     lc->grid_bounce = sms * occ_b;
-    int occ_cam = 0;
-    if (lc->camera) {
-        int occ_u = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_cam, k_camera<false, false>, lc->extend_threads, sh);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_u, k_camera<true, false>, lc->extend_threads, sh);
-        if (occ_u < occ_cam) occ_cam = occ_u;
-    }
-    lc->grid_camera = sms * (occ_cam < 1 ? 1 : occ_cam);
+    lc->grid_camera = sms * std::max(1, occ_cam);
+    lc->grid_trace = sms * std::max(1, occupancy(trace_rays_kernel(smem), 256, lc->smem_trace));   // k_volume_decide runs on it too
+    lc->grid_features = sms * std::max(1, occupancy(features_kernel(smem), 256, lc->smem_trace));
     lc->grid_light = sms * 8;
     if (getenv("B200PT_DEBUG"))
         fprintf(stderr, "[b200pt] launch cfg: bvh depth %d (bvh4 %d) max_stack %d dyn_stack %d bvh_bytes %u smem %d dyn %d wide %d thresh %d fuse %d big %d camera %d | CTAs/SM extend %d connect %d shadow %d shade %d bounce %d camera %d\n",
-                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)lc->bvh_in_smem, (int)lc->trav_dyn, (int)lc->wide, lc->dyn_thresh, lc->fuse, (int)lc->big, (int)lc->camera,
+                bvh_max_depth, bvh4_depth, lc->max_stack, lc->dyn_stack, sc.bvh_bytes, (int)smem, (int)lc->trav_dyn, (int)lc->wide, lc->dyn_thresh, lc->fuse, (int)lc->big, (int)lc->camera,
                 occ_e, occ_c, occ_sh, occ_s, occ_b, occ_cam);
     return 0;
 }
 
-void launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
-                   const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active) {
+CallPlan plan_call(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, bool medium, uint32_t class_mask) {
+    CallPlan cp;
+    cp.pre = sc.n_volumes != 0u || cfg.EnableAtmosphere != 0u;              // volumes and / or the atmosphere (csrc/atmosphere.cuh)
+    cp.fuse = lc.fuse != 0 && !cp.pre;                                      // the fused shading kernels need the BVH in shared memory and no volumes
+    cp.camera = lc.camera && !cp.pre;
+    cp.uniform = sc.uniform_class != 0xFFu && !cp.pre;
+    cp.walks = cfg.EnableAtmosphere != 0u || sc.n_grids != 0u;
+    cp.class_mask = cp.pre ? (class_mask | (1u << MC_GENERAL)) : class_mask;   // volume / atmosphere events ride in the general queue
+    // WAVE_IMPLIED: k_camera's paths are all inside the image only without chunked dispatch (overhang paths are born dead and keep their full
+    // state), and only the fused shading kernels infer the state.  WAVE_STORE: sub-wave 0 ends every path exactly once when the bounce loop
+    // provably runs dry -- not with a pre-pass (DEAD_EVENT ends, channel-split paths), not with medium walks (the runaway guard may stop them),
+    // not at MaxDepth 0 (no bounce runs, the slots must read zero).
+    cp.implied = cp.camera && cfg.ScreenSplitCount == 1u && cp.fuse;
+    cp.store = !cp.pre && !medium && cfg.MaxDepth > 0u;
+    return cp;
+}
+
+// ------------------------------------------------------------------------------------------------
+// host-callable launchers
+// ------------------------------------------------------------------------------------------------
+int launch_raygen(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample, uint32_t flags,
+                  const uint32_t *rng_carry, PathState ps, float4 *sample_buf, uint32_t *ctrl, WaveCounters *ctr, cudaStream_t st, const uint32_t *active) {
     if (active) k_raygen<true><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, ctrl, ctr, active);
     else k_raygen<false><<<lc.grid_light, 256, 0, st>>>(cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, ctrl, ctr, nullptr);
+    return 1;
 }
-int launch_camera(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P, uint32_t first_sample,
-                  uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q, WaveCounters *ctr,
-                  cudaStream_t st, const uint32_t *active) {
-    set_attrs_for_current_device();
-    const cudaError_t e = cudaMemsetAsync(ctrl, 0, CTRL_WORDS * sizeof(uint32_t), st);   // before any CTA appends to the parity-0 queues
-    if (e != cudaSuccess) return (int)e;
-    const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, true);
-#define B200PT_CAM(U, A) k_camera<U, A><<<lc.grid_camera, lc.extend_threads, sh, st>>>(sc, cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps, sample_buf, hit_out, ctrl, q, lc.max_stack, ctr, active)
-    if (sc.uniform_class != 0xFFu) { if (active) B200PT_CAM(true, true); else B200PT_CAM(true, false); }
-    else { if (active) B200PT_CAM(false, true); else B200PT_CAM(false, false); }
-#undef B200PT_CAM
-    return 0;
+int launch_camera(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P,
+                  uint32_t first_sample, uint32_t flags, const uint32_t *rng_carry, PathState ps, float4 *sample_buf, float4 *hit_out, uint32_t *ctrl, Queues q,
+                  WaveCounters *ctr, cudaStream_t st, const uint32_t *active) {
+    camera_kernel(cp.uniform, active != nullptr)<<<lc.grid_camera, lc.extend_threads, lc.smem_extend, st>>>(sc, cfg, disp, n_disp, P, first_sample, flags, rng_carry, ps,
+                                                                                                           sample_buf, hit_out, ctrl, q, lc.max_stack, ctr, active);
+    return 1;
 }
 void launch_resolve_adaptive(const LaunchCfg &lc, const DevConfig &cfg, uint32_t n_disp, uint32_t A, const uint32_t *active,
                              const float4 *sample_buf, float4 *image, uint4 *state, cudaStream_t st) {
@@ -1552,73 +1578,42 @@ void launch_adaptive_update(uint4 *state, uint32_t npix, float threshold, uint32
     k_adaptive_update<<<tiles, 256, 0, st>>>(state, npix, threshold, min_samples, decide ? 1u : 0u, tile_count);
     k_adaptive_compact<<<tiles, 256, 0, st>>>(state, npix, tile_count, active, active_count);
 }
-void launch_extend(const LaunchCfg &lc, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
-                   WaveCounters *ctr, bool primary, cudaStream_t st) {
-    set_attrs_for_current_device();
-    const bool smem = lc.bvh_in_smem;
-    if (lc.trav_dyn) {
-        const size_t sh = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem);
-#define B200PT_EXT_DYN(S, P, W) k_extend_dyn<S, P, W><<<lc.grid_extend, 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr)
-        if (lc.wide) { if (primary) B200PT_EXT_DYN(false, true, true); else B200PT_EXT_DYN(false, false, true); }
-        else if (smem) { if (primary) B200PT_EXT_DYN(true, true, false); else B200PT_EXT_DYN(true, false, false); }
-        else { if (primary) B200PT_EXT_DYN(false, true, false); else B200PT_EXT_DYN(false, false, false); }
-#undef B200PT_EXT_DYN
-        return;
-    }
-    const size_t sh = trace_smem_bytes(sc, lc.max_stack, lc.extend_threads, smem);
-    const bool uniform = sc.uniform_class != 0xFFu && sc.pre_pass == 0u;
-#define B200PT_EXT(S, P, U) k_extend<S, P, U><<<lc.grid_extend, S ? lc.extend_threads : 256, sh, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr)
-#define B200PT_EXT_U(S, P) do { if (uniform) B200PT_EXT(S, P, true); else B200PT_EXT(S, P, false); } while (0)
-    if (smem) { if (primary) B200PT_EXT_U(true, true); else B200PT_EXT_U(true, false); }
-    else { if (primary) B200PT_EXT_U(false, true); else B200PT_EXT_U(false, false); }
-#undef B200PT_EXT_U
-#undef B200PT_EXT
+int launch_extend(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, PathState ps, float4 *hit_out, uint32_t *ctrl, uint32_t parity, Queues q,
+                  WaveCounters *ctr, bool primary, cudaStream_t st) {
+    if (lc.trav_dyn)
+        extend_dyn_kernel(lc.bvh_in_smem, primary, lc.wide)<<<lc.grid_extend, lc.extend_threads, lc.smem_extend, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr);
+    else extend_kernel(lc.bvh_in_smem, primary, cp.uniform)<<<lc.grid_extend, lc.extend_threads, lc.smem_extend, st>>>(sc, ps, hit_out, ctrl, parity, q, lc.max_stack, ctr);
+    return 1;
 }
-// k_shade_miss + one k_shade_hit<CLASS> per material class present in the scene (+ k_shade_volume).  fuse (0 / 1): see k_shade_hit.
-// Returns the number of kernels launched.
-int launch_shade(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
-                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr,
-                 int fuse, uint32_t class_mask, uint32_t flags, cudaStream_t st) {
-    set_attrs_for_current_device();
+// k_shade_miss + one k_shade_hit<CLASS> per material class of the call (+ k_shade_volume).  cp.fuse: see k_shade_hit.
+int launch_shade(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, PathState ps, PathState dst, ShadeOut so, const float4 *hit_in,
+                 uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st) {
     int launched = 1;
     k_shade_miss<<<lc.grid_light, 256, 0, st>>>(sc, cfg, ps, ctrl, parity, q.miss, sample_buf, rng_carry, ctr, flags);
-    const size_t shb = trace_smem_bytes(sc, lc.max_stack, lc.bounce_threads, true);
-#define B200PT_SHADE(C) do { if (class_mask & (1u << C)) { launched++;                                                                                              \
-        if (fuse) k_shade_hit<C, false, true><<<lc.grid_bounce, lc.bounce_threads, shb, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags); \
-        else if (sc.pre_pass) k_shade_hit<C, true, false><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);       \
-        else k_shade_hit<C, false, false><<<lc.grid_shade, 128, 0, st>>>(sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags); } } while (0)
-    B200PT_SHADE(MC_DIFFUSE); B200PT_SHADE(MC_METAL); B200PT_SHADE(MC_GLASS); B200PT_SHADE(MC_GENERAL);
-#undef B200PT_SHADE
-    if (sc.pre_pass) { launched++; k_shade_volume<<<lc.grid_light, 128, 0, st>>>(sc, cfg, ps, so, ctrl, parity, q, ctr); }
+    for (uint32_t c = 0; c < MC_COUNT; c++) {
+        if (!(cp.class_mask & (1u << c))) continue;
+        launched++;
+        shade_kernel(c, cp.pre, cp.fuse)<<<cp.fuse ? lc.grid_bounce : lc.grid_shade, cp.fuse ? lc.bounce_threads : 128, cp.fuse ? lc.smem_bounce : 0, st>>>(
+            sc, cfg, ps, dst, so, hit_in, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
+    }
+    if (cp.pre) { launched++; k_shade_volume<<<lc.grid_light, 128, 0, st>>>(sc, cfg, ps, so, ctrl, parity, q, ctr); }
     return launched;
 }
-void launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
-                          float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st) {
-    set_attrs_for_current_device();
-    const bool smem = lc.bvh_in_smem;
-    const size_t sh = trace_smem_bytes(sc, lc.max_stack, 256, smem);
-    if (smem) k_volume_decide<true><<<lc.grid_trace, 256, sh, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
-    else k_volume_decide<false><<<lc.grid_trace, 256, sh, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
+int launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
+                         float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st) {
+    volume_decide_kernel(lc.bvh_in_smem)<<<lc.grid_trace, 256, lc.smem_trace, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
+    return 1;
 }
-void launch_connect(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
-                    uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st) {
-    set_attrs_for_current_device();
-    const bool smem = lc.bvh_in_smem;
-    const bool walks = cfg.EnableAtmosphere != 0u || sc.n_grids != 0u;      // k_connect<.., WALKS>
+int launch_connect(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
+                   uint32_t *ctrl, uint32_t parity, Queues q, float4 *sample_buf, uint32_t *rng_carry, WaveCounters *ctr, uint32_t flags, cudaStream_t st) {
+    int launched = 1;
     if (lc.trav_dyn) {                                                      // shadow rays in their own dynamic-fetch kernel, then the join without tracing
-        const size_t shd = trace_smem_bytes(sc, lc.dyn_stack + 1, 256, smem) + DYN_RING_BYTES_HOST;
-#define B200PT_SH_DYN(S, W) k_shadow_dyn<S, W><<<lc.grid_shadow, 256, shd, st>>>(sc, so, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr)
-        if (lc.wide) B200PT_SH_DYN(false, true); else if (smem) B200PT_SH_DYN(true, false); else B200PT_SH_DYN(false, false);
-#undef B200PT_SH_DYN
-        if (walks) k_connect<false, false, true><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
-        else k_connect<false, false><<<lc.grid_connect, 256, 0, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
-        return;
+        shadow_dyn_kernel(lc.bvh_in_smem, lc.wide)<<<lc.grid_shadow, 256, lc.smem_shadow, st>>>(sc, so, ctrl, parity, q, lc.dyn_stack, lc.dyn_thresh, ctr);
+        launched++;
     }
-    const size_t sh = trace_smem_bytes(sc, lc.max_stack, smem ? lc.extend_threads : 256, smem);
-#define B200PT_CONNECT(S, W, T) k_connect<S, true, W><<<lc.grid_connect, T, sh, st>>>(sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags)
-    if (smem) { if (walks) B200PT_CONNECT(true, true, lc.extend_threads); else B200PT_CONNECT(true, false, lc.extend_threads); }
-    else { if (walks) B200PT_CONNECT(false, true, 256); else B200PT_CONNECT(false, false, 256); }
-#undef B200PT_CONNECT
+    connect_kernel(lc.bvh_in_smem, !lc.trav_dyn, cp.walks)<<<lc.grid_connect, lc.extend_threads, lc.trav_dyn ? 0 : lc.smem_extend, st>>>(
+        sc, cfg, src, dst, so, ctrl, parity, q, sample_buf, rng_carry, lc.max_stack, ctr, flags);
+    return launched;
 }
 void launch_resolve(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch *disp, uint32_t n_disp, uint32_t P,
                     const float4 *sample_buf, float4 *image, cudaStream_t st) {
@@ -1628,13 +1623,10 @@ void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const
                          float *T_out, float *scatter_out, int32_t *vol_out, uint32_t *rng_out, cudaStream_t st) {
     k_volume_walks<<<(n + 127u) / 128u, 128, 0, st>>>(sc, n, org, dir, seeds, ray_depth, T_out, scatter_out, vol_out, rng_out);
 }
-void launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
-                       float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st) {
-    set_attrs_for_current_device();
-    const bool smem = lc.bvh_in_smem;
-    const size_t sh = trace_smem_bytes(sc, lc.max_stack, 256, smem);
-    if (smem) k_trace_rays<true><<<lc.grid_trace, 256, sh, st>>>(sc, n, org, dir, tmin, tmax, t_out, prim_out, inst_out, uv_out, lc.max_stack, stats);
-    else k_trace_rays<false><<<lc.grid_trace, 256, sh, st>>>(sc, n, org, dir, tmin, tmax, t_out, prim_out, inst_out, uv_out, lc.max_stack, stats);
+int launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
+                      float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st) {
+    trace_rays_kernel(lc.bvh_in_smem)<<<lc.grid_trace, 256, lc.smem_trace, st>>>(sc, n, org, dir, tmin, tmax, t_out, prim_out, inst_out, uv_out, lc.max_stack, stats);
+    return 1;
 }
 
 } // namespace b200pt
