@@ -323,6 +323,32 @@ int32_t b200pt_volume_walks(b200pt_handle h, uint32_t n, const float *origins3, 
                             float *out_T, float *out_scatter, int32_t *out_volume, uint32_t *out_rng2);
 /* traversal cost of the same query: nodes_tris_out[2*i] = BVH nodes visited, [2*i+1] = triangles tested (measurement hook) */
 int32_t b200pt_trace_stats(b200pt_handle h, uint32_t n, const float *origins3, const float *directions3, float tmin, float tmax, uint32_t *nodes_tris_out);
+/* Traversal test hook: ray i (per-ray tmin[i] < t < tmax[i]) through one traversal shape the renderer can launch and one query kind.
+ * shape: B200PT_TRAV_SHARED / _GLOBAL: BVH2 stack walk, one ray per thread, BVH staged in shared memory / read from global memory;
+ *        _FLAT: the slot-by-slot walk of scenes of at most B200PT_FLAT_MAX triangles; _FIXED_ORIGIN: the same with every ray starting at
+ *        origins3[0] (the camera kernel's table; closest-hit only); _DYN2 / _DYN4: the dynamic-fetch kernels over the BVH2 / the BVH4;
+ *        _DYN4_SPILL: the BVH4 with a 4-entry shared-memory stack, so the local-memory overflow stack carries the walk.
+ * kind:  B200PT_QUERY_CLOSEST: t_out (-1 on a miss), prim_out / inst_out (0xFFFFFFFF on a miss), uv_out2;
+ *        B200PT_QUERY_ANY: occluded_out[i] = 1 when some triangle has tmin < t < tmax;
+ *        B200PT_QUERY_TARGET: light visibility: a triangle occludes when t < tmax, or when t == tmax and its id (instance-major triangle
+ *        index) is below target_gid[i]; tmax_test[i] >= 0 is the acceptance bound of the triangle test (the fused shading kernel passes
+ *        nextafter(tmax) for light rays and tmax for sky rays), < 0 takes nextafter(tmax).
+ * fma_slabs != 0: the one-FMA slab form of secondary rays instead of subtract-then-multiply.
+ * stats3_out (optional): [3*i] nodes visited, [3*i+1] triangles tested, [3*i+2] pushes refused by a full stack.
+ * B200PT_ERR_WRONG_ARGUMENTS when the scene has no such shape (no flat walk, no BVH4, BVH too big for shared memory). */
+#define B200PT_TRAV_SHARED       0
+#define B200PT_TRAV_GLOBAL       1
+#define B200PT_TRAV_FLAT         2
+#define B200PT_TRAV_FIXED_ORIGIN 3
+#define B200PT_TRAV_DYN2         4
+#define B200PT_TRAV_DYN4         5
+#define B200PT_TRAV_DYN4_SPILL   6
+#define B200PT_QUERY_CLOSEST     0
+#define B200PT_QUERY_ANY         1
+#define B200PT_QUERY_TARGET      2
+int32_t b200pt_trace_query(b200pt_handle h, int32_t shape, int32_t kind, int32_t fma_slabs, uint32_t n, const float *origins3, const float *directions3,
+                           const float *tmin, const float *tmax, const uint32_t *target_gid, const float *tmax_test,
+                           float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out2, uint32_t *occluded_out, uint32_t *stats3_out);
 
 /* Energy-compensation lookup-table baker (SURVEY.md 8f row 2).
  * Replaces LookupTableCalculator::CalculateTable(tableSize, sampleCount) (PathTracer/LookupTableCalculator.h:8,

@@ -47,4 +47,16 @@ def _denoise(name, **kw):                                           # per-pixel 
 _denoise("cornell_box"); _denoise("cornell_box_glass")
 run("cornell_box_glass", 48, 48, 2, 8)                              # dynamic-fetch BVH2 kernels, class queues (glass / diffuse)
 os.environ["B200PT_WIDE"] = "1"; run("viking_room", 48, 48, 1, 4); del os.environ["B200PT_WIDE"]              # BVH4 + textures
+def _queries(name):                                                 # b200pt_trace_query: every shape the scene has, every query kind, with and without stats
+    import vpt_b200 as pt
+    T = util.product_tracer(name, 16, 16)
+    rng = np.random.default_rng(1)
+    o = (rng.random((300, 3)) * 6 - 3).astype(np.float32); d = rng.normal(size=(300, 3)).astype(np.float32)
+    for shape in pt.PathTracer.TRAV_SHAPES:
+        for kind in ("closest", "any", "target"):
+            for stats in (True, False):
+                try: T.trace_query(shape, kind, o, d, 1e-4, 1e6, target=np.arange(300) % 7, fma=kind != "closest", stats=stats)
+                except pt.B200ptError: pass                             # shape absent in this scene (flat walk, BVH4, shared memory)
+    print(name, "trace_query ok")
+_queries("cornell_box"); _queries("viking_room")
 print("sanitize_small done")

@@ -188,6 +188,7 @@ def lib():
             "b200pt_trace_closest": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
             "b200pt_scene_stats": [C.c_void_p] + [C.POINTER(C.c_uint32)] * 4,
             "b200pt_trace_stats": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p],
+            "b200pt_trace_query": [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32] + [C.c_void_p] * 12,
             "b200pt_bake_lut": [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p],
             "b200pt_bake_luts_to_dir": [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32],
             "b200pt_decode_image_file": [C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_void_p)],
@@ -662,6 +663,26 @@ class PathTracer:
         st = np.zeros((n, 2), np.uint32)
         self._ck(self.L.b200pt_trace_stats(self.h, n, _p(org), _p(dirs), C.c_float(tmin), C.c_float(tmax), _p(st)))
         return st
+
+    TRAV_SHAPES = {"shared": 0, "global": 1, "flat": 2, "fixed_origin": 3, "dyn2": 4, "dyn4": 5, "dyn4_spill": 6}   # B200PT_TRAV_*
+    QUERY_KINDS = {"closest": 0, "any": 1, "target": 2}                                                            # B200PT_QUERY_*
+
+    def trace_query(self, shape, kind, org, dirs, tmin, tmax, target=None, tmax_test=None, fma=False, stats=True):
+        """b200pt_trace_query: per-ray tmin / tmax (scalars broadcast).  Returns a dict: closest -> t, prim, inst, uv; any / target ->
+        occluded (bool); stats [n, 3] (nodes visited, triangles tested, refused pushes) from the counting instantiations, or None with
+        stats=False (the renderer's own instantiations)."""
+        org = np.ascontiguousarray(org, np.float32).reshape(-1, 3); dirs = np.ascontiguousarray(dirs, np.float32).reshape(-1, 3); n = len(org)
+        lo = np.ascontiguousarray(np.broadcast_to(np.float32(tmin) if np.isscalar(tmin) else np.asarray(tmin, np.float32), (n,)))
+        hi = np.ascontiguousarray(np.broadcast_to(np.float32(tmax) if np.isscalar(tmax) else np.asarray(tmax, np.float32), (n,)))
+        k = self.QUERY_KINDS[kind]
+        tg = np.ascontiguousarray(np.broadcast_to(np.asarray(0xFFFFFFFF if target is None else target, np.uint32), (n,)))
+        tt = np.ascontiguousarray(np.broadcast_to(np.asarray(-1.0 if tmax_test is None else tmax_test, np.float32), (n,)))
+        t = np.zeros(n, np.float32); prim = np.zeros(n, np.uint32); inst = np.zeros(n, np.uint32); uv = np.zeros((n, 2), np.float32)
+        occ = np.zeros(n, np.uint32); st = np.zeros((n, 3), np.uint32) if stats else None
+        self._ck(self.L.b200pt_trace_query(self.h, self.TRAV_SHAPES[shape], k, int(bool(fma)), n, _p(org), _p(dirs), _p(lo), _p(hi), _p(tg), _p(tt),
+                                           _p(t), _p(prim), _p(inst), _p(uv), _p(occ), _p(st) if stats else None))
+        if k == 0: return dict(t=t, prim=prim, inst=inst, uv=uv, stats=st)
+        return dict(occluded=occ.astype(bool), stats=st)
 
     def scene_stats(self):
         a, b, c, d = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()

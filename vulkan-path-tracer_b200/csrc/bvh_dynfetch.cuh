@@ -44,8 +44,10 @@ __device__ __forceinline__ void dyn_pop(DynRay &r, uint32_t s_step) {
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r.cur) : "r"(r.s_top) : "memory");
 }
 
-template <bool SMEM, bool FMA_SLABS>
-__device__ __forceinline__ void dyn_node_step(const BvhView &b, DynRay &r, uint32_t s_step, uint32_t s_limit) {
+// COUNT (test hook only): cnt[0] node visits, cnt[1] triangle tests, cnt[2] pushes refused by a full stack (bvh_trace's counters).
+template <bool SMEM, bool FMA_SLABS, bool COUNT = false>
+__device__ __forceinline__ void dyn_node_step(const BvhView &b, DynRay &r, uint32_t s_step, uint32_t s_limit, uint32_t *cnt = nullptr) {
+    if (COUNT) cnt[0]++;
     const float4 *np = b.nodes + (size_t)r.cur * 4;
     const float4 n0 = ld4<SMEM>(np), n1 = ld4<SMEM>(np + 1), n2 = ld4<SMEM>(np + 2), n3 = ld4<SMEM>(np + 3);
     float ax0, ax1, ay0, ay1, az0, az1, bx0, bx1, by0, by1, bz0, bz1;
@@ -74,6 +76,7 @@ __device__ __forceinline__ void dyn_node_step(const BvhView &b, DynRay &r, uint3
         const bool a_first = an <= bn;
         const int near_c = a_first ? c0 : c1, far_c = a_first ? c1 : c0;
         if (r.s_top < s_limit) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(r.s_top), "r"(far_c) : "memory"); r.s_top += s_step; }
+        else if (COUNT) cnt[2]++;
         r.cur = near_c;
     } else if (ha) {
         r.cur = c0;
@@ -90,9 +93,11 @@ __device__ __forceinline__ void dyn_node_step(const BvhView &b, DynRay &r, uint3
 // Hit children are ordered front to back with a 5-exchange sorting network on packed keys (entry distance, 2 low mantissa bits
 // replaced by the slot number); the nearest is entered, the others are pushed far-to-near.  The shared-memory column holds the usual
 // case, deeper stacks overflow to a per-thread local-memory array, so no push is ever dropped.
-__device__ __forceinline__ void dyn_push4(DynRay &r, int v, uint32_t s_step, uint32_t s_limit, int *spill) {
+template <bool COUNT = false>
+__device__ __forceinline__ void dyn_push4(DynRay &r, int v, uint32_t s_step, uint32_t s_limit, int *spill, uint32_t *cnt = nullptr) {
     if (r.s_top < s_limit) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(r.s_top), "r"(v) : "memory"); r.s_top += s_step; }
     else if (r.n_spill < DYN_SPILL) spill[r.n_spill++] = v;
+    else if (COUNT) cnt[2]++;
 }
 __device__ __forceinline__ void dyn_pop4(DynRay &r, uint32_t s_step, const int *spill) {
     if (r.n_spill > 0) r.cur = spill[--r.n_spill];
@@ -118,8 +123,9 @@ __device__ __forceinline__ int dyn_sel4(float4 ch, uint32_t key) {
     const uint32_t k = key & 3u;
     return __float_as_int(k == 0u ? ch.x : (k == 1u ? ch.y : (k == 2u ? ch.z : ch.w)));
 }
-template <bool FMA_SLABS>
-__device__ __forceinline__ void dyn_node4_step(const float4 *nodes4, DynRay &r, uint32_t s_step, uint32_t s_limit, int *spill) {
+template <bool FMA_SLABS, bool COUNT = false>
+__device__ __forceinline__ void dyn_node4_step(const float4 *nodes4, DynRay &r, uint32_t s_step, uint32_t s_limit, int *spill, uint32_t *cnt = nullptr) {
+    if (COUNT) cnt[0]++;
     const float4 *np = nodes4 + (size_t)r.cur * 8;
     const float4 LX = __ldg(np), LY = __ldg(np + 1), LZ = __ldg(np + 2), HX = __ldg(np + 3), HY = __ldg(np + 4), HZ = __ldg(np + 5), CH = __ldg(np + 6);
     uint32_t k0 = dyn_child_key<FMA_SLABS>(r, LX.x, LY.x, LZ.x, HX.x, HY.x, HZ.x, 0u);
@@ -135,15 +141,16 @@ __device__ __forceinline__ void dyn_node4_step(const float4 *nodes4, DynRay &r, 
     if (k0 == 0xFFFFFFFFu) { dyn_pop4(r, s_step, spill); return; }
     r.cur = dyn_sel4(CH, k0);
     if (k1 != 0xFFFFFFFFu) {
-        if (k3 != 0xFFFFFFFFu) dyn_push4(r, dyn_sel4(CH, k3), s_step, s_limit, spill);
-        if (k2 != 0xFFFFFFFFu) dyn_push4(r, dyn_sel4(CH, k2), s_step, s_limit, spill);
-        dyn_push4(r, dyn_sel4(CH, k1), s_step, s_limit, spill);
+        if (k3 != 0xFFFFFFFFu) dyn_push4<COUNT>(r, dyn_sel4(CH, k3), s_step, s_limit, spill, cnt);
+        if (k2 != 0xFFFFFFFFu) dyn_push4<COUNT>(r, dyn_sel4(CH, k2), s_step, s_limit, spill, cnt);
+        dyn_push4<COUNT>(r, dyn_sel4(CH, k1), s_step, s_limit, spill, cnt);
     }
 }
 
 // One triangle of the current leaf.  Returns true when an ANYHIT ray found its occluder (the ray is finished: cur = DYN_DONE).
-template <bool SMEM, bool ANYHIT, bool WIDE = false>
-__device__ __forceinline__ bool dyn_leaf_step(const BvhView &b, DynRay &r, uint32_t s_step, const int *spill = nullptr) {
+template <bool SMEM, bool ANYHIT, bool WIDE = false, bool COUNT = false>
+__device__ __forceinline__ bool dyn_leaf_step(const BvhView &b, DynRay &r, uint32_t s_step, const int *spill = nullptr, uint32_t *cnt = nullptr) {
+    if (COUNT) cnt[1]++;
     const uint32_t ref = (uint32_t)(~r.cur);
     const uint32_t slot = ref >> 2, rest = ref & 3u;
     const float4 *tp = b.tris + (size_t)slot * 3;
@@ -160,6 +167,22 @@ __device__ __forceinline__ bool dyn_leaf_step(const BvhView &b, DynRay &r, uint3
     if (rest == 0u) { if (WIDE) dyn_pop4(r, s_step, spill); else dyn_pop(r, s_step); }
     else r.cur = (int)~(((slot + 1u) << 2) | (rest - 1u));
     return false;
+}
+
+// One round of the while-while loop for every lane of the warp: the node phase (each lane descends until it holds a leaf or is done), then
+// the leaf phase (one triangle per iteration until the lane pops an inner node or finishes).  on_occluded() runs in the lane whose ANYHIT ray
+// just found its occluder.  Returns the ballot of the lanes still traversing.  Shared by k_extend_dyn, k_shadow_dyn and the traversal test
+// hook (trace_query.cu).
+template <bool SMEM, bool ANYHIT, bool WIDE, bool FMA_SLABS, bool COUNT = false, class OnOccluded>
+__device__ __forceinline__ uint32_t dyn_round(const BvhView &b, const float4 *nodes4, DynRay &r, uint32_t s_step, uint32_t s_limit, int *spill,
+                                          OnOccluded &&on_occluded, uint32_t *cnt = nullptr) {
+    if (WIDE) { while (r.cur >= 0) dyn_node4_step<FMA_SLABS, COUNT>(nodes4, r, s_step, s_limit, spill, cnt); }
+    else { while (r.cur >= 0) dyn_node_step<SMEM, FMA_SLABS, COUNT>(b, r, s_step, s_limit, cnt); }
+    __syncwarp();
+    while (r.cur < 0 && r.cur != DYN_DONE) {
+        if (dyn_leaf_step<SMEM, ANYHIT, WIDE, COUNT>(b, r, s_step, spill, cnt)) on_occluded();
+    }
+    return __ballot_sync(0xFFFFFFFFu, r.cur != DYN_DONE);
 }
 
 // Warp-local pool of consecutive work items, refilled from a global counter.  All members are warp-uniform.

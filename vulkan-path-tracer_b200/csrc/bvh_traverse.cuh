@@ -114,21 +114,27 @@ __device__ __forceinline__ bool tri_test(float3 v0, float3 e1, float3 e2, float3
     return (det != 0.0f) & (u >= 0.0f) & (u <= 1.0f) & (v >= 0.0f) & (__fadd_rn(u, v) <= 1.0f) & (t > tmin) & (t < tmax);
 }
 
+// Acceptance bound of a light-visibility (TARGET) query whose target the ray hits at tL: the next float above tL, so the target's own hit
+// and exact ties at tL pass the triangle test and the tie rule decides them.  Shared by bvh_trace, the fused k_shade_hit, k_shadow_dyn
+// and the traversal test hook.
+__device__ __forceinline__ float light_tmax_test(float tL) { return __uint_as_float(__float_as_uint(tL) + 1u); }
+
 // stack: shared-memory column of this thread, entries at stack[k * stride] (addressed through the shared window: STS/LDS with
 // an incrementally maintained address instead of a generic-pointer computation per push).
 // Slab test: with FMA_SLABS the plane distances are one FFMA each, t = n*inv - (o*inv) (12 FFMA per node instead of 12 FADD + 12 FMUL).
 // That form perturbs a plane by <= 6e-8*|o| (the rounding of o*inv); the node boxes carry an absolute pad of 2e-6 * scene extent
 // (lbvh.cu: k_emit), so it is conservative for every origin within ~16 scene extents -- i.e. for all secondary rays, whose origins lie
-// on scene surfaces.  Camera rays (origin anywhere) and the test hook use the subtract-then-multiply form (FMA_SLABS = false).
+// on scene surfaces.  Camera rays (origin anywhere) use the subtract-then-multiply form (FMA_SLABS = false).
 // TARGET (with ANYHIT): "is anything in front of triangle target_gid, which the ray hits at tmax?"  A triangle occludes when
 // t < tmax, or t == tmax and its id is lower than the target's (the tie rule of the closest-hit query); the target itself never does.
+// COUNT: node visits, triangle tests and pushes refused by a full stack (a refused push drops a subtree: wrong answers, not a fault).
 template <bool SMEM, bool ANYHIT, bool COUNT = false, bool TARGET = false, bool FMA_SLABS = false>
 __device__ __forceinline__ bool bvh_trace(const BvhView &b, float3 o, float3 d, float tmin, float tmax, HitRec &h,
                                           int *stack, int stride, int max_stack, uint32_t *n_nodes = nullptr, uint32_t *n_tris = nullptr,
-                                          uint32_t target_gid = 0xFFFFFFFFu, float tmax_test_in = -1.0f) {
+                                          uint32_t target_gid = 0xFFFFFFFFu, float tmax_test_in = -1.0f, uint32_t *n_refused = nullptr) {
     // TARGET: admit t == tmax (tmax > 0).  A caller that serves both NEE queries with one copy of this loop (the fused k_shade_hit) passes the
     // acceptance bound itself: nextafter(tL) for a light ray, tmax for a sky ray (whose target 0xFFFFFFFF makes every t < tmax an occluder).
-    const float tmax_test = TARGET ? (tmax_test_in >= 0.0f ? tmax_test_in : __uint_as_float(__float_as_uint(tmax) + 1u)) : tmax;
+    const float tmax_test = TARGET ? (tmax_test_in >= 0.0f ? tmax_test_in : light_tmax_test(tmax)) : tmax;
     h.slot = 0xFFFFFFFFu; h.gid = 0xFFFFFFFFu; h.t = tmax; h.u = 0.0f; h.v = 0.0f;
     uint32_t best_gid = 0xFFFFFFFFu;
     bool found = false;
@@ -193,6 +199,7 @@ __device__ __forceinline__ bool bvh_trace(const BvhView &b, float3 o, float3 d, 
                 const bool a_first = an <= bn;
                 const int near_c = a_first ? c0 : c1, far_c = a_first ? c1 : c0;
                 if (s_top < s_limit) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(s_top), "r"(far_c) : "memory"); s_top += s_step; }
+                else if (COUNT && n_refused) (*n_refused)++;
                 cur = near_c;
                 continue;
             } else if (ha) { cur = c0; continue; }

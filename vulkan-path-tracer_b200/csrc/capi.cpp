@@ -262,6 +262,14 @@ int32_t b200pt_trace_stats(b200pt_handle h, uint32_t n, const float *o, const fl
     if (n && (!o || !d || !nodes_tris)) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { std::vector<float> t(n), uv(2 * (size_t)n); std::vector<uint32_t> p(n), i(n); e.trace_closest(n, o, d, tmin, tmax, t.data(), p.data(), i.data(), uv.data(), nodes_tris); });
 }
+int32_t b200pt_trace_query(b200pt_handle h, int32_t shape, int32_t kind, int32_t fma_slabs, uint32_t n, const float *o, const float *d, const float *tmin,
+                           const float *tmax, const uint32_t *target, const float *tmax_test, float *t, uint32_t *prim, uint32_t *inst, float *uv,
+                           uint32_t *occluded, uint32_t *stats) {
+    if (shape < 0 || shape >= TQ_SHAPES || kind < TQ_CLOSEST || kind > TQ_TARGET) return B200PT_ERR_WRONG_ARGUMENTS;
+    if (n && (!o || !d || !tmin || !tmax || (kind == TQ_TARGET && (!target || !tmax_test)) || (kind == TQ_CLOSEST ? (!t || !prim || !inst || !uv) : !occluded)))
+        return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.trace_query(shape, kind, fma_slabs != 0, n, o, d, tmin, tmax, target, tmax_test, t, prim, inst, uv, occluded, stats); });
+}
 int32_t b200pt_bake_lut(b200pt_handle h, int32_t kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out, float *elapsed_ms) {
     if (!out || kind < 0 || kind > 2 || !sx || !sy || !sz) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { e.bake_lut(kind, sx, sy, sz, sample_count, seed, slices, out, elapsed_ms); });

@@ -990,6 +990,41 @@ void Engine::trace_closest(uint32_t n, const float *org, const float *dir, float
     cudaFree(d_o); cudaFree(d_d); cudaFree(d_t); cudaFree(d_uv); cudaFree(d_p); cudaFree(d_i); if (d_st) cudaFree(d_st);
     CK(e); CK(cudaGetLastError());
 }
+void Engine::trace_query(int shape, int kind, bool fma, uint32_t n, const float *org, const float *dir, const float *tmin, const float *tmax, const uint32_t *target,
+                         const float *tmax_test, float *t, uint32_t *prim, uint32_t *inst, float *uv, uint32_t *occluded, uint32_t *stats) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!n) return;
+    std::vector<void *> bufs;
+    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
+    auto dev = [&](size_t bytes, const void *src) -> void * {               // device buffer, filled from src when given
+        void *p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) fail(e);
+        bufs.push_back(p);
+        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
+        return p;
+    };
+    const bool any = kind != TQ_CLOSEST, tgt = kind == TQ_TARGET;
+    TraceQuery q{};
+    q.n = n;
+    q.org = (const float *)dev((size_t)n * 12, org); q.dir = (const float *)dev((size_t)n * 12, dir);
+    q.tmin = (const float *)dev((size_t)n * 4, tmin); q.tmax = (const float *)dev((size_t)n * 4, tmax);
+    if (tgt) { q.target = (const uint32_t *)dev((size_t)n * 4, target); q.tmax_test = (const float *)dev((size_t)n * 4, tmax_test); }
+    if (any) q.occluded = (uint32_t *)dev((size_t)n * 4, nullptr);
+    else { q.t = (float *)dev((size_t)n * 4, nullptr); q.prim = (uint32_t *)dev((size_t)n * 4, nullptr); q.inst = (uint32_t *)dev((size_t)n * 4, nullptr); q.uv = (float *)dev((size_t)n * 8, nullptr); }
+    if (stats) q.stats = (uint32_t *)dev((size_t)n * 12, nullptr);
+    const int r = launch_trace_query(lc_, ds_, bvh_.depth4, shape, kind, fma, q, stream_);
+    if (r == TQ_UNSUPPORTED) { for (void *p : bufs) cudaFree(p); throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "trace_query: the scene has no such traversal shape" }; }
+    if (r != 0) fail((cudaError_t)r);
+    auto get = [&](void *dst, const void *src, size_t bytes) { cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, stream_); if (e != cudaSuccess) fail(e); };
+    if (any) get(occluded, q.occluded, (size_t)n * 4);
+    else { get(t, q.t, (size_t)n * 4); get(prim, q.prim, (size_t)n * 4); get(inst, q.inst, (size_t)n * 4); get(uv, q.uv, (size_t)n * 8); }
+    if (stats) get(stats, q.stats, (size_t)n * 12);
+    const cudaError_t e = cudaStreamSynchronize(stream_);
+    for (void *p : bufs) cudaFree(p);
+    CK(e); CK(cudaGetLastError());
+}
 // LookupTableCalculator::CalculateTable (PT/LookupTableCalculator.cpp:44-157) on this engine's device and stream.
 // slices == 0 picks enough dispatch slices to give every SM ~2048 resident threads.
 void Engine::bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out_host, float *elapsed_ms) {

@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers of the sm_90a kernels (wavefront_kernels.cu, lbvh.cu, post_kernels.cu, denoise_kernels.cu)
+// kernels.h -- host-callable launchers of the sm_90a kernels (wavefront_kernels.cu, lbvh.cu, post_kernels.cu, denoise_kernels.cu, trace_query.cu)
 #pragma once
 #include "device_types.h"
 #include <cuda_runtime.h>
@@ -17,6 +17,7 @@ struct LaunchCfg {
     int grid_shadow;    // persistent grid of k_shadow_dyn
     bool wide;          // the dynamic-fetch kernels walk the BVH4 (DevScene::nodes4)
     int dyn_stack;      // shared-memory stack entries per thread of the dynamic-fetch kernels (BVH4: overflow goes to local memory)
+    int wide_cap;       // BVH4: most shared-memory stack entries per thread (B200PT_WIDE_STACK, default WIDE_STACK_DEFAULT)
     bool big;           // bvh_in_smem with a BVH > 64 KiB: one 512-thread CTA per SM for k_extend, k_camera, k_connect and the fused k_shade_hit
     int extend_threads; // CTA size of k_extend / k_extend_dyn, k_camera and k_connect (256; big mode's one-ray-per-thread kernels: 512)
     int bounce_threads; // CTA size of the fused k_shade_hit (128, big: 512)
@@ -102,6 +103,21 @@ void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const
                          float *T_out, float *scatter_out, int32_t *vol_out, uint32_t *rng_out, cudaStream_t st);
 int launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
                       float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st);
+// Shared-memory stack entries of the BVH4 dynamic-fetch kernels for a BVH4 of the given depth with a shared column of at most `cap` entries
+// (the rest goes to the DYN_SPILL overflow array); 0 when even that cannot hold three pushes per level.
+constexpr int WIDE_STACK_DEFAULT = 24;
+int bvh4_stack_entries(int bvh4_depth, int cap);
+
+// ---- traversal test hook (trace_query.cu, b200pt_trace_query): shapes and query kinds as in include/b200pt.h ----
+enum { TQ_SHARED = 0, TQ_GLOBAL, TQ_FLAT, TQ_FIXED_ORIGIN, TQ_DYN2, TQ_DYN4, TQ_DYN4_SPILL, TQ_SHAPES };
+enum { TQ_CLOSEST = 0, TQ_ANY, TQ_TARGET };
+constexpr int TQ_UNSUPPORTED = -1;            // the scene has no such shape (no flat walk, no BVH4, too big for shared memory)
+struct TraceQuery {                           // device arrays of n rays; target / tmax_test for TQ_TARGET, occluded for the any-hit kinds
+    uint32_t n; const float *org, *dir, *tmin, *tmax, *tmax_test; const uint32_t *target;
+    float *t; uint32_t *prim, *inst; float *uv; uint32_t *occluded; uint32_t *stats;   // stats: 3 per ray, or nullptr
+};
+// Returns cudaError_t as int, or TQ_UNSUPPORTED.
+int launch_trace_query(const LaunchCfg &lc, const DevScene &sc, int bvh4_depth, int shape, int kind, bool fma, const TraceQuery &q, cudaStream_t st);
 
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
 struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;
@@ -124,6 +140,8 @@ uint32_t bvh2_reinsert_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t ro
 uint32_t bvh2_sah_build_host(const float *ref_boxes, uint32_t n, float trav_cost, BvhNode *out, uint32_t *perm, int *depth, double *sah_cost);
 // mode 1: inner nodes only (download, rebuild, upload in place); mode 2: full build from r->h_ref_box, reference slots and tri_slot permuted
 // (falls back to mode 1 when the boxes were not kept); mode 3: mode 2 + insertion-based refinement; 4: mode 1 + refinement; 5: refinement only.  Returns cudaError_t as int.
+// A pass result deeper than BVH_STACK_MAX - 2 is dropped unless the input tree is deeper still (query_launch_cfg sizes the stacks from the depth).
+constexpr int BVH_STACK_MAX = 64;
 int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode = 1);
 // Downloads r->nodes, collapses, uploads r->nodes4 (own allocation).  Returns cudaError_t as int; leaves nodes4 = nullptr if the root is a leaf.
 int lbvh_build_wide(LbvhResult *r, cudaStream_t st);

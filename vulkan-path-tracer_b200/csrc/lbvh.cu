@@ -787,6 +787,9 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
         const uint32_t m = bvh2_reinsert_host(out.data(), n_in, 0, tmp.data(), ri_passes, ri_fraction, &d2, c2);
         if (m == n_in) { std::copy(tmp.begin(), tmp.begin() + m, out.begin()); depth = d2; if (cost_after) *cost_after = c2[1]; }
     };
+    // SAH and re-insertion trees of detail nested around a point can be far deeper than the LBVH (tests/test_traversal_queries.py): keep the
+    // shallower input rather than make every traversal kernel carry a deeper stack
+    auto depth_ok = [&](int d) { return d + 2 <= BVH_STACK_MAX || d <= r->max_depth; };
     const bool full = mode == 2 || mode == 3, refine = mode >= 3;
     if (full && r->h_ref_box && r->n_tris > (uint32_t)LBVH_LEAF_MAX && r->n_tris - 1 <= r->n_nodes) {
         std::vector<uint32_t> perm(r->n_tris);
@@ -794,7 +797,7 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
         { std::vector<BvhNode> scratch(r->n_nodes); int d; bvh2_sah_rebuild_host(h2.data(), r->n_nodes, r->root, scratch.data(), &d, c_old); }   // cost of the LBVH, for the log
         const uint32_t n = bvh2_sah_build_host(r->h_ref_box, r->n_tris, 1.0f, out.data(), perm.data(), &depth, &c_new);
         if (n != 0 && refine) reinsert(n, &c_new);
-        if (n != 0 && c_new < c_old[0]) {                                       // never trade the tree for a costlier one
+        if (n != 0 && c_new < c_old[0] && depth_ok(depth)) {                    // never trade the tree for a costlier one
             std::vector<BvhTri> t_old(r->n_tris), t_new(r->n_tris);
             LBVH_CHECK(cudaMemcpyAsync(t_old.data(), r->tris, (size_t)r->n_tris * sizeof(BvhTri), cudaMemcpyDeviceToHost, st));
             LBVH_CHECK(cudaStreamSynchronize(st));
@@ -821,7 +824,7 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
     }
     if (n == 0) return 0;
     if (sah) { sah[0] = cst[0]; sah[1] = cst[1] < cst[0] ? cst[1] : cst[0]; }
-    if (!(cst[1] < cst[0])) return 0;                                          // never trade the tree for a costlier one
+    if (!(cst[1] < cst[0]) || !depth_ok(depth)) return 0;                      // never trade the tree for a costlier one
     LBVH_CHECK(cudaMemcpyAsync(r->nodes, out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     r->root = 0; r->max_depth = depth;

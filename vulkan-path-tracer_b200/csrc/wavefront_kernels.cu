@@ -632,7 +632,7 @@ __global__ void __launch_bounds__(FUSE ? 512 : 128, FUSE ? 1 : SHADE_MIN_BLOCKS)
                             const float4 ta = tp[0], tb = tp[1], tc = tp[2];
                             float tL, uL, vL;
                             go = tri_test(f3(ta), f3(tb), f3(tc), ro, toW, 0.0001f, 1000000.0f, tL, uL, vL);
-                            tmax = tL; tmax_test = __uint_as_float(__float_as_uint(tL) + 1u);
+                            tmax = tL; tmax_test = light_tmax_test(tL);
                         }
                         n_shadow++;
                         if (go) {
@@ -913,11 +913,7 @@ __global__ void __launch_bounds__(256) k_extend_dyn(DevScene sc, PathState ps, f
         }
         const int thr_now = pool.empty() ? 1 : thresh;
         do {
-            if (WIDE) { while (r.cur >= 0) dyn_node4_step<!PRIMARY>(nodes4, r, s_step, s_limit, spill); }
-            else { while (r.cur >= 0) dyn_node_step<SMEM, !PRIMARY>(bv, r, s_step, s_limit); }
-            __syncwarp();
-            while (r.cur < 0 && r.cur != DYN_DONE) dyn_leaf_step<SMEM, false, WIDE>(bv, r, s_step, spill);
-            act = __ballot_sync(0xFFFFFFFFu, r.cur != DYN_DONE);
+            act = dyn_round<SMEM, false, WIDE, !PRIMARY>(bv, nodes4, r, s_step, s_limit, spill, [] {});
         } while (__popc(act) >= thr_now);
     }
 }
@@ -983,7 +979,7 @@ __global__ void __launch_bounds__(256, 4) k_shadow_dyn(DevScene sc, ShadeOut so,
                     const float4 ta = ld4<SMEM>(tp), tb = ld4<SMEM>(tp + 1), tc = ld4<SMEM>(tp + 2);
                     float tL, uL, vL;
                     if (tri_test(f3(ta), f3(tb), f3(tc), f3(lo4), f3(ld4_), 0.0001f, 1000000.0f, tL, uL, vL)) {
-                        dyn_init(r, f3(lo4), f3(ld4_), 0.0001f, tL, __uint_as_float(__float_as_uint(tL) + 1u), lgid, bv.root, s_base, s_step);
+                        dyn_init(r, f3(lo4), f3(ld4_), 0.0001f, tL, light_tmax_test(tL), lgid, bv.root, s_base, s_step);
                         r.gid = e;
                     } else {
                         atomicAnd(reinterpret_cast<unsigned int *>(&so.e0[i].w), ~(1u << 30));
@@ -1001,14 +997,9 @@ __global__ void __launch_bounds__(256, 4) k_shadow_dyn(DevScene sc, ShadeOut so,
         if (act == 0u) { if (tail == head && pool.empty()) break; else continue; }
         const int thr_now = (tail == head && pool.empty()) ? 1 : thresh;
         do {
-            if (WIDE) { while (r.cur >= 0) dyn_node4_step<true>(nodes4, r, s_step, s_limit, spill); }
-            else { while (r.cur >= 0) dyn_node_step<SMEM, true>(bv, r, s_step, s_limit); }
-            __syncwarp();
-            while (r.cur < 0 && r.cur != DYN_DONE) {
-                if (dyn_leaf_step<SMEM, true, WIDE>(bv, r, s_step, spill))  // occluded: drop the request
-                    atomicAnd(reinterpret_cast<unsigned int *>(&so.e0[r.gid >> 1].w), ~(1u << (29u + (r.gid & 1u))));
-            }
-            act = __ballot_sync(0xFFFFFFFFu, r.cur != DYN_DONE);
+            act = dyn_round<SMEM, true, WIDE, true>(bv, nodes4, r, s_step, s_limit, spill, [&] {   // occluded: drop the request
+                atomicAnd(reinterpret_cast<unsigned int *>(&so.e0[r.gid >> 1].w), ~(1u << (29u + (r.gid & 1u))));
+            });
         } while (__popc(act) >= thr_now);
     }
     for (int o = 16; o > 0; o >>= 1) n_shadow += __shfl_down_sync(0xFFFFFFFFu, n_shadow, o);
@@ -1436,6 +1427,12 @@ static int opt_in_shared_memory() {
     return rc;
 }
 
+int bvh4_stack_entries(int bvh4_depth, int cap) {
+    const int need = 3 * bvh4_depth + 2;                                    // worst case: three pushes per level
+    const int entries = need < cap ? need : cap;
+    return need - entries > DYN_SPILL ? 0 : entries;
+}
+
 // grid sizing: persistent grids = SM count x resident CTAs per SM for the chosen shared-memory footprint
 int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, LaunchCfg *lc) {
     { const int a = opt_in_shared_memory(); if (a != 0) return a; }
@@ -1443,7 +1440,10 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     cudaDeviceProp prop; cudaError_t e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) return (int)e;
     const int sms = prop.multiProcessorCount;
-    lc->max_stack = bvh_max_depth + 2; if (lc->max_stack < 4) lc->max_stack = 4; if (lc->max_stack > 64) lc->max_stack = 64;
+    // depth + 2 entries always suffice for the near-first walk (one push per level).  A full stack would drop the push -- a lost subtree, i.e.
+    // wrong hits with no error -- so a tree deeper than lbvh_refine_sah normally leaves (BVH_STACK_MAX) gets a deeper stack, and the scene is
+    // refused below when the shared memory of a launch cannot hold it.
+    lc->max_stack = std::max(bvh_max_depth + 2, 4);
     // Whole BVH in shared memory: <= 64 KiB -> several CTAs per SM (Cornell: 1.3 KiB); up to what fits beside the stacks of ONE 512-thread CTA per SM
     // -> "big" mode (config 4's glass scene: 108 KiB): k_extend, k_connect, k_camera and the fused k_shade_hit run 512-thread CTAs.
     const bool aligned = sc.bvh_bytes > 0 && (sc.bvh_bytes % 16u) == 0;
@@ -1477,12 +1477,11 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     if (const char *e = getenv("B200PT_WIDE")) { if (atoi(e) == 1 && lc->trav_dyn && !smem && sc.nodes4 != nullptr) lc->wide = true; }
     if (const char *e = getenv("B200PT_WIDE")) { if (atoi(e) == 0) lc->wide = false; }
     lc->dyn_stack = lc->max_stack;                                          // BVH2: depth + 2 entries always suffice
+    lc->wide_cap = WIDE_STACK_DEFAULT;
+    if (const char *e = getenv("B200PT_WIDE_STACK")) { int v = atoi(e); if (v >= 4 && v <= 96) lc->wide_cap = v; }
     if (lc->wide) {
-        const int need = 3 * bvh4_depth + 2;                                // worst case: three pushes per level
-        int cap = 24;
-        if (const char *e = getenv("B200PT_WIDE_STACK")) { int v = atoi(e); if (v >= 4 && v <= 96) cap = v; }
-        lc->dyn_stack = need < cap ? need : cap;
-        if (need - lc->dyn_stack > DYN_SPILL) lc->wide = false, lc->dyn_stack = lc->max_stack;   // deeper than shared column + overflow array: BVH2
+        lc->dyn_stack = bvh4_stack_entries(bvh4_depth, lc->wide_cap);
+        if (lc->dyn_stack == 0) lc->wide = false, lc->dyn_stack = lc->max_stack;   // deeper than shared column + overflow array: BVH2
     }
     // Bounce pipeline of scenes whose BVH is staged in shared memory and walked one ray per thread (the default elsewhere is 0):
     //   1 (default): k_shade_hit<., ., true> traces each NEE query the moment it is built and finishes the path (roulette, radiance, compaction)
@@ -1502,6 +1501,11 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     lc->smem_shadow = trace_smem_bytes(sc, lc->dyn_stack + 1, 256, smem) + DYN_RING_BYTES_HOST;
     lc->smem_bounce = trace_smem_bytes(sc, lc->max_stack, lc->bounce_threads, true);
     lc->smem_trace = trace_smem_bytes(sc, lc->max_stack, 256, smem);
+    // A stack the launches cannot hold (a tree far deeper than BVH_STACK_MAX): refuse the scene rather than truncate.  Big mode was checked
+    // against each kernel's own static shared memory above; elsewhere 8 KiB bounds it (k_camera's flat-walk table, ~4 KiB, is the largest).
+    if (!fits_big)
+        for (const size_t b : { lc->smem_extend, lc->smem_shadow, smem ? lc->smem_bounce : 0u, lc->smem_trace })   // the fused k_shade_hit runs only over a staged BVH
+            if (b + 8u * 1024u > 227u * 1024u) return (int)cudaErrorInvalidConfiguration;
     auto occupancy = [](auto fn, int threads, size_t smem_bytes) { int n = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, threads, smem_bytes); return n; };
     int occ_e = 0, occ_c = 0, occ_sh = 0;
     if (lc->trav_dyn) {
