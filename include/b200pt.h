@@ -349,6 +349,55 @@ int32_t b200pt_trace_stats(b200pt_handle h, uint32_t n, const float *origins3, c
 int32_t b200pt_trace_query(b200pt_handle h, int32_t shape, int32_t kind, int32_t fma_slabs, uint32_t n, const float *origins3, const float *directions3,
                            const float *tmin, const float *tmax, const uint32_t *target_gid, const float *tmax_test,
                            float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out2, uint32_t *occluded_out, uint32_t *stats3_out);
+/* Shading test hook: one shading step of the renderer's hit kernel (k_shade_hit, SH/ClosestHit.slang:40-238) for caller-given hits,
+ * through the same device functions and the same class instantiation, without the shadow queries.  Hit i: instance inst[i], primitive
+ * prim[i] of that instance's mesh, barycentrics uv2[2i..], world ray direction dir3, ray origin org3 and BSDF pdf pay_pdf[i] of the
+ * segment that reached it (the emission MIS term of a hit at Depth > 0), sampler state rng[i].  The sky draw, the light draw and the
+ * BSDF draw are made in the renderer's order and each is evaluated; c is the NEE term added when the shadow ray is unoccluded.
+ * L3 (optional): one more world direction per hit at which the BSDF is evaluated.  force_general != 0 runs the all-lobes instantiation
+ * instead of the triangle's material class.  The current config supplies the rest.  out: n records of B200PT_SQ_STRIDE floats at the
+ * offsets below (vectors in tangent space unless marked world; LIGHT_GID and RNG hold u32 bits).  B200PT_ERR_WRONG_ARGUMENTS for an
+ * instance or primitive out of range, and for scenes with volumes or the atmosphere on (their paths have walk-level hooks). */
+#define B200PT_SQ_N          0    /* shading normal (world) */
+#define B200PT_SQ_T          3    /* tangent (world, rotated) */
+#define B200PT_SQ_B          6    /* bitangent (world) */
+#define B200PT_SQ_NG         9    /* geometry normal (world) */
+#define B200PT_SQ_INSIDE     12   /* HitFromInside */
+#define B200PT_SQ_AX         13
+#define B200PT_SQ_AY         14
+#define B200PT_SQ_ETA        15
+#define B200PT_SQ_PM         16   /* lobe probabilities */
+#define B200PT_SQ_PD         17
+#define B200PT_SQ_PG         18
+#define B200PT_SQ_BASECOLOR  19
+#define B200PT_SQ_ROUGHNESS  22
+#define B200PT_SQ_V          23
+#define B200PT_SQ_H          26   /* sampled half vector */
+#define B200PT_SQ_EMITTED    29   /* emission term */
+#define B200PT_SQ_SKY_L      32
+#define B200PT_SQ_SKY_LV     35   /* radiance, pdf */
+#define B200PT_SQ_SKY_EVAL   39   /* BxDF, PDF */
+#define B200PT_SQ_SKY_C      43
+#define B200PT_SQ_LIGHT_L    46
+#define B200PT_SQ_LIGHT_LV   49
+#define B200PT_SQ_LIGHT_EVAL 53
+#define B200PT_SQ_LIGHT_C    57
+#define B200PT_SQ_LIGHT_GID  60   /* sampled emissive triangle */
+#define B200PT_SQ_BSDF_L     61   /* sampled direction, 0 when invalid */
+#define B200PT_SQ_BSDF_EVAL  64
+#define B200PT_SQ_VALID      68
+#define B200PT_SQ_SCATTER    69   /* sampled direction (world) */
+#define B200PT_SQ_SAMPLE     72   /* BxDF, PDF after the geometry-normal rejection */
+#define B200PT_SQ_REFRACTED  76
+#define B200PT_SQ_ENTERED    77   /* refracted into the object: a medium starts */
+#define B200PT_SQ_REJECTED   78
+#define B200PT_SQ_USER_L     79
+#define B200PT_SQ_USER_EVAL  82
+#define B200PT_SQ_RNG        86   /* sampler state after the step */
+#define B200PT_SQ_CLASS      87   /* material class whose instantiation ran */
+#define B200PT_SQ_STRIDE     88
+int32_t b200pt_shade_query(b200pt_handle h, int32_t force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv2,
+                           const float *dir3, const float *org3, const float *pay_pdf, const uint32_t *rng, const float *L3, float *out);
 
 /* Energy-compensation lookup-table baker (SURVEY.md 8f row 2).
  * Replaces LookupTableCalculator::CalculateTable(tableSize, sampleCount) (PathTracer/LookupTableCalculator.h:8,

@@ -140,6 +140,8 @@ def lib():
         L.orc_scene_world_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.orc_trace_closest.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.orc_shade_query.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32] + [C.c_void_p] * 9
+        L.orc_shade_query.restype = None
         L.orc_render.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.POINTER(OrcCounters)]
         L.orc_sample_pixel.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -343,6 +345,17 @@ class Scene:
         t = np.zeros(n, np.float32); prim = np.zeros(n, np.uint32); inst = np.zeros(n, np.uint32); uv = np.zeros((n, 2), np.float32)
         lib().orc_trace_closest(self.h, n, _p(org), _p(dirs), C.c_float(tmin), C.c_float(tmax), int(use_bvh), _p(t), _p(prim), _p(inst), _p(uv))
         return t, prim, inst, uv
+
+    def shade_query(self, cfg, inst, prim, uv, dirs, org, pay_pdf, rng, L=None, stride=88):
+        """orc_shade_query: [n, stride] float32 records laid out like B200PT_SQ_* (include/b200pt.h)"""
+        inst = np.ascontiguousarray(inst, np.uint32).reshape(-1); n = len(inst)
+        b = lambda a, dt, sh: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dt), sh))
+        prim, uv, dirs, org = b(prim, np.uint32, (n,)), b(uv, np.float32, (n, 2)), b(dirs, np.float32, (n, 3)), b(org, np.float32, (n, 3))
+        pay_pdf, rng = b(pay_pdf, np.float32, (n,)), b(rng, np.uint32, (n,))
+        Lw = None if L is None else b(L, np.float32, (n, 3))
+        out = np.zeros((n, stride), np.float32)
+        lib().orc_shade_query(self.h, C.byref(cfg), n, _p(inst), _p(prim), _p(uv), _p(dirs), _p(org), _p(pay_pdf), _p(rng), None if Lw is None else _p(Lw), _p(out))
+        return out
 
     def render(self, cfg, W, H, nframes, base_seed, frame0=0, image=None, rank=0, world=1, band_rows=1, nthreads=0):
         if image is None: image = np.zeros((H, W, 4), np.float32)

@@ -577,12 +577,17 @@ static Eval eval_dielectric_reflection(const Mat *m, const OrcScene *sc, const O
     return e;
 }
 /* :167-279 */
+/* :169-177: lobe probabilities */
+static void lobe_probs(const Mat *m, float *pm, float *pd, float *pg) {
+    *pm = m->Metallic;
+    *pd = (1.0f - m->Metallic) * (1.0f - m->Transmission);
+    *pg = (1.0f - m->Metallic) * m->Transmission;
+    float sum = *pm + *pd + *pg;
+    *pm /= sum; *pd /= sum; *pg /= sum;
+}
 static Eval eval_bsdf(const Mat *m, const OrcScene *sc, const OrcConfig *cfg, v3 V, v3 L) {
-    float pm = m->Metallic;
-    float pd = (1.0f - m->Metallic) * (1.0f - m->Transmission);
-    float pg = (1.0f - m->Metallic) * m->Transmission;
-    float sum = pm + pd + pg;
-    pm /= sum; pd /= sum; pg /= sum;
+    float pm, pd, pg;
+    lobe_probs(m, &pm, &pd, &pg);
     int refracted = L.z < 0.0f;
     v3 H; int validRefraction = 0;
     if (refracted) {
@@ -627,11 +632,8 @@ static Eval eval_bsdf(const Mat *m, const OrcScene *sc, const OrcConfig *cfg, v3
 }
 /* :94-165 */
 static BSample sample_bsdf(const Mat *m, const OrcScene *sc, const OrcConfig *cfg, Rng *rng, v3 V, v3 H) {
-    float pm = m->Metallic;
-    float pd = (1.0f - m->Metallic) * (1.0f - m->Transmission);
-    float pg = (1.0f - m->Metallic) * m->Transmission;
-    float sum = pm + pd + pg;
-    pm /= sum; pd /= sum; pg /= sum;
+    float pm, pd, pg;
+    lobe_probs(m, &pm, &pd, &pg);
     (void)pg;
     float F = orc_dielectric_fresnel(v3dot(V, H), m->Eta);
     float x1 = rng_f(rng);
@@ -1436,17 +1438,63 @@ static int scattered_in_volume(const OrcScene *sc, const OrcConfig *cfg, Payload
 /* ------------------------------------------------------------------------------------------------
  * ClosestHit: SH/ClosestHit.slang:20-378
  * ---------------------------------------------------------------------------------------------- */
+/* The parts of closest_hit that orc_shade_query runs too, so that the render path and the query path cannot drift apart. */
+/* :40-67: surface, material, isLight, rotated tangents */
+static int hit_surface(const OrcScene *sc, const OrcConfig *cfg, uint32_t inst, uint32_t prim, float bu, float bv, v3 rayDir, Surface *sf, Mat *m) {
+    const OrcMaterial *cm = &sc->d.materials[sc->d.instances[inst].material];
+    surface_init(sf, sc, cfg, inst, prim, bu, bv, rayDir, &sc->d.textures[cm->NormalTextureIndex]);
+    material_init(m, sc, cfg, cm, sf);
+    int isLight = m->EmissiveColor.x > 0.0f || m->EmissiveColor.y > 0.0f || m->EmissiveColor.z > 0.0f;  /* :65 */
+    surface_rotate_tangents(sf, m->AnisotropyRotation);                        /* :67 */
+    return isLight;
+}
+/* BSDF sampling :191-204: V in tangent space, the VNDF half vector and the sampled direction */
+static BSample hit_sample_bsdf(const OrcScene *sc, const OrcConfig *cfg, const Surface *sf, const Mat *m, Rng *rng, v3 rayDir, v3 *V, v3 *H) {
+    *V = surf_world_to_tangent(sf, v3normalize(v3neg(rayDir)));
+    *H = rng_ggx_vndf(rng, *V, m->Ax, m->Ay);
+    return sample_bsdf(m, sc, cfg, rng, *V, *H);
+}
+/* emission :265-317 of a hit at Depth `depth` reached from `origin` with BSDF pdf `pdf` */
+static v3 hit_emission(const OrcScene *sc, const OrcConfig *cfg, uint32_t inst, const Surface *sf, const Mat *m, int isLight, uint32_t depth, v3 origin, float pdf) {
+    v3 e = V3(0, 0, 0);
+    if (cfg->EnableMeshMIS) {
+        if (depth == 0 && isLight) {
+            e = v3add(e, m->EmissiveColor);
+        } else if (isLight) {
+            v3 w1 = xf_point(sc->xf[inst].o2w, sf->P1), w2 = xf_point(sc->xf[inst].o2w, sf->P2), w3 = xf_point(sc->xf[inst].o2w, sf->P3);
+            float area = v3length(v3cross(v3sub(w2, w1), v3sub(w3, w1))) * 0.5f;
+            v3 dl = v3sub(sf->WorldPos, origin);
+            float d2 = v3dot(dl, dl);
+            float cosTheta = fabsf(v3dot(sf->Normal, v3normalize(v3sub(origin, sf->WorldPos))));
+            uint32_t triCount = 0;
+            for (uint32_t i = 0; i < sc->n_emissive; i++) if (sc->emissive[i].instance == inst) { triCount = sc->emissive[i].tri_count; break; }
+            float lp = (1.0f / (float)sc->n_emissive) * (1.0f / (float)triCount) * (1.0f / area) * (d2 / cosTheta);
+            lp = fmaxf(lp, cfg->EmissiveMeshSamplingPDFBias);
+            e = v3add(e, v3scale(m->EmissiveColor, power_heuristic(pdf, lp)));
+        }
+    } else {
+        e = v3add(e, m->EmissiveColor);
+    }
+    return e;
+}
+/* sky draw :125-131: direction (world, and returned in tangent space) and radiance | pdf, radiance scaled once more by the intensity (Q7) */
+static v3 hit_sky_draw(const OrcScene *sc, const OrcConfig *cfg, const Surface *sf, Rng *rng, v3 *toSkyW, v4 *sky) {
+    importance_sample_sky(sc, cfg, rng, toSkyW, sky);
+    sky->x *= cfg->EnvironmentIntensity; sky->y *= cfg->EnvironmentIntensity; sky->z *= cfg->EnvironmentIntensity;
+    return surf_world_to_tangent(sf, *toSkyW);
+}
+/* one NEE term :341-344, :366-369: BxDF * T * radiance / pdf, MIS-weighted */
+static v3 nee_term(Eval e, v3 T, v4 lv) {
+    v3 c = v3divs(v3mul(v3mul(e.BxDF, T), V3(lv.x, lv.y, lv.z)), lv.w);
+    return v3scale(c, power_heuristic(lv.w, e.PDF));
+}
+
 static void closest_hit(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v3 rayDir, const Hit *h, OrcCounters *cnt) {
     pl->Emitted = V3(0, 0, 0);                                                  /* :24 */
     uint32_t inst = sc->tris[h->tri].inst, prim = sc->tris[h->tri].prim;
-    const OrcInstance *in = &sc->d.instances[inst];
-    const OrcMaterial *cm = &sc->d.materials[in->material];
     Surface sf;
-    surface_init(&sf, sc, cfg, inst, prim, h->u, h->v, rayDir, &sc->d.textures[cm->NormalTextureIndex]);
     Mat m;
-    material_init(&m, sc, cfg, cm, &sf);
-    int isLight = m.EmissiveColor.x > 0.0f || m.EmissiveColor.y > 0.0f || m.EmissiveColor.z > 0.0f;  /* :65 */
-    surface_rotate_tangents(&sf, m.AnisotropyRotation);                        /* :67 */
+    int isLight = hit_surface(sc, cfg, inst, prim, h->u, h->v, rayDir, &sf, &m);
 
     if (pl->InMedium) {                                                         /* :80-116 (Q6) */
         float dist = v3length(v3sub(pl->Origin, sf.WorldPos));
@@ -1469,9 +1517,7 @@ static void closest_hit(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v
     /* sky NEE :125-147 */
     v3 toSkyW = V3(0, 0, 0), toSkyT = V3(0, 0, 0); v4 sky = { 0, 0, 0, 0 }; int canHitSky = 0;
     if (cfg->EnableSkyMIS) {
-        importance_sample_sky(sc, cfg, &pl->Sampler, &toSkyW, &sky);
-        sky.x *= cfg->EnvironmentIntensity; sky.y *= cfg->EnvironmentIntensity; sky.z *= cfg->EnvironmentIntensity; /* Q7 */
-        toSkyT = surf_world_to_tangent(&sf, toSkyW);
+        toSkyT = hit_sky_draw(sc, cfg, &sf, &pl->Sampler, &toSkyW, &sky);
         uint32_t t0, t1;
         canHitSky = !does_ray_intersect(sc, v3add(sf.WorldPos, v3scale(sf.Normal, 1e-5f)), toSkyW, &t0, &t1, &cnt->shadow_rays);
         if (!canHitSky) { v4 z = { 0, 0, 0, 0 }; sky = z; }
@@ -1489,11 +1535,8 @@ static void closest_hit(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v
             if (!canHitLight) { v4 z = { 0, 0, 0, 0 }; light = z; }
         }
     }
-    /* BSDF sampling :191-204 */
-    v3 V = v3normalize(v3neg(rayDir));
-    V = surf_world_to_tangent(&sf, V);
-    v3 H = rng_ggx_vndf(&pl->Sampler, V, m.Ax, m.Ay);
-    BSample ss = sample_bsdf(&m, sc, cfg, &pl->Sampler, V, H);
+    v3 V, H;
+    BSample ss = hit_sample_bsdf(sc, cfg, &sf, &m, &pl->Sampler, rayDir, &V, &H);
     int wasRefracted = ss.L.z < 0.0f;
     v3 scatterW = surf_tangent_to_world(&sf, ss.L);
     if (!wasRefracted && v3dot(scatterW, sf.GeometryNormal) < 0.0f) { ss.PDF = 0.0f; ss.BxDF = V3(0, 0, 0); }   /* :220-225 */
@@ -1509,25 +1552,7 @@ static void closest_hit(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v
     Eval lightEval = { V3(0, 0, 0), 0.0f };
     if (cfg->EnableMeshMIS && canHitLight && !isLight) lightEval = eval_bsdf(&m, sc, cfg, V, toLightT); /* :250-256 */
 
-    /* emission :265-317 */
-    if (cfg->EnableMeshMIS) {
-        if (pl->Depth == 0 && isLight) {
-            pl->Emitted = v3add(pl->Emitted, m.EmissiveColor);
-        } else if (isLight) {
-            v3 w1 = xf_point(sc->xf[inst].o2w, sf.P1), w2 = xf_point(sc->xf[inst].o2w, sf.P2), w3 = xf_point(sc->xf[inst].o2w, sf.P3);
-            float area = v3length(v3cross(v3sub(w2, w1), v3sub(w3, w1))) * 0.5f;
-            v3 dl = v3sub(sf.WorldPos, pl->Origin);
-            float d2 = v3dot(dl, dl);
-            float cosTheta = fabsf(v3dot(sf.Normal, v3normalize(v3sub(pl->Origin, sf.WorldPos))));
-            uint32_t triCount = 0;
-            for (uint32_t i = 0; i < sc->n_emissive; i++) if (sc->emissive[i].instance == inst) { triCount = sc->emissive[i].tri_count; break; }
-            float lp = (1.0f / (float)sc->n_emissive) * (1.0f / (float)triCount) * (1.0f / area) * (d2 / cosTheta);
-            lp = fmaxf(lp, cfg->EmissiveMeshSamplingPDFBias);
-            pl->Emitted = v3add(pl->Emitted, v3scale(m.EmissiveColor, power_heuristic(pl->PDF, lp)));
-        }
-    } else {
-        pl->Emitted = v3add(pl->Emitted, m.EmissiveColor);
-    }
+    pl->Emitted = v3add(pl->Emitted, hit_emission(sc, cfg, inst, &sf, &m, isLight, pl->Depth, pl->Origin, pl->PDF));   /* :265-317 */
     /* payload write :319-324 */
     float off = -1e-3f * (wasRefracted ? 1.0f : 0.0f) + 1e-3f * (wasRefracted ? 0.0f : 1.0f);
     pl->Origin = v3add(sf.WorldPos, v3scale(sf.Normal, off));
@@ -1536,21 +1561,80 @@ static void closest_hit(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v
     pl->PDF = ss.PDF;
     /* NEE accumulation :326-372 (volume transmittance == 1 with VolumesCount == 0, SH/Volume.slang:419-446) */
     if (cfg->EnableSkyMIS && canHitSky) {
-        float pdf = sky.w;
         v3 T = v3s(cfg->VolumesCount ? volumes_transmittance(cfg, &pl->Sampler, pl->Origin, toSkyW, 0.0f) : 1.0f);     /* :332-333 */
         if (cfg->EnableAtmosphere) T = v3mul(T, atm_transmittance_nee(cfg, pl, pl->Origin, toSkyW));    /* :335-349: consumes random numbers whenever the sky is visible */
-        if (sky.w > 0.0f && skyEval.PDF > 0.0f) {
-            v3 c = v3divs(v3mul(v3mul(skyEval.BxDF, T), V3(sky.x, sky.y, sky.z)), pdf);
-            pl->Emitted = v3add(pl->Emitted, v3scale(c, power_heuristic(pdf, skyEval.PDF)));
-        }
+        if (sky.w > 0.0f && skyEval.PDF > 0.0f) pl->Emitted = v3add(pl->Emitted, nee_term(skyEval, T, sky));
     }
     if (cfg->EnableMeshMIS && !isLight && canHitLight && light.w > 0.0f && lightEval.PDF > 0.0f) {
         const float T = cfg->VolumesCount ? volumes_transmittance(cfg, &pl->Sampler, pl->Origin, toLightW, 0.0f) : 1.0f;    /* :364 */
-        v3 c = v3divs(v3mul(v3scale(lightEval.BxDF, T), V3(light.x, light.y, light.z)), light.w);
-        pl->Emitted = v3add(pl->Emitted, v3scale(c, power_heuristic(light.w, lightEval.PDF)));
+        pl->Emitted = v3add(pl->Emitted, nee_term(lightEval, v3s(T), light));
     }
     int invalid = ss.PDF <= 0.0f;                                               /* :375-376 */
     pl->Depth = ORC_MAX_DEPTH * (invalid ? 1u : 0u) + (pl->Depth + 1u * (invalid ? 0u : 1u));
+}
+
+/* One hit's shading step (pt_oracle.h): closest_hit's draws in its order, without the shadow rays, at Depth 1 outside any medium. */
+static void put3(float *o, v3 a) { o[0] = a.x; o[1] = a.y; o[2] = a.z; }
+static void put_eval(float *o, Eval e) { put3(o, e.BxDF); o[3] = e.PDF; }
+static void put_bits(float *o, uint32_t u) { memcpy(o, &u, 4); }
+void orc_shade_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv2, const float *dir3,
+                     const float *org3, const float *pay_pdf, const uint32_t *rng, const float *L3, float *out) {
+    for (uint32_t i = 0; i < n; i++) {
+        float *o = out + (size_t)i * ORC_SQ_STRIDE;
+        memset(o, 0, ORC_SQ_STRIDE * sizeof(float));
+        const v3 rayDir = v3normalize(V3(dir3[3 * i], dir3[3 * i + 1], dir3[3 * i + 2]));
+        Rng r = { rng[i] };
+        Surface sf; Mat m;
+        const int isLight = hit_surface(sc, cfg, inst[i], prim[i], uv2[2 * i], uv2[2 * i + 1], rayDir, &sf, &m);
+        put3(o + ORC_SQ_N, sf.Normal); put3(o + ORC_SQ_T, sf.Tangent); put3(o + ORC_SQ_B, sf.Bitangent); put3(o + ORC_SQ_NG, sf.GeometryNormal);
+        o[ORC_SQ_INSIDE] = (float)sf.HitFromInside;
+        float pm, pd, pg;
+        lobe_probs(&m, &pm, &pd, &pg);
+        o[ORC_SQ_AX] = m.Ax; o[ORC_SQ_AY] = m.Ay; o[ORC_SQ_ETA] = m.Eta; o[ORC_SQ_PM] = pm; o[ORC_SQ_PD] = pd; o[ORC_SQ_PG] = pg;
+        put3(o + ORC_SQ_BASECOLOR, m.BaseColor); o[ORC_SQ_ROUGHNESS] = m.Roughness;
+        put3(o + ORC_SQ_EMITTED, hit_emission(sc, cfg, inst[i], &sf, &m, isLight, 1u, V3(org3[3 * i], org3[3 * i + 1], org3[3 * i + 2]), pay_pdf[i]));
+        const v3 V = surf_world_to_tangent(&sf, v3normalize(v3neg(rayDir)));
+        if (cfg->EnableSkyMIS) {                                                /* :125-147 */
+            v3 w; v4 lv;
+            const v3 t = hit_sky_draw(sc, cfg, &sf, &r, &w, &lv);
+            put3(o + ORC_SQ_SKY_L, t); put3(o + ORC_SQ_SKY_LV, V3(lv.x, lv.y, lv.z)); o[ORC_SQ_SKY_LV + 3] = lv.w;
+            if (lv.w > 0.0f) {
+                const Eval e = eval_bsdf(&m, sc, cfg, V, t);
+                put_eval(o + ORC_SQ_SKY_EVAL, e);
+                if (e.PDF > 0.0f) put3(o + ORC_SQ_SKY_C, nee_term(e, v3s(1.0f), lv));
+            }
+        }
+        put_bits(o + ORC_SQ_LIGHT_GID, 0xFFFFFFFFu);
+        if (cfg->EnableMeshMIS && !isLight) {                                   /* :154-184 */
+            v3 w; v4 lv; uint32_t lt, li;
+            sample_emissive(sc, &r, sf.WorldPos, &w, &lv, &lt, &li);
+            o[ORC_SQ_LIGHT_LV] = lv.x; o[ORC_SQ_LIGHT_LV + 1] = lv.y; o[ORC_SQ_LIGHT_LV + 2] = lv.z; o[ORC_SQ_LIGHT_LV + 3] = lv.w;
+            if (li != 0xFFFFFFFFu) put_bits(o + ORC_SQ_LIGHT_GID, sc->xf[li].tri_base + lt);
+            if (lv.w > 0.0f) {
+                const v3 t = surf_world_to_tangent(&sf, w);
+                put3(o + ORC_SQ_LIGHT_L, t);
+                const Eval e = eval_bsdf(&m, sc, cfg, V, t);
+                put_eval(o + ORC_SQ_LIGHT_EVAL, e);
+                if (e.PDF > 0.0f) put3(o + ORC_SQ_LIGHT_C, nee_term(e, v3s(1.0f), lv));
+            }
+        }
+        v3 V2, H;
+        BSample ss = hit_sample_bsdf(sc, cfg, &sf, &m, &r, rayDir, &V2, &H);
+        put3(o + ORC_SQ_V, V2); put3(o + ORC_SQ_H, H);
+        put3(o + ORC_SQ_BSDF_L, ss.L); o[ORC_SQ_BSDF_EVAL] = ss.BxDF.x; o[ORC_SQ_BSDF_EVAL + 1] = ss.BxDF.y; o[ORC_SQ_BSDF_EVAL + 2] = ss.BxDF.z; o[ORC_SQ_BSDF_EVAL + 3] = ss.PDF;
+        o[ORC_SQ_VALID] = (ss.L.x != 0.0f || ss.L.y != 0.0f || ss.L.z != 0.0f) ? 1.0f : 0.0f;
+        const int wasRefracted = ss.L.z < 0.0f;                                 /* :220-238 */
+        const v3 scatterW = surf_tangent_to_world(&sf, ss.L);
+        const int rejected = !wasRefracted && v3dot(scatterW, sf.GeometryNormal) < 0.0f;
+        if (rejected) { ss.PDF = 0.0f; ss.BxDF = V3(0, 0, 0); }
+        put3(o + ORC_SQ_SCATTER, scatterW); put_eval(o + ORC_SQ_SAMPLE, (Eval){ ss.BxDF, ss.PDF });
+        o[ORC_SQ_REFRACTED] = (float)wasRefracted; o[ORC_SQ_ENTERED] = (float)(wasRefracted && !sf.HitFromInside); o[ORC_SQ_REJECTED] = (float)rejected;
+        if (L3) {
+            const v3 t = surf_world_to_tangent(&sf, V3(L3[3 * i], L3[3 * i + 1], L3[3 * i + 2]));
+            put3(o + ORC_SQ_USER_L, t); put_eval(o + ORC_SQ_USER_EVAL, eval_bsdf(&m, sc, cfg, V, t));
+        }
+        put_bits(o + ORC_SQ_RNG, r.seed);
+    }
 }
 
 /* Miss: SH/Miss.slang:8-76 */

@@ -167,6 +167,53 @@ void      orc_scene_world_triangles(const OrcScene *s, float *out9, uint32_t *in
 void orc_trace_closest(const OrcScene *s, uint32_t n, const float *org3, const float *dir3, float tmin, float tmax,
                        int use_bvh, float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out2);
 
+/* One hit's shading step, as closest_hit runs it (SH/ClosestHit.slang:40-238) but without the shadow rays: record i is the hit of
+ * instance inst[i], primitive prim[i] at barycentrics uv2[2i..], reached along dir3 from org3 with BSDF pdf pay_pdf[i] at Depth 1, outside
+ * any medium, drawing from rng[i].  The sky draw, the light draw and the BSDF draw are made in that order; each drawn direction is
+ * evaluated with EvaluateBSDF, and the NEE term c is the one the shader adds when the shadow ray is unoccluded.  L3 (optional): one more
+ * world-space direction per record to evaluate.  out: n records of ORC_SQ_STRIDE floats, laid out like B200PT_SQ_* of include/b200pt.h
+ * (vectors in tangent space unless named otherwise; LIGHT_GID and RNG hold u32 bits). */
+#define ORC_SQ_N          0    /* shading normal, world */
+#define ORC_SQ_T          3
+#define ORC_SQ_B          6
+#define ORC_SQ_NG         9    /* geometry normal, world */
+#define ORC_SQ_INSIDE     12
+#define ORC_SQ_AX         13
+#define ORC_SQ_AY         14
+#define ORC_SQ_ETA        15
+#define ORC_SQ_PM         16
+#define ORC_SQ_PD         17
+#define ORC_SQ_PG         18
+#define ORC_SQ_BASECOLOR  19
+#define ORC_SQ_ROUGHNESS  22
+#define ORC_SQ_V          23
+#define ORC_SQ_H          26
+#define ORC_SQ_EMITTED    29   /* emission term */
+#define ORC_SQ_SKY_L      32
+#define ORC_SQ_SKY_LV     35   /* radiance, pdf */
+#define ORC_SQ_SKY_EVAL   39   /* BxDF, PDF */
+#define ORC_SQ_SKY_C      43
+#define ORC_SQ_LIGHT_L    46
+#define ORC_SQ_LIGHT_LV   49
+#define ORC_SQ_LIGHT_EVAL 53
+#define ORC_SQ_LIGHT_C    57
+#define ORC_SQ_LIGHT_GID  60
+#define ORC_SQ_BSDF_L     61   /* 0 when the direction is invalid */
+#define ORC_SQ_BSDF_EVAL  64
+#define ORC_SQ_VALID      68
+#define ORC_SQ_SCATTER    69   /* world */
+#define ORC_SQ_SAMPLE     72   /* BxDF, PDF after the geometry-normal rejection */
+#define ORC_SQ_REFRACTED  76
+#define ORC_SQ_ENTERED    77
+#define ORC_SQ_REJECTED   78
+#define ORC_SQ_USER_L     79
+#define ORC_SQ_USER_EVAL  82
+#define ORC_SQ_RNG        86
+#define ORC_SQ_CLASS      87   /* GPU only: the material class whose kernel ran */
+#define ORC_SQ_STRIDE     88
+void orc_shade_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv2, const float *dir3,
+                     const float *org3, const float *pay_pdf, const uint32_t *rng, const float *L3, float *out);
+
 /* One reference dispatch sequence: frames [frame0, frame0+nframes) with Seed_f = PCG_HASH(base_seed + f)
  * (SURVEY 8d; the reference's own seed is wall-clock, PT/PathTracer.cpp:127-140), running-mean accumulate
  * into image (RGBA32F, W*H*4) exactly as SH/RayGen.slang:130-159.  Only rows y with

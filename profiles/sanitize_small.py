@@ -59,4 +59,14 @@ def _queries(name):                                                 # b200pt_tra
                 except pt.B200ptError: pass                             # shape absent in this scene (flat walk, BVH4, shared memory)
     print(name, "trace_query ok")
 _queries("cornell_box"); _queries("viking_room")
+def _shade(name):                                                   # b200pt_shade_query: every class instantiation and the general one, with an extra L
+    S = util.oracle_scene(name); T = util.product_tracer(name, 16, 16)
+    rng = np.random.default_rng(2)
+    o = (rng.normal(size=(300, 3)) * 0.3).astype(np.float32); d = rng.normal(size=(300, 3)); d = (d / np.linalg.norm(d, axis=1, keepdims=True)).astype(np.float32)
+    t, prim, inst, uv = S.trace_closest(o, d, 1e-3, 1e5); h = t > 0
+    for general in (False, True):
+        r = T.shade_query(inst[h], prim[h], uv[h], d[h], o[h], 0.5, np.arange(h.sum()), L=-d[h], force_general=general)
+        assert r.shape == (h.sum(), 88)
+    print(name, "shade_query ok")
+_shade("cornell_box"); _shade("cornell_box_glass")
 print("sanitize_small done")

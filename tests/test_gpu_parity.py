@@ -698,8 +698,27 @@ def _mixed_materials_edit(T):
     m = T.get_material(3 % n); m.Metallic = 0.4; m.Transmission = 0.3; m.Roughness = 0.4; T.set_material(3 % n, m)
 
 
+def _cornell_new_materials():
+    """Cornell with its walls and boxes swapped for materials no fixture has: anisotropic metal with rotation, a 0.5 / 0.5 mixed lobe, rough
+    glass at IOR 1.33 and 2.4, textured metallic (2x2, so the class is MC_GENERAL by texel)"""
+    sc = dict(util.scene_dict("cornell_box"))
+    tex = list(sc["textures"]) + [np.array([[[0], [255]], [[64], [191]]], np.uint8)]
+    mats = np.concatenate([sc["materials"], sc["materials"][:2]]).copy()
+    def put(i, **kw):
+        for k, v in kw.items(): mats[k][i] = v
+    put(0, Metallic=1.0, Roughness=0.35, Anisotropy=0.8, AnisotropyRotation=30.0, BaseColor=(0.9, 0.6, 0.3))
+    put(1, Metallic=0.5, Transmission=0.5, Roughness=0.4, SpecularColor=(0.9, 0.7, 0.5))
+    put(2, Transmission=1.0, IOR=1.33, Roughness=0.3)
+    put(4, Transmission=1.0, IOR=2.4, Roughness=0.15)
+    put(5, Metallic=1.0, Roughness=0.5, MetallicTextureIndex=len(tex) - 1)
+    inst = [(x, m, mat) for x, m, mat in sc["instances"]]
+    for k, mat in ((3, 4), (4, 5)): inst[k] = (inst[k][0], inst[k][1], mat)
+    sc.update(materials=mats, textures=tex, instances=inst)
+    return sc
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,depth", [("cornell_box", 8), ("cornell_box_glass", 12)])
+@pytest.mark.parametrize("name,depth", [("cornell_box", 8), ("cornell_box_glass", 12), ("cornell_new_materials", 8)])
 def test_fused_bounce_kernel_and_class_queues_return_the_same_image(pt, name, depth, monkeypatch):
     """The material-class hit queues (k_extend sorts hits by lobe set, k_shade_hit<CLASS> compiles the dead lobes out) and the fused shading
     kernel of shared-memory scenes (k_shade_hit<CLASS, ., true>: NEE shadow queries and the path epilogue inside the shading kernel) are
@@ -708,20 +727,32 @@ def test_fused_bounce_kernel_and_class_queues_return_the_same_image(pt, name, de
     exactly 0 only ever adds exact zeros, so images agree bit for bit except where the compiler contracts an a*b+c differently in two
     instantiations (a last-bit difference that a path may amplify across a branch; measured 98.6 % identical pixels on the four-class Cornell
     box after 4 frames, 94.4 % with a relative L2 of 1e-9 on the glass scene in big shared-memory mode): >= 90 % of the pixels identical,
-    rel. L2 < 1e-3.  The glass scene runs in big mode (opt-in, B200PT_SMEM_BIG=1), so the 512-thread fused kernel is compared as well."""
+    rel. L2 < 1e-3.  The glass scene runs in big mode (opt-in, B200PT_SMEM_BIG=1), so the 512-thread fused kernel is compared as well.
+    cornell_new_materials (_cornell_new_materials) is also compared with the oracle in every setting: >= 99.5 % of the pixels within 1e-4,
+    rel. L2 < 1e-3."""
     if name == "cornell_box_glass": monkeypatch.setenv("B200PT_SMEM_BIG", "1")
     W, H, frames = 192, 128, 4
     out = {}
     for fuse in ("1", "0"):
         for classes in ("1", "0"):
             monkeypatch.setenv("B200PT_FUSE", fuse); monkeypatch.setenv("B200PT_CLASSES", classes)
-            T = util.product_tracer(name, W, H, MaxDepth=depth)
-            _mixed_materials_edit(T)
+            if name == "cornell_new_materials": T = util.product_tracer("cornell_box", W, H, scene=_cornell_new_materials(), MaxDepth=depth)
+            else:
+                T = util.product_tracer(name, W, H, MaxDepth=depth)
+                _mixed_materials_edit(T)
             T.path_trace(frames, util.BASE_SEED)
             c = T.counters()
             out[fuse, classes] = (T.get_hdr().copy(), {k: c[k] for k in ("paths", "extend_rays", "surface_hits", "misses", "shadow_rays", "medium_events")})
     ref_img, ref_c = out["0", "0"]
     assert np.isfinite(ref_img).all() and ref_img[..., :3].max() > 0
+    if name == "cornell_new_materials":
+        raw, env_pdf, alias = util.env_small()
+        orc_img, _ = orc.Scene(_cornell_new_materials(), env_pdf, alias, util.luts()).render(util.oracle_config("cornell_box", MaxDepth=depth), W, H, frames, util.BASE_SEED)
+        for k, (img, _) in out.items():
+            a, b = orc_img[..., :3].astype(np.float64), img[..., :3].astype(np.float64)
+            close = np.all(np.abs(a - b) <= 1e-4 * np.maximum(np.abs(a), 1e-2), axis=-1).mean()
+            print(f"new materials against the oracle, FUSE={k[0]} CLASSES={k[1]}: {close:.5f} of the pixels agree, rel. L2 {util.rel_l2(b, a):.2e}")
+            assert close >= 0.995 and util.rel_l2(b, a) < 1e-3, (k, close)
     for k, (img, c) in out.items():
         same = np.all(img.view(np.uint32) == ref_img.view(np.uint32), axis=-1).mean()
         assert same >= 0.90 and util.rel_l2(img[..., :3], ref_img[..., :3]) < 1e-3, (k, same, util.rel_l2(img[..., :3], ref_img[..., :3]))

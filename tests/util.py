@@ -52,12 +52,13 @@ ATMOSPHERE_KEYS = ("EnableAtmosphere", "PlanetPosition", "PlanetRadius", "Atmosp
 _ORC2PT = {"SampleCount": "SamplesPerFrame", "EnvironmentIntensity": "SkyIntensity", "ScreenSplitCount": "ScreenChunkCount"}
 
 
-def product_tracer(name, W, H, env=None, device=0, **cfg_kw):
-    """PathTracer handle (C-ABI) with the same scene / env / LUTs / camera / config as oracle_scene + oracle_config."""
+def product_tracer(name, W, H, env=None, device=0, scene=None, **cfg_kw):
+    """PathTracer handle (C-ABI) with the same scene / env / LUTs / camera / config as oracle_scene + oracle_config (scene: a scene dict
+    to use instead of the fixture `name`)."""
     import vpt_b200 as pt
     raw, env_pdf, alias = env if env is not None else env_small()
     t = pt.PathTracer(device)
-    t.set_scene(scene_dict(name))
+    t.set_scene(scene_dict(name) if scene is None else scene)
     t.set_env_map(raw)
     t.set_luts(*luts())
     cfg = pt.default_config()

@@ -189,6 +189,7 @@ def lib():
             "b200pt_scene_stats": [C.c_void_p] + [C.POINTER(C.c_uint32)] * 4,
             "b200pt_trace_stats": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p],
             "b200pt_trace_query": [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32] + [C.c_void_p] * 12,
+            "b200pt_shade_query": [C.c_void_p, C.c_int32, C.c_uint32] + [C.c_void_p] * 9,
             "b200pt_bake_lut": [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p],
             "b200pt_bake_luts_to_dir": [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32],
             "b200pt_decode_image_file": [C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_void_p)],
@@ -221,6 +222,12 @@ class Atmosphere(C.Structure):      # b200pt_atmosphere (include/b200pt.h)
                 ("RayleighScatteringCoefficientMultiplier", C.c_float * 3), ("MieScatteringCoefficientMultiplier", C.c_float * 3),
                 ("OzoneAbsorptionCoefficientMultiplier", C.c_float * 3), ("RayleighDensityFalloff", C.c_float), ("MieDensityFalloff", C.c_float),
                 ("OzoneDensityFalloff", C.c_float), ("OzonePeak", C.c_float), ("SunColor", C.c_float * 3)]
+
+
+# record offsets of b200pt_shade_query (B200PT_SQ_* in include/b200pt.h; tests/test_shading_queries.py checks that they agree)
+SQ = dict(N=0, T=3, B=6, NG=9, INSIDE=12, AX=13, AY=14, ETA=15, PM=16, PD=17, PG=18, BASECOLOR=19, ROUGHNESS=22, V=23, H=26, EMITTED=29,
+          SKY_L=32, SKY_LV=35, SKY_EVAL=39, SKY_C=43, LIGHT_L=46, LIGHT_LV=49, LIGHT_EVAL=53, LIGHT_C=57, LIGHT_GID=60, BSDF_L=61, BSDF_EVAL=64,
+          VALID=68, SCATTER=69, SAMPLE=72, REFRACTED=76, ENTERED=77, REJECTED=78, USER_L=79, USER_EVAL=82, RNG=86, CLASS=87, STRIDE=88)
 
 
 def declared_symbols():
@@ -683,6 +690,21 @@ class PathTracer:
                                            _p(t), _p(prim), _p(inst), _p(uv), _p(occ), _p(st) if stats else None))
         if k == 0: return dict(t=t, prim=prim, inst=inst, uv=uv, stats=st)
         return dict(occluded=occ.astype(bool), stats=st)
+
+    def shade_query(self, inst, prim, uv, dirs, org, pay_pdf, rng, L=None, force_general=False):
+        """b200pt_shade_query: one shading step of k_shade_hit per hit.  Returns [n, B200PT_SQ_STRIDE] float32 records; SQ names the offsets."""
+        inst = np.ascontiguousarray(inst, np.uint32).reshape(-1); n = len(inst)
+        prim = np.ascontiguousarray(np.broadcast_to(np.asarray(prim, np.uint32), (n,)))
+        uv = np.ascontiguousarray(np.broadcast_to(np.asarray(uv, np.float32), (n, 2)))
+        dirs = np.ascontiguousarray(np.broadcast_to(np.asarray(dirs, np.float32), (n, 3)))
+        org = np.ascontiguousarray(np.broadcast_to(np.asarray(org, np.float32), (n, 3)))
+        pay_pdf = np.ascontiguousarray(np.broadcast_to(np.asarray(pay_pdf, np.float32), (n,)))
+        rng = np.ascontiguousarray(np.broadcast_to(np.asarray(rng, np.uint32), (n,)))
+        Lw = None if L is None else np.ascontiguousarray(np.broadcast_to(np.asarray(L, np.float32), (n, 3)))
+        out = np.zeros((n, SQ["STRIDE"]), np.float32)
+        self._ck(self.L.b200pt_shade_query(self.h, int(bool(force_general)), n, _p(inst), _p(prim), _p(uv), _p(dirs), _p(org), _p(pay_pdf), _p(rng),
+                                           None if Lw is None else _p(Lw), _p(out)))
+        return out
 
     def scene_stats(self):
         a, b, c, d = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()

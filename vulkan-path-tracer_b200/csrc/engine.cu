@@ -1025,6 +1025,45 @@ void Engine::trace_query(int shape, int kind, bool fma, uint32_t n, const float 
     for (void *p : bufs) cudaFree(p);
     CK(e); CK(cudaGetLastError());
 }
+void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv, const float *dir, const float *org,
+                         const float *pay_pdf, const uint32_t *rng, const float *L, float *out) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!has_env_ || !has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "shade_query: no environment map or no lookup tables" };
+    if (!n) return;
+    if (ds_.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: scenes with volumes or the atmosphere are not supported" };
+    std::vector<uint32_t> gid(n);
+    for (uint32_t i = 0; i < n; i++) {                                      // (instance, primitive) -> global triangle id, as k_world_tris numbers them
+        if (inst[i] >= h_instances_.size() || prim[i] >= h_meshes_[h_instances_[inst[i]].mesh].tri_count)
+            throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: instance or primitive out of range" };
+        gid[i] = h_instances_[inst[i]].tri_base + prim[i];
+    }
+    std::vector<void *> bufs;
+    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
+    auto dev = [&](size_t bytes, const void *src) -> void * {
+        void *p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) fail(e);
+        bufs.push_back(p);
+        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
+        return p;
+    };
+    ShadeQuery q{};
+    q.n = n; q.force_general = force_general;
+    q.gid = (const uint32_t *)dev((size_t)n * 4, gid.data()); q.rng = (const uint32_t *)dev((size_t)n * 4, rng);
+    q.uv = (const float *)dev((size_t)n * 8, uv); q.dir = (const float *)dev((size_t)n * 12, dir); q.org = (const float *)dev((size_t)n * 12, org);
+    q.pay_pdf = (const float *)dev((size_t)n * 4, pay_pdf);
+    if (L) q.L = (const float *)dev((size_t)n * 12, L);
+    const size_t out_bytes = (size_t)n * B200PT_SQ_STRIDE * sizeof(float);
+    q.out = (float *)dev(out_bytes, nullptr);
+    const int r = launch_shade_query(ds_, make_dev_config(), q, stream_);
+    if (r != 0) fail((cudaError_t)r);
+    cudaError_t e = cudaMemcpyAsync(out, q.out, out_bytes, cudaMemcpyDeviceToHost, stream_);
+    if (e != cudaSuccess) fail(e);
+    e = cudaStreamSynchronize(stream_);
+    for (void *p : bufs) cudaFree(p);
+    CK(e); CK(cudaGetLastError());
+}
 // LookupTableCalculator::CalculateTable (PT/LookupTableCalculator.cpp:44-157) on this engine's device and stream.
 // slices == 0 picks enough dispatch slices to give every SM ~2048 resident threads.
 void Engine::bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out_host, float *elapsed_ms) {

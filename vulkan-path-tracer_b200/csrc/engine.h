@@ -91,6 +91,9 @@ public:
     // b200pt_trace_query (host arrays; see include/b200pt.h)
     void trace_query(int shape, int kind, bool fma, uint32_t n, const float *org, const float *dir, const float *tmin, const float *tmax, const uint32_t *target,
                      const float *tmax_test, float *t, uint32_t *prim, uint32_t *inst, float *uv, uint32_t *occluded, uint32_t *stats);
+    // b200pt_shade_query (host arrays; see include/b200pt.h)
+    void shade_query(bool force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv, const float *dir, const float *org,
+                     const float *pay_pdf, const uint32_t *rng, const float *L, float *out);
     void scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const;
     void bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out_host, float *elapsed_ms);
 

@@ -119,6 +119,12 @@ struct TraceQuery {                           // device arrays of n rays; target
 // Returns cudaError_t as int, or TQ_UNSUPPORTED.
 int launch_trace_query(const LaunchCfg &lc, const DevScene &sc, int bvh4_depth, int shape, int kind, bool fma, const TraceQuery &q, cudaStream_t st);
 
+// ---- shading test hook (shade_query.cu, b200pt_shade_query) ----
+struct ShadeQuery {                           // device arrays of n hits; L may be nullptr; out: n x B200PT_SQ_STRIDE floats
+    uint32_t n; bool force_general; const uint32_t *gid, *rng; const float *uv, *dir, *org, *pay_pdf, *L; float *out;
+};
+int launch_shade_query(const DevScene &sc, const DevConfig &cfg, const ShadeQuery &q, cudaStream_t st);   // cudaError_t as int
+
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
 struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;
                     Bvh4Node *nodes4; uint32_t n_nodes4; int depth4;

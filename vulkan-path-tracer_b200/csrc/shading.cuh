@@ -118,12 +118,21 @@ __device__ __forceinline__ int wrap_repeat(int i, int n) {
 }
 __device__ __forceinline__ int clampi(int i, int lo, int hi) { return i < lo ? lo : (i > hi ? hi : i); }
 
+// UNORM8 texel -> float, correctly rounded like the texture unit's conversion and the host's c / 255 of 1x1 textures (DevMaterial::cbase ..):
+// under -prec-div=false a plain c / 255.0f is the approximate division, off by an ulp for about half of the 256 values, and the per-hit
+// path then differed from the per-material one (k_prepare_materials) on the same texels.  c * (1/255) is off for 126 of the values; one
+// FMA residual step rounds all 256 correctly (checked exhaustively), at two FMAs instead of a full division.
+__device__ __forceinline__ float unorm8(uint8_t c) {
+    const float x = (float)c, r = 0x1.010102p-8f;                           // fp32(1/255)
+    const float q = __fmul_rn(x, r);
+    return __fmaf_rn(__fmaf_rn(-q, 255.0f, x), r, q);
+}
 // RGBA8 / R8 UNORM, bilinear, REPEAT (PT/PathTracer.cpp:84-91). R8 -> (r,0,0,1).
 static __device__ __noinline__ float4 tex_sample_u8(const DevTexture t, float u, float v) {
     const int W = (int)t.w, H = (int)t.h;
     if (W == 1 && H == 1) {     // 1x1 defaults (PT/PathTracer.cpp:1557-1621): bilinear of equal texels is the texel
-        if (t.c == 4) { uchar4 p = *reinterpret_cast<const uchar4 *>(t.data); return make_float4((float)p.x / 255.0f, (float)p.y / 255.0f, (float)p.z / 255.0f, (float)p.w / 255.0f); }
-        return make_float4((float)t.data[0] / 255.0f, 0.0f, 0.0f, 1.0f);
+        if (t.c == 4) { uchar4 p = *reinterpret_cast<const uchar4 *>(t.data); return make_float4(unorm8(p.x), unorm8(p.y), unorm8(p.z), unorm8(p.w)); }
+        return make_float4(unorm8(t.data[0]), 0.0f, 0.0f, 1.0f);
     }
     float x = u * (float)W - 0.5f, y = v * (float)H - 0.5f;
     float fx = floorf(x), fy = floorf(y);
@@ -135,15 +144,15 @@ static __device__ __noinline__ float4 tex_sample_u8(const DevTexture t, float u,
         uchar4 p00 = __ldg(d + (size_t)y0 * W + x0), p10 = __ldg(d + (size_t)y0 * W + x1);
         uchar4 p01 = __ldg(d + (size_t)y1 * W + x0), p11 = __ldg(d + (size_t)y1 * W + x1);
         float4 o;
-        o.x = tex_mix(tex_mix((float)p00.x / 255.0f, (float)p10.x / 255.0f, ax), tex_mix((float)p01.x / 255.0f, (float)p11.x / 255.0f, ax), ay);
-        o.y = tex_mix(tex_mix((float)p00.y / 255.0f, (float)p10.y / 255.0f, ax), tex_mix((float)p01.y / 255.0f, (float)p11.y / 255.0f, ax), ay);
-        o.z = tex_mix(tex_mix((float)p00.z / 255.0f, (float)p10.z / 255.0f, ax), tex_mix((float)p01.z / 255.0f, (float)p11.z / 255.0f, ax), ay);
-        o.w = tex_mix(tex_mix((float)p00.w / 255.0f, (float)p10.w / 255.0f, ax), tex_mix((float)p01.w / 255.0f, (float)p11.w / 255.0f, ax), ay);
+        o.x = tex_mix(tex_mix(unorm8(p00.x), unorm8(p10.x), ax), tex_mix(unorm8(p01.x), unorm8(p11.x), ax), ay);
+        o.y = tex_mix(tex_mix(unorm8(p00.y), unorm8(p10.y), ax), tex_mix(unorm8(p01.y), unorm8(p11.y), ax), ay);
+        o.z = tex_mix(tex_mix(unorm8(p00.z), unorm8(p10.z), ax), tex_mix(unorm8(p01.z), unorm8(p11.z), ax), ay);
+        o.w = tex_mix(tex_mix(unorm8(p00.w), unorm8(p10.w), ax), tex_mix(unorm8(p01.w), unorm8(p11.w), ax), ay);
         return o;
     }
     const uint8_t *d = t.data;
-    float t00 = (float)__ldg(d + (size_t)y0 * W + x0) / 255.0f, t10 = (float)__ldg(d + (size_t)y0 * W + x1) / 255.0f;
-    float t01 = (float)__ldg(d + (size_t)y1 * W + x0) / 255.0f, t11 = (float)__ldg(d + (size_t)y1 * W + x1) / 255.0f;
+    float t00 = unorm8(__ldg(d + (size_t)y0 * W + x0)), t10 = unorm8(__ldg(d + (size_t)y0 * W + x1));
+    float t01 = unorm8(__ldg(d + (size_t)y1 * W + x0)), t11 = unorm8(__ldg(d + (size_t)y1 * W + x1));
     return make_float4(tex_mix(tex_mix(t00, t10, ax), tex_mix(t01, t11, ax), ay), 0.0f, 0.0f, 1.0f);
 }
 // RGBA32F env map, bilinear, REPEAT
