@@ -116,6 +116,18 @@ int32_t b200pt_material_count(b200pt_handle h, uint32_t *out);
 int32_t b200pt_get_material(b200pt_handle h, uint32_t index, b200pt_material *out);   /* GetMaterial */
 int32_t b200pt_set_material(b200pt_handle h, uint32_t index, const b200pt_material *m); /* SetMaterial (PathTracer.cpp:712-810) */
 int32_t b200pt_get_material_name(b200pt_handle h, uint32_t index, char *buf, uint32_t buf_size); /* GetMaterialName */
+/* ---- instance transforms: TLAS::Update (VulkanHelper/Include/Vulkan/TLAS.h:78-85, Source/Vulkan/TLASImpl.cpp:192-293) ----
+ * transforms: count x 16 floats, column-major, the layout of b200pt_instance.Transform, in InstanceIndex order; only rows 0-2 are used.
+ * The update replaces every instance transform -> ResetPathTracing(); camera, config, image size, partition, materials, volumes and the
+ * environment stay.  rebuild == 0 refits the tree in place (same topology, boxes recomputed on the GPU); rebuild != 0 builds the tree
+ * b200pt_set_scene_arrays would build for these transforms (B200PT_BVH_SAH honoured, traversal shape and launch configuration re-chosen).
+ * WRONG_ARGUMENTS: count != instance count, a null pointer or a non-finite entry; NO_SCENE without a scene.  A rejected call changes
+ * nothing.  A failed update restores the previous transforms: a failed rebuild keeps the previous tree, a failed refit refits the tree back
+ * to them (if that fails too, the handle reports NO_SCENE until the next set_scene).  The image equals that of a handle loaded with the
+ * moved scene. */
+int32_t b200pt_instance_count(b200pt_handle h, uint32_t *out);
+int32_t b200pt_get_instance_transforms(b200pt_handle h, float *transforms, uint32_t count);
+int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *transforms, uint32_t count, int32_t rebuild);
 int32_t b200pt_set_camera(b200pt_handle h, const float view_inverse[16], const float projection_inverse[16]); /* SetCameraViewInverse/ProjectionInverse */
 int32_t b200pt_get_camera(b200pt_handle h, float view_inverse[16], float projection_inverse[16]);
 /* the Editor/FlyCamera round trip that produces the matrices the shader really sees (Editor.cpp:45-48,1042-1051; FlyCamera.cpp:84-140) */

@@ -69,4 +69,15 @@ def _shade(name):                                                   # b200pt_sha
         assert r.shape == (h.sum(), 88)
     print(name, "shade_query ok")
 _shade("cornell_box"); _shade("cornell_box_glass")
+def _update(name, inst, env=None):                                  # instance updates: k_refit_slots / k_refit_level (/ k_refit_wide), and the rebuild path
+    for k, v in (env or {}).items(): os.environ[k] = v
+    T = util.product_tracer(name, 40, 30, MaxDepth=5)
+    T.path_trace(1, util.BASE_SEED)
+    xf = T.get_instance_transforms(); xf[inst, 12:15] += (0.3, -0.2, 0.1)
+    for rebuild in (False, True, False):
+        T.update_instance_transforms(xf, rebuild=rebuild); T.path_trace(1, util.BASE_SEED)
+        assert np.isfinite(T.get_hdr()).all()
+    for k in (env or {}): del os.environ[k]
+    print(name, "instance updates ok")
+_update("cornell_box", 5); _update("cornell_box_glass", 6); _update("viking_room", 0, {"B200PT_WIDE": "1"})
 print("sanitize_small done")

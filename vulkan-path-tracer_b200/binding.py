@@ -210,6 +210,8 @@ def lib():
             "b200pt_get_denoise_inputs": [C.c_void_p, C.POINTER(DenoiseParams), C.c_void_p, C.c_void_p, C.c_void_p],
             "b200pt_denoise_image": [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(DenoiseParams), C.c_void_p, C.c_int32],
             "b200pt_post_process_denoised": [C.c_void_p],
+            "b200pt_instance_count": [C.c_void_p, C.POINTER(C.c_uint32)], "b200pt_get_instance_transforms": [C.c_void_p, C.c_void_p, C.c_uint32],
+            "b200pt_update_instance_transforms": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32],
         }
         for name, args in sig.items():
             fn = getattr(L, name); fn.restype = C.c_int32; fn.argtypes = args
@@ -454,6 +456,20 @@ class PathTracer:
         for k in range(16): d.camera_view[k] = float(sc["camera_view"][k])
         d.camera_aspect = float(sc["aspect"])
         self._ck(self.L.b200pt_set_scene_arrays(self.h, C.byref(d)))
+
+    # ---- TLAS::Update: instance transforms (column-major 4x4, b200pt_instance.Transform) without reloading the scene
+    def instance_count(self):
+        n = C.c_uint32(); self._ck(self.L.b200pt_instance_count(self.h, C.byref(n))); return n.value
+
+    def get_instance_transforms(self):
+        """(n, 16) float32, column-major like the scene dict's instance transforms"""
+        out = np.zeros((self.instance_count(), 16), np.float32)
+        self._ck(self.L.b200pt_get_instance_transforms(self.h, _p(out), len(out))); return out
+
+    def update_instance_transforms(self, xf, rebuild=False):
+        """xf: (n, 16) column-major transforms, one per instance.  rebuild=False refits the tree in place; True builds it anew."""
+        xf = np.ascontiguousarray(xf, np.float32).reshape(-1, 16)
+        self._ck(self.L.b200pt_update_instance_transforms(self.h, _p(xf), len(xf), 1 if rebuild else 0))
 
     def set_env_map(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32)

@@ -108,6 +108,23 @@ int32_t b200pt_get_material_name(b200pt_handle h, uint32_t i, char *buf, uint32_
     return guard(h, [&](Engine &e) { if (i >= e.scene().material_names.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "material index out of range" };
         strncpy(buf, e.scene().material_names[i].c_str(), n - 1); buf[n - 1] = 0; });
 }
+int32_t b200pt_instance_count(b200pt_handle h, uint32_t *out) {
+    if (!out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { if (!e.has_scene()) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" }; *out = (uint32_t)e.scene().instances.size(); });
+}
+int32_t b200pt_get_instance_transforms(b200pt_handle h, float *xf, uint32_t count) {
+    if (!xf) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) {
+        if (!e.has_scene()) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+        const auto &in = e.scene().instances;
+        if (count != in.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform count differs from the instance count" };
+        for (size_t i = 0; i < in.size(); i++) memcpy(xf + i * 16, in[i].Transform, sizeof in[i].Transform);
+    });
+}
+int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *xf, uint32_t count, int32_t rebuild) {
+    if (!xf) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.update_instance_transforms(xf, count, rebuild != 0); });
+}
 int32_t b200pt_set_camera(b200pt_handle h, const float vi[16], const float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_camera(vi, pi); }); }
 int32_t b200pt_get_camera(b200pt_handle h, float vi[16], float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.get_camera(vi, pi); }); }
 int32_t b200pt_camera_from_view(const float view[16], float aspect, float vi[16], float pi[16]) {

@@ -79,7 +79,7 @@ void Engine::free_scene() {
     dfree(d_verts_); dfree(d_indices_); dfree(d_meshes_); dfree(d_instances_); dfree(d_materials_); dfree(d_textures_); dfree(d_emissive_); dfree(d_em_tris_); dfree(d_em_tri_base_); dfree(d_tri_class_);
     for (auto &p : d_texdata_) if (p) cudaFree(p);
     d_texdata_.clear();
-    lbvh_free(&bvh_);
+    lbvh_free(&bvh_); lbvh_refit_free(&refit_);
     has_scene_ = false;
 }
 
@@ -115,17 +115,7 @@ void Engine::upload_scene() {
     CK(cudaMalloc(&d_verts_, nv * sizeof(b200pt_vertex))); CK(cudaMemcpy(d_verts_, verts.data(), nv * sizeof(b200pt_vertex), cudaMemcpyHostToDevice));
     CK(cudaMalloc(&d_indices_, ni * 4)); CK(cudaMemcpy(d_indices_, idx.data(), ni * 4, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&d_meshes_, h_meshes_.size() * sizeof(DevMesh))); CK(cudaMemcpy(d_meshes_, h_meshes_.data(), h_meshes_.size() * sizeof(DevMesh), cudaMemcpyHostToDevice));
-    // instances: one per MeshInstance in loader order == InstanceIndex (TLASImpl.cpp:29-35)
-    h_instances_.assign(scene_.instances.size(), DevInstance{});
-    uint32_t tri_base = 0;
-    for (size_t i = 0; i < scene_.instances.size(); i++) {
-        const b200pt_instance &in = scene_.instances[i]; DevInstance &d = h_instances_[i];
-        for (int r = 0; r < 3; r++) for (int c = 0; c < 4; c++) d.o2w[r * 4 + c] = in.Transform[c * 4 + r];
-        mat3_inverse_from_o2w(d.o2w, d.w2o);
-        d.mesh = in.MeshIndex; d.material = in.MaterialIndex; d.tri_base = tri_base;
-        tri_base += h_meshes_[in.MeshIndex].tri_count;
-    }
-    n_tris_ = tri_base;
+    fill_instances();
     CK(cudaMalloc(&d_instances_, h_instances_.size() * sizeof(DevInstance)));
     {
         std::vector<DevMaterial> dm; dm.reserve(scene_.materials.size());
@@ -147,39 +137,99 @@ void Engine::upload_scene() {
         dt[i] = { d_texdata_[i], t.width, t.height, t.channels, 0 };
     }
     CK(cudaMalloc(&d_textures_, dt.size() * sizeof(DevTexture))); CK(cudaMemcpy(d_textures_, dt.data(), dt.size() * sizeof(DevTexture), cudaMemcpyHostToDevice));
+    ds_.verts = d_verts_; ds_.indices = d_indices_; ds_.meshes = d_meshes_; ds_.instances = d_instances_; ds_.materials = d_materials_;
+    CK(cudaMalloc(&d_tri_class_, std::max<size_t>(1, n_tris_)));
+    rebuild_tri_class();
+    ds_.textures = d_textures_; ds_.emissive = d_emissive_;
+    build_bvh(&bvh_, &ds_, &lc_);
+}
+
+// DevInstance of every instance from scene_.instances (o2w = rows 0-2 of the column-major Transform, w2o its inverse); emissive_tri_count is
+// rebuild_emissive's.  set_scene and update_instance_transforms both use it.
+void Engine::fill_instances() {
+    // instances: one per MeshInstance in loader order == InstanceIndex (TLASImpl.cpp:29-35)
+    h_instances_.assign(scene_.instances.size(), DevInstance{});
+    uint32_t tri_base = 0;
+    for (size_t i = 0; i < scene_.instances.size(); i++) {
+        const b200pt_instance &in = scene_.instances[i]; DevInstance &d = h_instances_[i];
+        for (int r = 0; r < 3; r++) for (int c = 0; c < 4; c++) d.o2w[r * 4 + c] = in.Transform[c * 4 + r];
+        mat3_inverse_from_o2w(d.o2w, d.w2o);
+        d.mesh = in.MeshIndex; d.material = in.MaterialIndex; d.tri_base = tri_base;
+        tri_base += h_meshes_[in.MeshIndex].tri_count;
+    }
+    n_tris_ = tri_base;
+}
+
+// The acceleration structure of the instances in d_instances_, built into *out (which the caller owns, also on failure): the BVH fields of *ds
+// and the launch configuration *lc are set from it.  set_scene and update_instance_transforms(rebuild) both use it.
+void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc) {
     // acceleration structure: GPU LBVH over the flattened instances
     // tree-quality pass over the GPU LBVH: same hits, fewer node visits / triangle tests.  Level 3 (full binned-SAH build + insertion-based
     // refinement) is the default;
     // B200PT_BVH_SAH=0..5 overrides (0 = plain LBVH).
     int sah_mode = 3;
     if (const char *e = getenv("B200PT_BVH_SAH")) sah_mode = (e[0] >= '0' && e[0] <= '5' && e[1] == 0) ? e[0] - '0' : 3;
-    int r = lbvh_build(d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, &bvh_, stream_, sah_mode == 2 || sah_mode == 3);
+    int r = lbvh_build(d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_, sah_mode == 2 || sah_mode == 3);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build failed: ") + cudaGetErrorString((cudaError_t)r) };
     if (sah_mode) {
         double sah[2];
-        r = lbvh_refine_sah(&bvh_, stream_, sah, sah_mode);
+        r = lbvh_refine_sah(out, stream_, sah, sah_mode);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refine_sah failed: ") + cudaGetErrorString((cudaError_t)r) };
-        if (getenv("B200PT_DEBUG")) fprintf(stderr, "[b200pt] SAH pass (mode %d): cost %.3f -> %.3f, depth %d\n", sah_mode, sah[0], sah[1], bvh_.max_depth);
+        if (getenv("B200PT_DEBUG")) fprintf(stderr, "[b200pt] SAH pass (mode %d): cost %.3f -> %.3f, depth %d\n", sah_mode, sah[0], sah[1], out->max_depth);
     }
-    ds_.verts = d_verts_; ds_.indices = d_indices_; ds_.meshes = d_meshes_; ds_.instances = d_instances_; ds_.materials = d_materials_;
-    CK(cudaMalloc(&d_tri_class_, std::max<size_t>(1, n_tris_)));
-    rebuild_tri_class();
-    ds_.textures = d_textures_; ds_.emissive = d_emissive_; ds_.nodes = bvh_.nodes; ds_.tris = bvh_.tris; ds_.shade_tris = bvh_.shade; ds_.tri_slot = bvh_.tri_slot;
-    ds_.n_tris = bvh_.n_tris; ds_.n_nodes = bvh_.n_nodes; ds_.root = bvh_.root; ds_.bvh_bytes = bvh_.bytes <= 0xFFFFFFFFull ? (uint32_t)bvh_.bytes : 0;
-    ds_.nodes4 = nullptr; ds_.n_nodes4 = 0;
-    if (bvh_.bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
-        r = lbvh_build_wide(&bvh_, stream_);
+    ds->nodes = out->nodes; ds->tris = out->tris; ds->shade_tris = out->shade; ds->tri_slot = out->tri_slot;
+    ds->n_tris = out->n_tris; ds->n_nodes = out->n_nodes; ds->root = out->root; ds->bvh_bytes = out->bytes <= 0xFFFFFFFFull ? (uint32_t)out->bytes : 0;
+    ds->nodes4 = nullptr; ds->n_nodes4 = 0;
+    if (out->bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
+        r = lbvh_build_wide(out, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build_wide failed: ") + cudaGetErrorString((cudaError_t)r) };
-        ds_.nodes4 = bvh_.nodes4; ds_.n_nodes4 = bvh_.n_nodes4;
+        ds->nodes4 = out->nodes4; ds->n_nodes4 = out->n_nodes4;
     }
     // A handful of triangle slots (the 12-triangle Cornell box): shared-memory traversals test them in order, no hierarchy (bvh_traverse.cuh).
     {
         uint32_t flat_max = 16;
         if (const char *e = getenv("B200PT_FLAT_MAX")) { const int v = atoi(e); if (v >= 0 && v <= 64) flat_max = (uint32_t)v; }
-        ds_.n_flat = (bvh_.n_tris <= flat_max) ? bvh_.n_tris : 0u;
+        ds->n_flat = (out->n_tris <= flat_max) ? out->n_tris : 0u;
     }
-    int q = query_launch_cfg(ds_, bvh_.max_depth, bvh_.depth4, &lc_);
+    int q = query_launch_cfg(*ds, out->max_depth, out->depth4, lc);
     if (q != 0) throw CudaError{ B200PT_ERR_CUDA, "query_launch_cfg failed" };
+}
+
+// TLAS::Update (VulkanHelper/Source/Vulkan/TLASImpl.cpp:192-293): every instance transform replaced, the tree refit in place (rebuild == false)
+// or built anew as set_scene would build it; then ResetPathTracing.  Camera, config, image size, partition, materials, volumes and the
+// environment stay.  Every argument is checked before anything changes.  A failed update restores the previous transforms: a failed rebuild keeps
+// the previous tree, a failed refit refits the tree back to them (and if that fails too, the handle has no scene until the next set_scene).
+void Engine::update_instance_transforms(const float *xf, uint32_t count, bool rebuild) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!xf || count != scene_.instances.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform count differs from the instance count" };
+    for (size_t i = 0; i < (size_t)count * 16; i++) if (!std::isfinite(xf[i])) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform entry is not finite" };
+    sync_all();                                                 // the waves in flight neither read a half-updated tree nor resolve into the new accumulation
+    std::vector<b200pt_instance> old = scene_.instances;
+    auto apply = [&](const std::vector<b200pt_instance> &inst) {
+        scene_.instances = inst;
+        fill_instances();
+        rebuild_emissive();                                     // DevEmissive::xf, the world-space EmTri, and d_instances_ (o2w / w2o)
+    };
+    std::vector<b200pt_instance> moved = old;
+    for (uint32_t i = 0; i < count; i++) memcpy(moved[i].Transform, xf + (size_t)i * 16, sizeof moved[i].Transform);
+    apply(moved);
+    if (!rebuild) {
+        auto refit = [&]() { return lbvh_refit(&bvh_, &refit_, d_verts_, d_indices_, d_meshes_, d_instances_, (uint32_t)h_instances_.size(), stream_); };
+        const int r = refit();
+        if (r != 0) {                                           // back to the previous transforms, and the tree refit to them
+            apply(old);
+            if (refit() != 0) has_scene_ = false;               // the tree matches neither: no render until set_scene
+            throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refit failed: ") + cudaGetErrorString((cudaError_t)r) };
+        }
+    } else {
+        LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
+        try { build_bvh(&fresh, &ds, &lc); }
+        catch (...) { lbvh_free(&fresh); apply(old); throw; }
+        lbvh_free(&bvh_); lbvh_refit_free(&refit_);
+        bvh_ = fresh; ds_ = ds; lc_ = lc;
+    }
+    reset();
 }
 
 // 1x1 textures (the defaults of PathTracer.cpp:1557-1621, or any constant texture) are resolved to their texel value here

@@ -20,6 +20,8 @@ public:
     void set_config(const b200pt_config &c);
     const b200pt_config &config() const { return cfg_; }
     void set_material(uint32_t idx, const b200pt_material &m);
+    // TLAS::Update: count x 16 floats (b200pt_instance::Transform), refit in place or (rebuild) the tree set_scene would build
+    void update_instance_transforms(const float *transforms, uint32_t count, bool rebuild);
     // PathTracer::AddVolume / SetVolume / RemoveVolume / SetPhaseFunction / AddDensityDataToVolume / RemoveDensityDataFromVolume (volumes.cuh)
     uint32_t add_volume(const b200pt_volume &v);
     void set_volume(uint32_t idx, const b200pt_volume &v);
@@ -102,6 +104,8 @@ public:
 private:
     void free_scene();
     void upload_scene();
+    void fill_instances();                          // h_instances_ and n_tris_ from scene_.instances
+    void build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc);   // the BVH half of upload_scene
     void rebuild_emissive();
     void rebuild_tri_class();                       // per-triangle shading class (MaterialClass) + the set of classes present in the scene
     void upload_volumes();
@@ -141,6 +145,7 @@ private:
     DevGrid *d_grids_ = nullptr; int density_data_counter_ = 0;   // PathTracer.cpp:1508-1513: slots are handed out round-robin
     b200pt_atmosphere atmosphere_{};
     LbvhResult bvh_{};
+    LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
     LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
     uint8_t *d_tri_class_ = nullptr; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c

@@ -2,6 +2,7 @@
 #pragma once
 #include "device_types.h"
 #include <cuda_runtime.h>
+#include <vector>
 
 namespace b200pt {
 
@@ -151,6 +152,15 @@ constexpr int BVH_STACK_MAX = 64;
 int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode = 1);
 // Downloads r->nodes, collapses, uploads r->nodes4 (own allocation).  Returns cudaError_t as int; leaves nodes4 = nullptr if the root is a leaf.
 int lbvh_build_wide(LbvhResult *r, cudaStream_t st);
+// Refit in place after the instance transforms changed (d_instances holds the new o2w): the topology, slot order and tri_slot of r stay,
+// every slot record and box, every reachable BVH2 child box (padded from the new scene bounds) and every BVH4 child box are recomputed.
+// The state (per-slot slab assignment, BVH2 levels, BVH4 source map) is derived at the first call and kept in s; it belongs to r's tree
+// and is freed (lbvh_refit_free) whenever that tree is replaced.  Returns cudaError_t as int.
+struct LbvhRefit { uint32_t *slot_jk = nullptr; float *slot_box = nullptr, *node_box = nullptr, *bounds = nullptr; int32_t *order = nullptr, *src4 = nullptr;
+                   std::vector<uint32_t> level_off; uint32_t n4 = 0; bool ready = false; };
+int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+               uint32_t n_instances, cudaStream_t st);
+void lbvh_refit_free(LbvhRefit *s);
 
 // ---- post chain (post_kernels.cu) ----
 struct PostParams { float Exposure, Gamma, BloomThreshold, BloomStrength, FalloffRange; };

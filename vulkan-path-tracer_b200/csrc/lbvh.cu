@@ -52,27 +52,47 @@ __device__ __forceinline__ void atomic_max_f(float *addr, float v) {
 }
 
 // ---- 1. world triangles + scene bounds -------------------------------------------------------
+__device__ __forceinline__ uint32_t instance_of(const DevInstance *__restrict__ inst, uint32_t n_inst, uint32_t gid) {
+    uint32_t a = 0, b = n_inst - 1;                                      // last instance with tri_base <= gid
+    while (a < b) { uint32_t mid = (a + b + 1) >> 1; if (inst[mid].tri_base <= gid) a = mid; else b = mid - 1; }
+    return a;
+}
+// The 48-B record of global triangle gid (primitive prim of instance a) and its world box bb (lo xyz, hi xyz).  k_world_tris and the refit
+// (k_refit_slots) both call this, so a refit slot holds exactly the record a fresh build of the moved scene would hold.
+__device__ __forceinline__ BvhTri world_tri(const DevInstance &in, uint32_t a, uint32_t gid, uint32_t prim, const b200pt_vertex &A, const b200pt_vertex &B,
+                                            const b200pt_vertex &C, float bb[6]) {
+    const float3 v0 = xf_point_rn(in.o2w, A.Position[0], A.Position[1], A.Position[2]);
+    const float3 v1 = xf_point_rn(in.o2w, B.Position[0], B.Position[1], B.Position[2]);
+    const float3 v2 = xf_point_rn(in.o2w, C.Position[0], C.Position[1], C.Position[2]);
+    BvhTri t;
+    t.a = make_float4(v0.x, v0.y, v0.z, __uint_as_float(gid));
+    t.b = make_float4(__fsub_rn(v1.x, v0.x), __fsub_rn(v1.y, v0.y), __fsub_rn(v1.z, v0.z), __uint_as_float(a));
+    t.c = make_float4(__fsub_rn(v2.x, v0.x), __fsub_rn(v2.y, v0.y), __fsub_rn(v2.z, v0.z), __uint_as_float(prim));
+    bb[0] = fminf(v0.x, fminf(v1.x, v2.x)); bb[3] = fmaxf(v0.x, fmaxf(v1.x, v2.x));
+    bb[1] = fminf(v0.y, fminf(v1.y, v2.y)); bb[4] = fmaxf(v0.y, fmaxf(v1.y, v2.y));
+    bb[2] = fminf(v0.z, fminf(v1.z, v2.z)); bb[5] = fmaxf(v0.z, fmaxf(v1.z, v2.z));
+    return t;
+}
+__device__ __forceinline__ void reduce_bounds(float lo[3], float hi[3], float *bounds) {   // warp-reduce, then one atomic per warp (whole warps call it)
+    for (int k = 0; k < 3; k++) {
+        for (int o = 16; o > 0; o >>= 1) { lo[k] = fminf(lo[k], __shfl_down_sync(0xFFFFFFFFu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_down_sync(0xFFFFFFFFu, hi[k], o)); }
+        if ((threadIdx.x & 31) == 0) { atomic_min_f(&bounds[k], lo[k]); atomic_max_f(&bounds[3 + k], hi[k]); }
+    }
+}
 __global__ void k_world_tris(const b200pt_vertex *__restrict__ verts, const uint32_t *__restrict__ indices, const DevMesh *__restrict__ meshes,
                              const DevInstance *__restrict__ inst, uint32_t n_inst, uint32_t n_tris,
                              BvhTri *__restrict__ tmp, ShadeTri *__restrict__ shade, float *__restrict__ cent, float *__restrict__ bounds /*6*/) {
     const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
     float lo[3] = { 3.0e38f, 3.0e38f, 3.0e38f }, hi[3] = { -3.0e38f, -3.0e38f, -3.0e38f };
     if (gid < n_tris) {
-        uint32_t a = 0, b = n_inst - 1;                                  // last instance with tri_base <= gid
-        while (a < b) { uint32_t mid = (a + b + 1) >> 1; if (inst[mid].tri_base <= gid) a = mid; else b = mid - 1; }
+        const uint32_t a = instance_of(inst, n_inst, gid);
         const DevInstance &in = inst[a];
         const uint32_t prim = gid - in.tri_base;
         const DevMesh m = meshes[in.mesh];
         const uint32_t *ix = indices + m.ibase + (size_t)prim * 3;
         const b200pt_vertex &A = verts[m.vbase + ix[0]], &B = verts[m.vbase + ix[1]], &C = verts[m.vbase + ix[2]];
-        const float3 v0 = xf_point_rn(in.o2w, A.Position[0], A.Position[1], A.Position[2]);
-        const float3 v1 = xf_point_rn(in.o2w, B.Position[0], B.Position[1], B.Position[2]);
-        const float3 v2 = xf_point_rn(in.o2w, C.Position[0], C.Position[1], C.Position[2]);
-        BvhTri t;
-        t.a = make_float4(v0.x, v0.y, v0.z, __uint_as_float(gid));
-        t.b = make_float4(__fsub_rn(v1.x, v0.x), __fsub_rn(v1.y, v0.y), __fsub_rn(v1.z, v0.z), __uint_as_float(a));
-        t.c = make_float4(__fsub_rn(v2.x, v0.x), __fsub_rn(v2.y, v0.y), __fsub_rn(v2.z, v0.z), __uint_as_float(prim));
-        tmp[gid] = t;
+        float bb[6];
+        tmp[gid] = world_tri(in, a, gid, prim, A, B, C, bb);
         ShadeTri sh;
         sh.r[0] = make_float4(A.Position[0], A.Position[1], A.Position[2], __uint_as_float(a));
         sh.r[1] = make_float4(B.Position[0], B.Position[1], B.Position[2], __uint_as_float(prim));
@@ -82,16 +102,10 @@ __global__ void k_world_tris(const b200pt_vertex *__restrict__ verts, const uint
         sh.r[5] = make_float4(C.Normal[0], C.Normal[1], C.Normal[2], B.TexCoord[0]);
         sh.r[6] = make_float4(B.TexCoord[1], C.TexCoord[0], C.TexCoord[1], 0.0f);
         shade[gid] = sh;
-        lo[0] = fminf(v0.x, fminf(v1.x, v2.x)); hi[0] = fmaxf(v0.x, fmaxf(v1.x, v2.x));
-        lo[1] = fminf(v0.y, fminf(v1.y, v2.y)); hi[1] = fmaxf(v0.y, fmaxf(v1.y, v2.y));
-        lo[2] = fminf(v0.z, fminf(v1.z, v2.z)); hi[2] = fmaxf(v0.z, fmaxf(v1.z, v2.z));
-        float *bb = cent + (size_t)gid * 6;                              // per-triangle AABB (unsorted)
-        bb[0] = lo[0]; bb[1] = lo[1]; bb[2] = lo[2]; bb[3] = hi[0]; bb[4] = hi[1]; bb[5] = hi[2];
+        for (int k = 0; k < 3; k++) { lo[k] = bb[k]; hi[k] = bb[3 + k]; }
+        for (int k = 0; k < 6; k++) cent[(size_t)gid * 6 + k] = bb[k];  // per-triangle AABB (unsorted)
     }
-    for (int k = 0; k < 3; k++) {                                        // warp-reduce, then one atomic per warp
-        for (int o = 16; o > 0; o >>= 1) { lo[k] = fminf(lo[k], __shfl_down_sync(0xFFFFFFFFu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_down_sync(0xFFFFFFFFu, hi[k], o)); }
-        if ((threadIdx.x & 31) == 0) { atomic_min_f(&bounds[k], lo[k]); atomic_max_f(&bounds[3 + k], hi[k]); }
-    }
+    reduce_bounds(lo, hi, bounds);
 }
 
 // ---- 1b. early split clipping: fat boxes of thin diagonal triangles are cut into up to 8 references ------------------
@@ -126,6 +140,34 @@ __device__ __forceinline__ int clip_poly(const float3 *in, int n, int axis, floa
     }
     return m;
 }
+// Reference box of slab j of k (k >= 2) of triangle t with world box bb: slabs cut the longest axis of bb into k equal parts, so the k slabs
+// cover the triangle whatever order they are taken in.  k_make_refs and the refit (k_refit_slots) both call this.
+__device__ __forceinline__ void slab_ref_box(const BvhTri &t, const float *bb, uint32_t j, uint32_t k, float *o) {
+    const float ex = bb[3] - bb[0], ey = bb[4] - bb[1], ez = bb[5] - bb[2];
+    const int axis = (ex >= ey && ex >= ez) ? 0 : (ey >= ez ? 1 : 2);
+    const float lo = bb[axis], w = (bb[3 + axis] - bb[axis]) / (float)k;
+    const float3 v0 = make_float3(t.a.x, t.a.y, t.a.z), v1 = make_float3(t.a.x + t.b.x, t.a.y + t.b.y, t.a.z + t.b.z), v2 = make_float3(t.a.x + t.c.x, t.a.y + t.c.y, t.a.z + t.c.z);
+    const float s0 = lo + w * (float)j, s1 = (j + 1 == k) ? bb[3 + axis] : lo + w * (float)(j + 1);
+    float3 p0[8], p1[8];                                                 // a triangle clipped by two planes has <= 5 vertices
+    p0[0] = v0; p0[1] = v1; p0[2] = v2;
+    int m = clip_poly(p0, 3, axis, s0, true, p1);
+    m = clip_poly(p1, m, axis, s1, false, p0);
+    float blo[3] = { 3.0e38f, 3.0e38f, 3.0e38f }, bhi[3] = { -3.0e38f, -3.0e38f, -3.0e38f };
+    for (int a = 0; a < m; a++) {
+        blo[0] = fminf(blo[0], p0[a].x); blo[1] = fminf(blo[1], p0[a].y); blo[2] = fminf(blo[2], p0[a].z);
+        bhi[0] = fmaxf(bhi[0], p0[a].x); bhi[1] = fmaxf(bhi[1], p0[a].y); bhi[2] = fmaxf(bhi[2], p0[a].z);
+    }
+    for (int q = 0; q < 3; q++) {
+        float l = bb[q], h = bb[3 + q];
+        if (q == axis) { l = s0; h = s1; }
+        if (m >= 1) {                                                    // clipped polygon bounds, padded, never beyond the triangle's own box
+            const float pad = 1e-5f * fmaxf(fabsf(blo[q]), fabsf(bhi[q])) + 1e-6f * (bb[3 + q] - bb[q]) + 1e-30f;
+            l = fmaxf(l, blo[q] - pad); h = fminf(h, bhi[q] + pad);
+            if (l > h) { l = bb[q]; h = bb[3 + q]; if (q == axis) { l = s0; h = s1; } }
+        }
+        o[q] = l; o[3 + q] = h;
+    }
+}
 __global__ void k_make_refs(const BvhTri *__restrict__ tmp, const float *__restrict__ aabb, const uint32_t *__restrict__ ksplit, const uint32_t *__restrict__ ref_off,
                             uint32_t n, float *__restrict__ ref_box, uint32_t *__restrict__ ref_tri) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -133,33 +175,9 @@ __global__ void k_make_refs(const BvhTri *__restrict__ tmp, const float *__restr
     const float *bb = aabb + (size_t)i * 6;
     const uint32_t k = ksplit[i], r0 = ref_off[i];
     if (k == 1) { for (int q = 0; q < 6; q++) ref_box[(size_t)r0 * 6 + q] = bb[q]; ref_tri[r0] = i; return; }
-    const float ex = bb[3] - bb[0], ey = bb[4] - bb[1], ez = bb[5] - bb[2];
-    const int axis = (ex >= ey && ex >= ez) ? 0 : (ey >= ez ? 1 : 2);
-    const float lo = bb[axis], w = (bb[3 + axis] - bb[axis]) / (float)k;
     const BvhTri t = tmp[i];
-    const float3 v0 = make_float3(t.a.x, t.a.y, t.a.z), v1 = make_float3(t.a.x + t.b.x, t.a.y + t.b.y, t.a.z + t.b.z), v2 = make_float3(t.a.x + t.c.x, t.a.y + t.c.y, t.a.z + t.c.z);
     for (uint32_t j = 0; j < k; j++) {
-        const float s0 = lo + w * (float)j, s1 = (j + 1 == k) ? bb[3 + axis] : lo + w * (float)(j + 1);
-        float3 p0[8], p1[8];                                             // a triangle clipped by two planes has <= 5 vertices
-        p0[0] = v0; p0[1] = v1; p0[2] = v2;
-        int m = clip_poly(p0, 3, axis, s0, true, p1);
-        m = clip_poly(p1, m, axis, s1, false, p0);
-        float blo[3] = { 3.0e38f, 3.0e38f, 3.0e38f }, bhi[3] = { -3.0e38f, -3.0e38f, -3.0e38f };
-        for (int a = 0; a < m; a++) {
-            blo[0] = fminf(blo[0], p0[a].x); blo[1] = fminf(blo[1], p0[a].y); blo[2] = fminf(blo[2], p0[a].z);
-            bhi[0] = fmaxf(bhi[0], p0[a].x); bhi[1] = fmaxf(bhi[1], p0[a].y); bhi[2] = fmaxf(bhi[2], p0[a].z);
-        }
-        float *o = ref_box + (size_t)(r0 + j) * 6;
-        for (int q = 0; q < 3; q++) {
-            float l = bb[q], h = bb[3 + q];
-            if (q == axis) { l = s0; h = s1; }
-            if (m >= 1) {                                                // clipped polygon bounds, padded, never beyond the triangle's own box
-                const float pad = 1e-5f * fmaxf(fabsf(blo[q]), fabsf(bhi[q])) + 1e-6f * (bb[3 + q] - bb[q]) + 1e-30f;
-                l = fmaxf(l, blo[q] - pad); h = fminf(h, bhi[q] + pad);
-                if (l > h) { l = bb[q]; h = bb[3 + q]; if (q == axis) { l = s0; h = s1; } }
-            }
-            o[q] = l; o[3 + q] = h;
-        }
+        slab_ref_box(t, bb, j, k, ref_box + (size_t)(r0 + j) * 6);
         ref_tri[r0 + j] = i;
     }
 }
@@ -327,27 +345,96 @@ __device__ __forceinline__ int lbvh_child_ref(int c, const int2 *range) {
     if (r.y - r.x + 1 <= LBVH_LEAF_MAX) return ~((r.x << 2) | (r.y - r.x));
     return c;
 }
+// absolute pad: the FMA slab test of bvh_trace perturbs a plane by <= 6e-8*|ray origin|; 2e-6 * (largest |coordinate| of the scene)
+// keeps it conservative for origins within ~16 scene extents (every secondary ray), and also covers the rounding of the
+// subtract-multiply form, so the traversal needs no slack factor on its interval comparison
+__device__ __forceinline__ float scene_pad(const float *bounds) {
+    float ext = 0.0f;
+    for (int k = 0; k < 6; k++) ext = fmaxf(ext, fabsf(bounds[k]));
+    return 2e-6f * ext + 1e-30f;
+}
+__device__ __forceinline__ void pad_child(const float *box, float pabs, float *lo, float *hi) {   // box: lo xyz, hi xyz (unpadded)
+    for (int k = 0; k < 3; k++) { const float p = 4e-7f * fmaxf(fabsf(box[k]), fabsf(box[3 + k])) + pabs; lo[k] = box[k] - p; hi[k] = box[3 + k] + p; }
+}
 __global__ void k_emit(int n_int, const int *__restrict__ left, const int *__restrict__ right, const int2 *__restrict__ range, const float *__restrict__ leaf_box,
                        const float *__restrict__ node_box, const float *__restrict__ bounds, BvhNode *__restrict__ nodes) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_int) return;
-    // absolute pad: the FMA slab test of bvh_trace perturbs a plane by <= 6e-8*|ray origin|; 2e-6 * (largest |coordinate| of the scene)
-    // keeps it conservative for origins within ~16 scene extents (every secondary ray), and also covers the rounding of the
-    // subtract-multiply form, so the traversal needs no slack factor on its interval comparison
-    float ext = 0.0f;
-    for (int k = 0; k < 6; k++) ext = fmaxf(ext, fabsf(bounds[k]));
-    const float pabs = 2e-6f * ext + 1e-30f;
+    const float pabs = scene_pad(bounds);
     const int l = left[i], r = right[i];
     const float *a = l < 0 ? leaf_box + (size_t)(~l) * 6 : node_box + (size_t)l * 6;
     const float *b = r < 0 ? leaf_box + (size_t)(~r) * 6 : node_box + (size_t)r * 6;
     BvhNode nd;
-    for (int k = 0; k < 3; k++) {
-        const float pa = 4e-7f * fmaxf(fabsf(a[k]), fabsf(a[3 + k])) + pabs, pb = 4e-7f * fmaxf(fabsf(b[k]), fabsf(b[3 + k])) + pabs;
-        nd.lo0[k] = a[k] - pa; nd.hi0[k] = a[3 + k] + pa;
-        nd.lo1[k] = b[k] - pb; nd.hi1[k] = b[3 + k] + pb;
-    }
+    pad_child(a, pabs, nd.lo0, nd.hi0); pad_child(b, pabs, nd.lo1, nd.hi1);
     nd.c0 = lbvh_child_ref(l, range); nd.c1 = lbvh_child_ref(r, range); nd._pad[0] = nd._pad[1] = 0;
     nodes[i] = nd;
+}
+
+// ---- 8. refit after the instance transforms changed (Engine::update_instance_transforms without rebuild) --------------------------------
+// Topology, slot order, tri_slot and the shading records stay; every slot's 48-B record, its reference box, every reachable BVH2 child box
+// (re-padded from the NEW scene bounds) and the BVH4 child boxes are recomputed.  Deterministic: min / max unions and one fixed arithmetic.
+// slot_jk[i] = (j << 16) | k: slot i is slab j of the k slots holding its triangle (k == 1: the whole triangle box).
+__global__ void k_refit_slots(const b200pt_vertex *__restrict__ verts, const uint32_t *__restrict__ indices, const DevMesh *__restrict__ meshes,
+                              const DevInstance *__restrict__ inst, uint32_t n_inst, const uint32_t *__restrict__ slot_jk, uint32_t n,
+                              BvhTri *__restrict__ tris, float *__restrict__ slot_box, float *__restrict__ bounds) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    float lo[3] = { 3.0e38f, 3.0e38f, 3.0e38f }, hi[3] = { -3.0e38f, -3.0e38f, -3.0e38f };
+    if (i < n) {
+        const uint32_t gid = __float_as_uint(tris[i].a.w);
+        const uint32_t a = instance_of(inst, n_inst, gid);
+        const DevInstance &in = inst[a];
+        const uint32_t prim = gid - in.tri_base;
+        const DevMesh m = meshes[in.mesh];
+        const uint32_t *ix = indices + m.ibase + (size_t)prim * 3;
+        float bb[6];
+        const BvhTri t = world_tri(in, a, gid, prim, verts[m.vbase + ix[0]], verts[m.vbase + ix[1]], verts[m.vbase + ix[2]], bb);
+        tris[i] = t;
+        const uint32_t jk = slot_jk[i], k = jk & 0xFFFFu;
+        float *o = slot_box + (size_t)i * 6;
+        if (k <= 1) { for (int q = 0; q < 6; q++) o[q] = bb[q]; }
+        else slab_ref_box(t, bb, jk >> 16, k, o);
+        for (int q = 0; q < 3; q++) { lo[q] = bb[q]; hi[q] = bb[3 + q]; }
+    }
+    reduce_bounds(lo, hi, bounds);
+}
+// One level of the BVH2 (nodes order[first, first + count), all at the same depth), deepest level first: child boxes from the slot boxes of
+// a leaf reference or from node_box of an inner child (written by the level below), padded as k_emit pads them; node_box[node] = the union.
+__global__ void k_refit_level(const int32_t *__restrict__ order, uint32_t first, uint32_t count, const float *__restrict__ slot_box,
+                              const float *__restrict__ bounds, BvhNode *__restrict__ nodes, float *__restrict__ node_box) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const int32_t n = order[first + i];
+    BvhNode nd = nodes[n];
+    const float pabs = scene_pad(bounds);
+    float u[6] = { 3.0e38f, 3.0e38f, 3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f };
+#pragma unroll
+    for (int s = 0; s < 2; s++) {
+        const int32_t c = s ? nd.c1 : nd.c0;
+        float box[6] = { 3.0e38f, 3.0e38f, 3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f };
+        if (c < 0) {                                                      // leaf: slots [first, first + count)
+            const uint32_t r = (uint32_t)(~c), f = r >> 2, cnt = (r & 3u) + 1u;
+            for (uint32_t q = f; q < f + cnt; q++)
+                for (int k = 0; k < 3; k++) { box[k] = fminf(box[k], slot_box[(size_t)q * 6 + k]); box[3 + k] = fmaxf(box[3 + k], slot_box[(size_t)q * 6 + 3 + k]); }
+        } else {
+            for (int k = 0; k < 6; k++) box[k] = __ldcg(node_box + (size_t)c * 6 + k);
+        }
+        pad_child(box, pabs, s ? nd.lo1 : nd.lo0, s ? nd.hi1 : nd.hi0);
+        for (int k = 0; k < 3; k++) { u[k] = fminf(u[k], box[k]); u[3 + k] = fmaxf(u[3 + k], box[3 + k]); }
+    }
+    nodes[n] = nd;
+    for (int k = 0; k < 6; k++) __stcg(node_box + (size_t)n * 6 + k, u[k]);
+}
+// BVH4 child boxes: bvh4_collapse_host copies every BVH4 child box verbatim from one BVH2 child box; src[4 * node4 + k] names it
+// ((BVH2 node << 1) | side, or -1 for an empty slot), so the refit BVH4 is exactly as conservative as the refit BVH2.
+__global__ void k_refit_wide(const int32_t *__restrict__ src, uint32_t n4, const BvhNode *__restrict__ nodes2, Bvh4Node *__restrict__ nodes4) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4 * 4u) return;
+    const int32_t s = src[i];
+    if (s < 0) return;
+    const BvhNode &N = nodes2[s >> 1];
+    const float *lo = (s & 1) ? N.lo1 : N.lo0, *hi = (s & 1) ? N.hi1 : N.hi0;
+    Bvh4Node &o = nodes4[i >> 2]; const uint32_t k = i & 3u;
+    o.lox[k] = lo[0]; o.loy[k] = lo[1]; o.loz[k] = lo[2]; o.hix[k] = hi[0]; o.hiy[k] = hi[1]; o.hiz[k] = hi[2];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -356,16 +443,17 @@ __global__ void k_emit(int n_int, const int *__restrict__ left, const int *__res
 // copied verbatim from the BVH2 nodes, so the BVH4 is exactly as conservative as the BVH2 (same padded boxes, same leaves): both
 // structures return identical hits.  Nodes are emitted in breadth-first order (the hot top levels are contiguous).
 // ------------------------------------------------------------------------------------------------
-uint32_t bvh4_collapse_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *out, int *depth4) {
+// src (optional, 4 entries per BVH4 node): the BVH2 child box each BVH4 child box was copied from, (BVH2 node << 1) | side, -1 when empty
+static uint32_t bvh4_collapse_src(const BvhNode *nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *out, int *depth4, int32_t *src) {
     if (depth4) *depth4 = 0;
     if (root2 < 0 || n_nodes2 == 0) return 0;
-    struct Slot { int32_t child; float lo[3], hi[3]; };
+    struct Slot { int32_t child, src; float lo[3], hi[3]; };
     auto area = [](const Slot &s) { const float dx = s.hi[0] - s.lo[0], dy = s.hi[1] - s.lo[1], dz = s.hi[2] - s.lo[2]; return dx * dy + dy * dz + dz * dx; };
     bool bad = false;                                                       // a child index outside the array or a cycle: not a tree
     auto slots_of = [&](int32_t n, Slot &a, Slot &b) {
         if ((uint32_t)n >= n_nodes2) { bad = true; n = 0; }
         const BvhNode &N = nodes2[n];
-        a.child = N.c0; b.child = N.c1;
+        a.child = N.c0; b.child = N.c1; a.src = n * 2; b.src = n * 2 + 1;
         for (int k = 0; k < 3; k++) { a.lo[k] = N.lo0[k]; a.hi[k] = N.hi0[k]; b.lo[k] = N.lo1[k]; b.hi[k] = N.hi1[k]; }
     };
     std::vector<std::pair<int32_t, int>> queue;                          // (BVH2 node, depth) of BVH4 node i, in emission order
@@ -397,11 +485,15 @@ uint32_t bvh4_collapse_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t ro
                 o.child[k] = BVH4_EMPTY;
             }
             o._pad[k] = 0;
+            if (src) src[i * 4 + k] = k < ns ? sl[k].src : -1;
         }
     }
     if (bad || queue.size() > (size_t)n_nodes2) { if (depth4) *depth4 = 0; return 0; }
     if (depth4) *depth4 = max_d;
     return (uint32_t)queue.size();
+}
+uint32_t bvh4_collapse_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *out, int *depth4) {
+    return bvh4_collapse_src(nodes2, n_nodes2, root2, out, depth4, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -828,6 +920,118 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
     LBVH_CHECK(cudaMemcpyAsync(r->nodes, out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     r->root = 0; r->max_depth = depth;
+    return 0;
+}
+
+void lbvh_refit_free(LbvhRefit *s) {
+    if (s->slot_jk) cudaFree(s->slot_jk);
+    if (s->slot_box) cudaFree(s->slot_box);
+    if (s->node_box) cudaFree(s->node_box);
+    if (s->bounds) cudaFree(s->bounds);
+    if (s->order) cudaFree(s->order);
+    if (s->src4) cudaFree(s->src4);
+    *s = LbvhRefit{};
+}
+
+// What the refit needs of the tree, derived once at the first update (set_scene pays nothing for it): the slots' (j, k), the reachable BVH2
+// nodes by depth, and the BVH4's source map.  k = slots holding the triangle; j, the slab a slot stands for, follows where the tree placed the
+// slot: the slots of one triangle are ranked by the centre of their leaf's box along the triangle's longest axis (ties: slot order).  Any
+// permutation of 0..k-1 covers the triangle; this one keeps the build's slab in every slot whose leaf holds no other slab of its triangle, so
+// a refit before anything moved gives back the build's boxes there.
+static int lbvh_refit_prepare(const LbvhResult *r, LbvhRefit *s, cudaStream_t st) {
+    const uint32_t n = r->n_tris, np = r->n_prims;
+    std::vector<BvhTri> ht(n);
+    LBVH_CHECK(cudaMemcpyAsync(ht.data(), r->tris, (size_t)n * sizeof(BvhTri), cudaMemcpyDeviceToHost, st));
+    std::vector<BvhNode> h2(r->root >= 0 ? r->n_nodes : 0);
+    if (!h2.empty()) LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes, (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
+    LBVH_CHECK(cudaStreamSynchronize(st));
+    std::vector<uint32_t> gid(n), jk(n);
+    for (uint32_t i = 0; i < n; i++) { memcpy(&gid[i], &ht[i].a.w, 4); if (gid[i] >= np) gid[i] = 0u; }
+    s->level_off.clear(); s->n4 = 0;
+    std::vector<float> cen((size_t)n * 3, 0.0f);                               // centre of the box of the leaf holding each slot
+    std::vector<int32_t> order;
+    if (!h2.empty()) {
+        order.push_back(r->root);                                              // breadth-first: each depth is one contiguous range
+        s->level_off.push_back(0);
+        for (size_t b = 0; b < order.size();) {
+            const size_t e = order.size();
+            for (size_t i = b; i < e; i++) {
+                const BvhNode &N = h2[order[i]];
+                for (int c = 0; c < 2; c++) {
+                    const int32_t ch = c ? N.c1 : N.c0;
+                    if (ch >= 0) { order.push_back(ch); continue; }
+                    const uint32_t rr = (uint32_t)(~ch), f = rr >> 2, m = (rr & 3u) + 1u;
+                    const float *lo = c ? N.lo1 : N.lo0, *hi = c ? N.hi1 : N.hi0;
+                    for (uint32_t q = f; q < f + m && q < n; q++) for (int k = 0; k < 3; k++) cen[(size_t)q * 3 + k] = 0.5f * (lo[k] + hi[k]);
+                }
+            }
+            if (order.size() > r->n_nodes) return (int)cudaErrorInvalidValue;   // not a tree
+            s->level_off.push_back((uint32_t)e); b = e;
+        }
+    }
+    {   // slots grouped by triangle (counting sort, slot order inside a group), then ranked along the triangle's longest axis
+        std::vector<uint32_t> off(np + 1, 0u), slots(n);
+        for (uint32_t i = 0; i < n; i++) off[gid[i] + 1]++;
+        for (uint32_t g = 0; g < np; g++) off[g + 1] += off[g];
+        std::vector<uint32_t> fill(off.begin(), off.end() - 1);
+        for (uint32_t i = 0; i < n; i++) slots[fill[gid[i]]++] = i;
+        for (uint32_t g = 0; g < np; g++) {
+            uint32_t *b = slots.data() + off[g], *e = slots.data() + off[g + 1];
+            const uint32_t k = (uint32_t)(e - b);
+            if (k == 0) continue;
+            if (k > 1) {
+                const BvhTri &t = ht[*b];
+                float lo[3], hi[3];
+                const float v[3][3] = { { t.a.x, t.a.y, t.a.z }, { t.a.x + t.b.x, t.a.y + t.b.y, t.a.z + t.b.z }, { t.a.x + t.c.x, t.a.y + t.c.y, t.a.z + t.c.z } };
+                for (int q = 0; q < 3; q++) { lo[q] = fminf(v[0][q], fminf(v[1][q], v[2][q])); hi[q] = fmaxf(v[0][q], fmaxf(v[1][q], v[2][q])); }
+                const float ex = hi[0] - lo[0], ey = hi[1] - lo[1], ez = hi[2] - lo[2];
+                const int axis = (ex >= ey && ex >= ez) ? 0 : (ey >= ez ? 1 : 2);
+                std::stable_sort(b, e, [&](uint32_t x, uint32_t y) { return cen[(size_t)x * 3 + axis] < cen[(size_t)y * 3 + axis]; });
+            }
+            for (uint32_t j = 0; j < k; j++) jk[b[j]] = (j << 16) | k;
+        }
+    }
+    LBVH_CHECK(cudaMalloc(&s->slot_jk, (size_t)n * 4));
+    LBVH_CHECK(cudaMalloc(&s->slot_box, (size_t)n * 6 * sizeof(float)));
+    LBVH_CHECK(cudaMalloc(&s->bounds, 6 * sizeof(float)));
+    LBVH_CHECK(cudaMemcpyAsync(s->slot_jk, jk.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    if (!h2.empty()) {
+        LBVH_CHECK(cudaMalloc(&s->order, order.size() * 4));
+        LBVH_CHECK(cudaMalloc(&s->node_box, (size_t)r->n_nodes * 6 * sizeof(float)));
+        LBVH_CHECK(cudaMemcpyAsync(s->order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
+        if (r->nodes4) {                                                     // the collapse is deterministic: re-run on the unchanged BVH2 it was built from
+            std::vector<Bvh4Node> h4(r->n_nodes); std::vector<int32_t> src((size_t)r->n_nodes * 4);
+            int d4 = 0;
+            const uint32_t n4 = bvh4_collapse_src(h2.data(), r->n_nodes, r->root, h4.data(), &d4, src.data());
+            if (n4 != r->n_nodes4) return (int)cudaErrorInvalidValue;
+            LBVH_CHECK(cudaMalloc(&s->src4, (size_t)n4 * 4 * 4));
+            LBVH_CHECK(cudaMemcpyAsync(s->src4, src.data(), (size_t)n4 * 4 * 4, cudaMemcpyHostToDevice, st));
+            s->n4 = n4;
+        }
+    }
+    LBVH_CHECK(cudaStreamSynchronize(st));
+    s->ready = true;
+    return 0;
+}
+
+int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+               uint32_t n_instances, cudaStream_t st) {
+    if (!r->tris || r->n_tris == 0 || n_instances == 0) return (int)cudaErrorInvalidValue;
+    if (!s->ready) {
+        const int e = lbvh_refit_prepare(r, s, st);
+        if (e != 0) { lbvh_refit_free(s); return e; }
+    }
+    const uint32_t n = r->n_tris;
+    const float binit[6] = { 3.0e38f, 3.0e38f, 3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f };
+    LBVH_CHECK(cudaMemcpyAsync(s->bounds, binit, sizeof(binit), cudaMemcpyHostToDevice, st));
+    k_refit_slots<<<(n + 255) / 256, 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, n_instances, s->slot_jk, n, r->tris, s->slot_box, s->bounds);
+    for (size_t l = s->level_off.size(); l-- > 1;) {                         // deepest level first
+        const uint32_t first = s->level_off[l - 1], count = s->level_off[l] - first;
+        k_refit_level<<<(count + 255) / 256, 256, 0, st>>>(s->order, first, count, s->slot_box, s->bounds, r->nodes, s->node_box);
+    }
+    if (s->n4) k_refit_wide<<<(s->n4 * 4 + 255) / 256, 256, 0, st>>>(s->src4, s->n4, r->nodes, r->nodes4);
+    LBVH_CHECK(cudaGetLastError());
+    LBVH_CHECK(cudaStreamSynchronize(st));
     return 0;
 }
 
