@@ -119,14 +119,17 @@ int32_t b200pt_get_material_name(b200pt_handle h, uint32_t index, char *buf, uin
 /* ---- instance transforms: TLAS::Update (VulkanHelper/Include/Vulkan/TLAS.h:78-85, Source/Vulkan/TLASImpl.cpp:192-293) ----
  * transforms: count x 16 floats, column-major, the layout of b200pt_instance.Transform, in InstanceIndex order; only rows 0-2 are used.
  * The update replaces every instance transform -> ResetPathTracing(); camera, config, image size, partition, materials, volumes and the
- * environment stay.  rebuild == 0 refits the tree in place (same topology, boxes recomputed on the GPU); rebuild != 0 builds the tree
- * b200pt_set_scene_arrays would build for these transforms (B200PT_BVH_SAH honoured, traversal shape and launch configuration re-chosen).
+ * environment stay.  rebuild == 0 refits the tree in place (same topology, boxes recomputed on the GPU); rebuild == B200PT_REBUILD_GPU builds
+ * a new tree on the GPU (PLOC clustering over the LBVH's references, milliseconds, close to the SAH tree's quality; B200PT_BVH_SAH not read);
+ * any other nonzero value builds the tree b200pt_set_scene_arrays would build for these transforms (B200PT_BVH_SAH honoured, host passes).
+ * Both rebuilds re-choose the traversal shape and launch configuration.
  * WRONG_ARGUMENTS: count != instance count, a null pointer or a non-finite entry; NO_SCENE without a scene.  A rejected call changes
  * nothing.  A failed update restores the previous transforms: a failed rebuild keeps the previous tree, a failed refit refits the tree back
  * to them (if that fails too, the handle reports NO_SCENE until the next set_scene).  The image equals that of a handle loaded with the
  * moved scene. */
 int32_t b200pt_instance_count(b200pt_handle h, uint32_t *out);
 int32_t b200pt_get_instance_transforms(b200pt_handle h, float *transforms, uint32_t count);
+#define B200PT_REBUILD_GPU 2
 int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *transforms, uint32_t count, int32_t rebuild);
 int32_t b200pt_set_camera(b200pt_handle h, const float view_inverse[16], const float projection_inverse[16]); /* SetCameraViewInverse/ProjectionInverse */
 int32_t b200pt_get_camera(b200pt_handle h, float view_inverse[16], float projection_inverse[16]);
@@ -447,6 +450,16 @@ int32_t b200pt_bvh2_sah_build(const float *ref_boxes, uint32_t n, float trav_cos
 /* Third opt-in level (B200PT_BVH_SAH=3 = level 2 followed by this): insertion-based refinement of a BVH2 -- the `fraction` largest nodes
  * are re-inserted where they add the least surface area, `passes` times.  Leaves are kept; output conventions as b200pt_bvh2_sah_rebuild. */
 int32_t b200pt_bvh2_reinsert(const void *nodes2, uint32_t n_nodes2, int32_t root2, void *nodes_out, int32_t passes, float fraction, uint32_t *n_out, int32_t *depth_out, double *sah_before_after);
+
+/* GPU tree builder (update_instance_transforms with B200PT_REBUILD_GPU): PLOC clustering over reference boxes in the given (Morton) order,
+ * leaves of <= 4 references by the SAH leaf rule, nodes depth-first with root 0, perm_out[new slot] = old slot.  Pure CPU restatement of the
+ * device builder, with the conventions of b200pt_bvh2_sah_build (trav_cost 1): *n_out = 0 when n <= 4 or a box is inverted / NaN. */
+int32_t b200pt_bvh2_ploc_build(const float *ref_boxes, uint32_t n, void *nodes_out, uint32_t *perm_out, uint32_t *n_out, int32_t *depth_out, double *sah_cost);
+/* Test hook: the device builder and the device BVH4 collapse the engine runs, on these boxes.  nodes_out: room for n - 1 BVH2 nodes,
+ * perm_out: n entries, nodes4_out: room for n - 1 BVH4 nodes (layouts as in b200pt_bvh4_collapse).  Equals b200pt_bvh2_ploc_build and
+ * b200pt_bvh4_collapse of its nodes bit for bit; rejects what b200pt_bvh2_ploc_build rejects (zero counts). */
+int32_t b200pt_bvh2_ploc_build_query(b200pt_handle h, const float *ref_boxes, uint32_t n, void *nodes_out, uint32_t *perm_out, uint32_t *n_out, int32_t *depth_out,
+                                     void *nodes4_out, uint32_t *n4_out, int32_t *depth4_out);
 
 /* ---- standalone codecs of the loader / image-output API (no GPU needed) ---- */
 /* stbi_load(.., STBI_rgb_alpha) / stbi_loadf semantics (AssetImporterImpl.cpp:494-545); free with b200pt_free */

@@ -74,7 +74,7 @@ def _update(name, inst, env=None):                                  # instance u
     T = util.product_tracer(name, 40, 30, MaxDepth=5)
     T.path_trace(1, util.BASE_SEED)
     xf = T.get_instance_transforms(); xf[inst, 12:15] += (0.3, -0.2, 0.1)
-    for rebuild in (False, True, False):
+    for rebuild in (False, True, "gpu", False):                         # refit, host rebuild, GPU rebuild (ploc.cu), refit of the GPU tree
         T.update_instance_transforms(xf, rebuild=rebuild); T.path_trace(1, util.BASE_SEED)
         assert np.isfinite(T.get_hdr()).all()
     for k in (env or {}): del os.environ[k]

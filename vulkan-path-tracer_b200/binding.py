@@ -198,6 +198,9 @@ def lib():
             "b200pt_build_env_alias": [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_float)],
             "b200pt_bvh4_collapse": [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32)],
             "b200pt_bvh2_sah_build": [C.c_void_p, C.c_uint32, C.c_float, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.POINTER(C.c_double)],
+            "b200pt_bvh2_ploc_build": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.POINTER(C.c_double)],
+            "b200pt_bvh2_ploc_build_query": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32),
+                                             C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32)],
             "b200pt_bvh2_reinsert": [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_int32, C.c_float, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.c_void_p],
             "b200pt_bvh2_sah_rebuild": [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.c_void_p],
             "b200pt_load_gltf": [C.c_char_p, C.POINTER(C.POINTER(SceneDesc))], "b200pt_free_scene": [C.POINTER(SceneDesc)],
@@ -317,6 +320,17 @@ def bvh2_sah_build(ref_boxes, trav_cost=1.0):
     n, d, c = C.c_uint32(), C.c_int32(), C.c_double()
     r = lib().b200pt_bvh2_sah_build(_p(rb), len(rb), C.c_float(trav_cost), _p(out), _p(perm), C.byref(n), C.byref(d), C.byref(c))
     if r != OK: raise B200ptError(r, "bvh2_sah_build")
+    return out[:n.value].copy(), perm, d.value, c.value
+
+
+def bvh2_ploc_build(ref_boxes):
+    """PLOC build from reference boxes [n, 6] in Morton order (csrc/lbvh.cu: bvh2_ploc_build_host, the host restatement of the GPU builder).
+    Returns (nodes, perm, depth, sah_cost); no nodes for n <= 4 or an inverted / NaN box."""
+    rb = np.ascontiguousarray(ref_boxes, np.float32).reshape(-1, 6)
+    out = np.zeros(max(len(rb) - 1, 1), BVH2_DTYPE); perm = np.zeros(len(rb), np.uint32)
+    n, d, c = C.c_uint32(), C.c_int32(), C.c_double()
+    r = lib().b200pt_bvh2_ploc_build(_p(rb), len(rb), _p(out), _p(perm), C.byref(n), C.byref(d), C.byref(c))
+    if r != OK: raise B200ptError(r, "bvh2_ploc_build")
     return out[:n.value].copy(), perm, d.value, c.value
 
 
@@ -466,10 +480,27 @@ class PathTracer:
         out = np.zeros((self.instance_count(), 16), np.float32)
         self._ck(self.L.b200pt_get_instance_transforms(self.h, _p(out), len(out))); return out
 
+    REBUILD_GPU = 2     # B200PT_REBUILD_GPU
+
     def update_instance_transforms(self, xf, rebuild=False):
-        """xf: (n, 16) column-major transforms, one per instance.  rebuild=False refits the tree in place; True builds it anew."""
+        """xf: (n, 16) column-major transforms, one per instance.  rebuild: False / 0 refits the tree in place; "gpu" / REBUILD_GPU (2, the C
+        API's B200PT_REBUILD_GPU) builds a new tree on the GPU (PLOC, milliseconds); True / 1 builds the tree set_scene would build (host passes)."""
         xf = np.ascontiguousarray(xf, np.float32).reshape(-1, 16)
-        self._ck(self.L.b200pt_update_instance_transforms(self.h, _p(xf), len(xf), 1 if rebuild else 0))
+        modes = {"gpu": self.REBUILD_GPU, self.REBUILD_GPU: self.REBUILD_GPU, True: 1, False: 0}   # True == 1, False == 0 as keys
+        if isinstance(rebuild, (np.integer, np.bool_)): rebuild = rebuild.item()
+        if not isinstance(rebuild, (str, bool, int)) or rebuild not in modes:
+            raise ValueError(f"rebuild must be False / 0, True / 1 or 'gpu' / {self.REBUILD_GPU}, not {rebuild!r}")
+        mode = modes[rebuild]
+        self._ck(self.L.b200pt_update_instance_transforms(self.h, _p(xf), len(xf), mode))
+
+    def bvh2_ploc_build_query(self, ref_boxes):
+        """b200pt_bvh2_ploc_build_query: the GPU builder and the GPU BVH4 collapse on reference boxes [n, 6] in the given order.
+        Returns (nodes, perm, depth, nodes4, depth4)."""
+        rb = np.ascontiguousarray(ref_boxes, np.float32).reshape(-1, 6)
+        out = np.zeros(max(len(rb) - 1, 1), BVH2_DTYPE); perm = np.zeros(len(rb), np.uint32); out4 = np.zeros(max(len(rb) - 1, 1), BVH4_DTYPE)
+        n, d, n4, d4 = C.c_uint32(), C.c_int32(), C.c_uint32(), C.c_int32()
+        self._ck(self.L.b200pt_bvh2_ploc_build_query(self.h, _p(rb), len(rb), _p(out), _p(perm), C.byref(n), C.byref(d), _p(out4), C.byref(n4), C.byref(d4)))
+        return out[:n.value].copy(), perm, d.value, out4[:n4.value].copy(), d4.value
 
     def set_env_map(self, rgba):
         rgba = np.ascontiguousarray(rgba, np.float32)

@@ -123,7 +123,7 @@ int32_t b200pt_get_instance_transforms(b200pt_handle h, float *xf, uint32_t coun
 }
 int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *xf, uint32_t count, int32_t rebuild) {
     if (!xf) return B200PT_ERR_WRONG_ARGUMENTS;
-    return guard(h, [&](Engine &e) { e.update_instance_transforms(xf, count, rebuild != 0); });
+    return guard(h, [&](Engine &e) { e.update_instance_transforms(xf, count, rebuild); });
 }
 int32_t b200pt_set_camera(b200pt_handle h, const float vi[16], const float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_camera(vi, pi); }); }
 int32_t b200pt_get_camera(b200pt_handle h, float vi[16], float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.get_camera(vi, pi); }); }
@@ -365,6 +365,25 @@ int32_t b200pt_bvh2_sah_build(const float *ref_boxes, uint32_t n, float trav_cos
     if (depth_out) *depth_out = d;
     if (sah_cost) *sah_cost = c;
     return B200PT_OK;
+}
+int32_t b200pt_bvh2_ploc_build(const float *ref_boxes, uint32_t n, void *out, uint32_t *perm, uint32_t *n_out, int32_t *depth_out, double *sah_cost) {
+    if (!ref_boxes || !out || !perm || !n_out || !n) return B200PT_ERR_WRONG_ARGUMENTS;
+    int d = 0; double c = 0.0;
+    try { *n_out = b200pt::bvh2_ploc_build_host(ref_boxes, n, static_cast<b200pt::BvhNode *>(out), perm, &d, &c); }
+    catch (...) { return B200PT_ERR_OUT_OF_MEMORY; }
+    if (depth_out) *depth_out = d;
+    if (sah_cost) *sah_cost = c;
+    return B200PT_OK;
+}
+int32_t b200pt_bvh2_ploc_build_query(b200pt_handle h, const float *ref_boxes, uint32_t n, void *nodes_out, uint32_t *perm_out, uint32_t *n_out, int32_t *depth_out,
+                                     void *nodes4_out, uint32_t *n4_out, int32_t *depth4_out) {
+    if (!ref_boxes || !nodes_out || !perm_out || !n_out || !nodes4_out || !n4_out || !n) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) {
+        int d = 0, d4 = 0;
+        e.ploc_build_query(ref_boxes, n, static_cast<b200pt::BvhNode *>(nodes_out), perm_out, n_out, &d, static_cast<b200pt::Bvh4Node *>(nodes4_out), n4_out, &d4);
+        if (depth_out) *depth_out = d;
+        if (depth4_out) *depth4_out = d4;
+    });
 }
 int32_t b200pt_bvh2_reinsert(const void *nodes2, uint32_t n_nodes2, int32_t root2, void *out, int32_t passes, float fraction, uint32_t *n_out, int32_t *depth_out, double *sah) {
     if (!nodes2 || !out || !n_out || !n_nodes2 || passes < 0 || passes > 64 || !(fraction >= 0.0f && fraction <= 1.0f)) return B200PT_ERR_WRONG_ARGUMENTS;

@@ -40,6 +40,7 @@ Engine::Engine(int device) : device_(device) {
     }
     CK(cudaEventCreateWithFlags(&image_free_ev_, cudaEventDisableTiming));
     CK(cudaMallocHost(&h_active_count_, sizeof(uint32_t)));
+    CK(cudaMallocHost(&h_small_, 4 * sizeof(uint32_t)));
     b200pt_default_adaptive(&adaptive_);
     b200pt_default_atmosphere(&atmosphere_);
     memset(&last_, 0, sizeof last_);
@@ -51,6 +52,7 @@ Engine::~Engine() {
     if (stream_) cudaStreamSynchronize(stream_);
     free_scene(); free_wave(); free_post(); free_adaptive(); free_denoise(); dfree(d_dn_img_);
     if (h_active_count_) cudaFreeHost(h_active_count_);
+    if (h_small_) cudaFreeHost(h_small_);
     dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_); for (auto &l : d_luts_) dfree(l);
     dfree(d_image_); dfree(d_ctr_); dfree(d_volumes_); dfree(d_grids_); grids_.clear(); dfree(d_tri_class_);
     for (int c = 0; c < 2; c++) {
@@ -162,15 +164,23 @@ void Engine::fill_instances() {
 
 // The acceleration structure of the instances in d_instances_, built into *out (which the caller owns, also on failure): the BVH fields of *ds
 // and the launch configuration *lc are set from it.  set_scene and update_instance_transforms(rebuild) both use it.
-void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc) {
+// gpu_builder: the tree is built on the device (PLOC over the LBVH's references, ploc.cu) instead of by the host tree-quality passes.
+void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_builder) {
     // acceleration structure: GPU LBVH over the flattened instances
     // tree-quality pass over the GPU LBVH: same hits, fewer node visits / triangle tests.  Level 3 (full binned-SAH build + insertion-based
     // refinement) is the default;
     // B200PT_BVH_SAH=0..5 overrides (0 = plain LBVH).
     int sah_mode = 3;
     if (const char *e = getenv("B200PT_BVH_SAH")) sah_mode = (e[0] >= '0' && e[0] <= '5' && e[1] == 0) ? e[0] - '0' : 3;
-    int r = lbvh_build(d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_, sah_mode == 2 || sah_mode == 3);
+    if (gpu_builder) sah_mode = 0;
+    float *d_ref_box = nullptr;
+    int r = lbvh_build(d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_, sah_mode == 2 || sah_mode == 3,
+                       gpu_builder ? &d_ref_box : nullptr);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build failed: ") + cudaGetErrorString((cudaError_t)r) };
+    if (gpu_builder) {
+        r = lbvh_ploc_rebuild(out, d_ref_box, h_small_, stream_);                      // frees d_ref_box
+        if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_ploc_rebuild failed: ") + cudaGetErrorString((cudaError_t)r) };
+    }
     if (sah_mode) {
         double sah[2];
         r = lbvh_refine_sah(out, stream_, sah, sah_mode);
@@ -181,7 +191,7 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc) {
     ds->n_tris = out->n_tris; ds->n_nodes = out->n_nodes; ds->root = out->root; ds->bvh_bytes = out->bytes <= 0xFFFFFFFFull ? (uint32_t)out->bytes : 0;
     ds->nodes4 = nullptr; ds->n_nodes4 = 0;
     if (out->bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
-        r = lbvh_build_wide(out, stream_);
+        r = gpu_builder ? lbvh_build_wide_device(out, h_small_, stream_) : lbvh_build_wide(out, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build_wide failed: ") + cudaGetErrorString((cudaError_t)r) };
         ds->nodes4 = out->nodes4; ds->n_nodes4 = out->n_nodes4;
     }
@@ -195,11 +205,11 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc) {
     if (q != 0) throw CudaError{ B200PT_ERR_CUDA, "query_launch_cfg failed" };
 }
 
-// TLAS::Update (VulkanHelper/Source/Vulkan/TLASImpl.cpp:192-293): every instance transform replaced, the tree refit in place (rebuild == false)
-// or built anew as set_scene would build it; then ResetPathTracing.  Camera, config, image size, partition, materials, volumes and the
+// TLAS::Update (VulkanHelper/Source/Vulkan/TLASImpl.cpp:192-293): every instance transform replaced, the tree refit in place (rebuild == 0),
+// built anew on the device (B200PT_REBUILD_GPU) or as set_scene would build it (any other value); then ResetPathTracing.  Camera, config, image size, partition, materials, volumes and the
 // environment stay.  Every argument is checked before anything changes.  A failed update restores the previous transforms: a failed rebuild keeps
 // the previous tree, a failed refit refits the tree back to them (and if that fails too, the handle has no scene until the next set_scene).
-void Engine::update_instance_transforms(const float *xf, uint32_t count, bool rebuild) {
+void Engine::update_instance_transforms(const float *xf, uint32_t count, int rebuild) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
     if (!xf || count != scene_.instances.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform count differs from the instance count" };
@@ -224,7 +234,7 @@ void Engine::update_instance_transforms(const float *xf, uint32_t count, bool re
         }
     } else {
         LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
-        try { build_bvh(&fresh, &ds, &lc); }
+        try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
         catch (...) { lbvh_free(&fresh); apply(old); throw; }
         lbvh_free(&bvh_); lbvh_refit_free(&refit_);
         bvh_ = fresh; ds_ = ds; lc_ = lc;
@@ -1254,6 +1264,33 @@ void Engine::post_process_denoised() {
 }
 void Engine::scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const {
     if (tris) *tris = n_tris_; if (nodes) *nodes = bvh_.n_nodes; if (emissive) *emissive = n_emissive_; if (textures) *textures = (uint32_t)scene_.textures.size();
+}
+
+// The launchers update_instance_transforms(B200PT_REBUILD_GPU) runs, on the caller's boxes in the given order (no scene needed).  Rejects what
+// bvh2_ploc_build_host rejects: nothing is written but zero counts.
+void Engine::ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes_out, uint32_t *perm_out, uint32_t *n_out, int *depth_out,
+                              Bvh4Node *nodes4_out, uint32_t *n4_out, int *depth4_out) {
+    CK(cudaSetDevice(device_));
+    *n_out = 0; *depth_out = 0; *n4_out = 0; *depth4_out = 0;
+    for (size_t i = 0; i < (size_t)n; i++)
+        for (int a = 0; a < 3; a++) if (!(ref_boxes[i * 6 + a] <= ref_boxes[i * 6 + 3 + a])) return;
+    struct Bufs { float *box = nullptr; BvhNode *nodes = nullptr; uint32_t *perm = nullptr; Bvh4Node *nodes4 = nullptr;
+                  ~Bufs() { dfree(box); dfree(nodes); dfree(perm); dfree(nodes4); } } b;
+    CK(cudaMalloc(&b.box, (size_t)n * 6 * sizeof(float))); CK(cudaMalloc(&b.nodes, (size_t)(n - 1) * sizeof(BvhNode))); CK(cudaMalloc(&b.perm, (size_t)n * 4));
+    CK(cudaMemcpyAsync(b.box, ref_boxes, (size_t)n * 6 * sizeof(float), cudaMemcpyHostToDevice, stream_));
+    uint32_t n2 = 0; int d2 = 0;
+    int r = ploc_build(b.box, n, b.nodes, b.perm, &n2, &d2, h_small_, stream_);
+    if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("ploc_build failed: ") + cudaGetErrorString((cudaError_t)r) };
+    if (n2 == 0) return;
+    CK(cudaMalloc(&b.nodes4, (size_t)n2 * sizeof(Bvh4Node)));
+    uint32_t n4 = 0; int d4 = 0;
+    r = bvh4_collapse_device(b.nodes, n2, 0, b.nodes4, &n4, &d4, h_small_, stream_);
+    if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("bvh4_collapse_device failed: ") + cudaGetErrorString((cudaError_t)r) };
+    CK(cudaMemcpyAsync(nodes_out, b.nodes, (size_t)n2 * sizeof(BvhNode), cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(perm_out, b.perm, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
+    if (n4) CK(cudaMemcpyAsync(nodes4_out, b.nodes4, (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    *n_out = n2; *depth_out = d2; *n4_out = n4; *depth4_out = d4;
 }
 
 } // namespace b200pt

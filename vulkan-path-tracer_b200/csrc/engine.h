@@ -20,8 +20,9 @@ public:
     void set_config(const b200pt_config &c);
     const b200pt_config &config() const { return cfg_; }
     void set_material(uint32_t idx, const b200pt_material &m);
-    // TLAS::Update: count x 16 floats (b200pt_instance::Transform), refit in place or (rebuild) the tree set_scene would build
-    void update_instance_transforms(const float *transforms, uint32_t count, bool rebuild);
+    // TLAS::Update: count x 16 floats (b200pt_instance::Transform); rebuild: 0 refits in place, B200PT_REBUILD_GPU builds on the device (PLOC),
+    // any other value builds the tree set_scene would build
+    void update_instance_transforms(const float *transforms, uint32_t count, int rebuild);
     // PathTracer::AddVolume / SetVolume / RemoveVolume / SetPhaseFunction / AddDensityDataToVolume / RemoveDensityDataFromVolume (volumes.cuh)
     uint32_t add_volume(const b200pt_volume &v);
     void set_volume(uint32_t idx, const b200pt_volume &v);
@@ -97,6 +98,9 @@ public:
     void shade_query(bool force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv, const float *dir, const float *org,
                      const float *pay_pdf, const uint32_t *rng, const float *L, float *out);
     void scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const;
+    // b200pt_bvh2_ploc_build_query (host arrays; see include/b200pt.h): the device builder and the device collapse on the caller's boxes
+    void ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes_out, uint32_t *perm_out, uint32_t *n_out, int *depth_out,
+                          Bvh4Node *nodes4_out, uint32_t *n4_out, int *depth4_out);
     void bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out_host, float *elapsed_ms);
 
     std::string last_error;
@@ -105,7 +109,7 @@ private:
     void free_scene();
     void upload_scene();
     void fill_instances();                          // h_instances_ and n_tris_ from scene_.instances
-    void build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc);   // the BVH half of upload_scene
+    void build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_builder = false);   // the BVH half of upload_scene
     void rebuild_emissive();
     void rebuild_tri_class();                       // per-triangle shading class (MaterialClass) + the set of classes present in the scene
     void upload_volumes();
@@ -146,6 +150,7 @@ private:
     b200pt_atmosphere atmosphere_{};
     LbvhResult bvh_{};
     LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
+    uint32_t *h_small_ = nullptr;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
     LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
     uint8_t *d_tri_class_ = nullptr; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c

@@ -133,7 +133,8 @@ struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri 
 // Builds into ONE contiguous allocation [nodes | tris] (so small scenes can be staged to smem with one bulk copy).
 // Returns cudaError_t as int.
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
-               const DevInstance *h_instances, const DevMesh *h_meshes, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes = false);
+               const DevInstance *h_instances, const DevMesh *h_meshes, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes = false,
+               float **dev_ref_box = nullptr);   // dev_ref_box: receives the Morton-ordered per-slot reference boxes (device, n_tris x 6; the caller frees)
 void lbvh_free(LbvhResult *r);
 // BVH2 -> BVH4 on the host (pure CPU code, unit-tested without a GPU through b200pt_bvh4_collapse).  `out` must hold n_nodes2 entries.
 // Returns the number of BVH4 nodes written (0 if the root is a leaf), *depth4 = depth of the BVH4 (root = 1).
@@ -145,6 +146,23 @@ uint32_t bvh2_sah_rebuild_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t
 uint32_t bvh2_reinsert_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t root2, BvhNode *out, int passes, float fraction, int *depth, double sah[2]);
 // Full binned-SAH build from per-slot reference boxes (n x 6 floats); leaves are re-formed, perm[new slot] = old slot; see lbvh.cu.
 uint32_t bvh2_sah_build_host(const float *ref_boxes, uint32_t n, float trav_cost, BvhNode *out, uint32_t *perm, int *depth, double *sah_cost);
+// PLOC build from reference boxes in Morton order (pure CPU code; the host restatement of ploc_build, which must match it bit for bit).
+// Conventions and rejections of bvh2_sah_build_host; *depth = inner-node depth (root = 1).
+uint32_t bvh2_ploc_build_host(const float *ref_boxes, uint32_t n, BvhNode *out, uint32_t *perm, int *depth, double *sah_cost);
+// ---- GPU tree build (ploc.cu) ----
+// The PLOC build of n reference boxes (device, Morton order, unpadded) into out (room for n - 1 nodes) and perm (n entries) on the device:
+// *n_out nodes (0 when n <= LBVH_LEAF_MAX), *depth; the two come back in one readback.  h_small: caller-owned pinned host memory of 4 words
+// for the readbacks (one per clustering step).  Returns cudaError_t as int.
+int ploc_build(const float *d_ref_box, uint32_t n, BvhNode *d_out, uint32_t *d_perm, uint32_t *n_out, int *depth, uint32_t *h_small, cudaStream_t st);
+// BVH2 -> BVH4 on the device, byte for byte bvh4_collapse_host's output (breadth-first, level by level).  d_out: room for n_nodes2 nodes.
+// h_small: pinned host word for the per-level count.
+int bvh4_collapse_device(const BvhNode *d_nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *d_out, uint32_t *n4, int *depth4, uint32_t *h_small, cudaStream_t st);
+// The GPU rebuild of an LBVH (update_instance_transforms(rebuild == 2)): ploc_build over the Morton-ordered reference boxes lbvh_build kept on the
+// device, then the BvhTri slots permuted and tri_slot re-derived on the device.  A tree deeper than BVH_STACK_MAX - 2 and than the LBVH is
+// dropped (the LBVH stays).  Frees d_ref_box.  Returns cudaError_t as int.
+int lbvh_ploc_rebuild(LbvhResult *r, float *d_ref_box, uint32_t *h_small, cudaStream_t st);
+// lbvh_build_wide with the collapse on the device (scratch of n_nodes BVH4 nodes; r->nodes4 is allocated at the exact size).
+int lbvh_build_wide_device(LbvhResult *r, uint32_t *h_small, cudaStream_t st);
 // mode 1: inner nodes only (download, rebuild, upload in place); mode 2: full build from r->h_ref_box, reference slots and tri_slot permuted
 // (falls back to mode 1 when the boxes were not kept); mode 3: mode 2 + insertion-based refinement; 4: mode 1 + refinement; 5: refinement only.  Returns cudaError_t as int.
 // A pass result deeper than BVH_STACK_MAX - 2 is dropped unless the input tree is deeper still (query_launch_cfg sizes the stacks from the depth).

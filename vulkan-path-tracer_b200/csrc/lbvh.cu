@@ -9,6 +9,7 @@
 // Output layout (one contiguous allocation so small scenes are staged into shared memory with one TMA bulk copy):
 //   [ BvhNode x max(N-1,1) | BvhTri x N ]   nodes: 64 B, both child boxes in the parent; tris: 48 B, Morton order.
 #include "kernels.h"
+#include "bvh_build_rules.cuh"
 #include <vector>
 #include <condition_variable>
 #include <mutex>
@@ -348,14 +349,8 @@ __device__ __forceinline__ int lbvh_child_ref(int c, const int2 *range) {
 // absolute pad: the FMA slab test of bvh_trace perturbs a plane by <= 6e-8*|ray origin|; 2e-6 * (largest |coordinate| of the scene)
 // keeps it conservative for origins within ~16 scene extents (every secondary ray), and also covers the rounding of the
 // subtract-multiply form, so the traversal needs no slack factor on its interval comparison
-__device__ __forceinline__ float scene_pad(const float *bounds) {
-    float ext = 0.0f;
-    for (int k = 0; k < 6; k++) ext = fmaxf(ext, fabsf(bounds[k]));
-    return 2e-6f * ext + 1e-30f;
-}
-__device__ __forceinline__ void pad_child(const float *box, float pabs, float *lo, float *hi) {   // box: lo xyz, hi xyz (unpadded)
-    for (int k = 0; k < 3; k++) { const float p = 4e-7f * fmaxf(fabsf(box[k]), fabsf(box[3 + k])) + pabs; lo[k] = box[k] - p; hi[k] = box[3 + k] + p; }
-}
+__device__ __forceinline__ float scene_pad(const float *bounds) { return bvh_scene_pad(bounds); }
+__device__ __forceinline__ void pad_child(const float *box, float pabs, float *lo, float *hi) { bvh_pad_child(box, pabs, lo, hi); }   // box: lo xyz, hi xyz (unpadded)
 __global__ void k_emit(int n_int, const int *__restrict__ left, const int *__restrict__ right, const int2 *__restrict__ range, const float *__restrict__ leaf_box,
                        const float *__restrict__ node_box, const float *__restrict__ bounds, BvhNode *__restrict__ nodes) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -448,7 +443,7 @@ static uint32_t bvh4_collapse_src(const BvhNode *nodes2, uint32_t n_nodes2, int3
     if (depth4) *depth4 = 0;
     if (root2 < 0 || n_nodes2 == 0) return 0;
     struct Slot { int32_t child, src; float lo[3], hi[3]; };
-    auto area = [](const Slot &s) { const float dx = s.hi[0] - s.lo[0], dy = s.hi[1] - s.lo[1], dz = s.hi[2] - s.lo[2]; return dx * dy + dy * dz + dz * dx; };
+    auto area = [](const Slot &s) { return bvh4_slot_area(s.lo, s.hi); };   // ploc.cu's device collapse ranks by the same bits
     bool bad = false;                                                       // a child index outside the array or a cycle: not a tree
     auto slots_of = [&](int32_t n, Slot &a, Slot &b) {
         if ((uint32_t)n >= n_nodes2) { bad = true; n = 0; }
@@ -841,6 +836,56 @@ uint32_t bvh2_sah_build_host(const float *ref_boxes, uint32_t n, float trav_cost
     return n_out;
 }
 
+// PLOC build from reference boxes in Morton order: the host restatement of ploc.cu's device builder, step for step through the same helpers
+// (bvh_build_rules.cuh), so the two give the same nodes, perm and depth bit for bit.  Every reference starts as a cluster; each step, every
+// cluster finds its nearest neighbour (ploc_nearest), each mutual pair i < j merges into a new node (left i, right j) that takes position i,
+// and the surviving clusters are compacted in order.  Leaves by ploc_leaf_ok (the topmost qualifying node wins), nodes depth-first, left
+// first, root 0, child boxes padded by bvh_pad_child with the pad of the references' union.  Conventions and rejections of bvh2_sah_build_host.
+uint32_t bvh2_ploc_build_host(const float *ref_boxes, uint32_t n, BvhNode *out, uint32_t *perm, int *depth, double *sah_cost) {
+    if (depth) *depth = 0;
+    if (sah_cost) *sah_cost = 0.0;
+    if (!ref_boxes || !out || !perm || n <= (uint32_t)LBVH_LEAF_MAX || n >= (1u << 28)) return 0;
+    for (size_t i = 0; i < (size_t)n; i++)
+        for (int a = 0; a < 3; a++) if (!(ref_boxes[i * 6 + a] <= ref_boxes[i * 6 + 3 + a])) return 0;   // NaN or inverted box
+    std::vector<float> box((size_t)(2 * n - 1) * 6);
+    std::copy(ref_boxes, ref_boxes + (size_t)n * 6, box.begin());
+    std::vector<PlocMeta> meta(2 * n - 1, PlocMeta{ 1u, 0u, 0u, 1u });
+    std::vector<uint32_t> child(2 * (size_t)(n - 1)), cl(n), nxt, nn(n);
+    for (uint32_t i = 0; i < n; i++) cl[i] = i;
+    uint32_t next = n;
+    while (cl.size() > 1) {
+        const uint32_t m = (uint32_t)cl.size();
+        for (uint32_t i = 0; i < m; i++) nn[i] = ploc_nearest(cl.data(), m, i, box.data());
+        nxt.clear();
+        for (uint32_t i = 0; i < m; i++) {
+            const uint32_t j = nn[i];
+            const bool mutual = nn[j] == i;
+            if (mutual && j < i) continue;                                     // merged into position j
+            uint32_t id = cl[i];
+            if (mutual) { id = next++; ploc_merge(id, cl[i], cl[j], n, box.data(), meta.data(), child.data()); }
+            nxt.push_back(id);
+        }
+        cl.swap(nxt);
+    }
+    const uint32_t root = cl[0], n_out = meta[root].sub;
+    const float pabs = bvh_scene_pad(&box[(size_t)root * 6]);
+    struct Task { uint32_t x, idx, first; };
+    std::vector<Task> stack{ { root, 0u, 0u } };
+    while (!stack.empty()) {
+        const Task t = stack.back(); stack.pop_back();
+        uint32_t kid_idx[2], kid_first[2];
+        ploc_emit(t.x, t.idx, t.first, n, box.data(), meta.data(), child.data(), pabs, out, perm, kid_idx, kid_first);
+        for (int s = 0; s < 2; s++) if (kid_idx[s] != 0xFFFFFFFFu) stack.push_back({ child[2 * (size_t)(t.x - n) + s], kid_idx[s], kid_first[s] });
+    }
+    if (depth) *depth = (int)meta[root].dep;
+    if (sah_cost) {
+        int d; double c; tree_depth_cost(out, n_out, &d, &c);
+        const float *rb = &box[(size_t)root * 6]; const double ra = sah_area(rb, rb + 3);
+        *sah_cost = ra > 0 ? c / ra : 0.0;
+    }
+    return n_out;
+}
+
 int lbvh_build_wide(LbvhResult *r, cudaStream_t st) {
     r->nodes4 = nullptr; r->n_nodes4 = 0; r->depth4 = 0;
     if (!r->nodes || r->root < 0 || r->n_nodes == 0) return 0;
@@ -1048,7 +1093,9 @@ void lbvh_free(LbvhResult *r) {
 }
 
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
-               const DevInstance *, const DevMesh *, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes) {
+               const DevInstance *, const DevMesh *, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes,
+               float **dev_ref_box) {
+    if (dev_ref_box) *dev_ref_box = nullptr;
     out->shade = nullptr; out->tri_slot = nullptr; out->h_ref_box = nullptr; out->n_prims = n_tris;
     out->nodes = nullptr; out->tris = nullptr; out->n_nodes = 0; out->n_tris = n_tris; out->root = 0; out->max_depth = 1; out->bytes = 0;
     out->nodes4 = nullptr; out->n_nodes4 = 0; out->depth4 = 0;
@@ -1141,7 +1188,9 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
         if (out->h_ref_box) LBVH_CHECK(cudaMemcpy(out->h_ref_box, leaf_box, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
     }
     cudaFree(tmp); cudaFree(aabb); cudaFree(bounds); cudaFree(ksplit); cudaFree(ref_off);
-    cudaFree(ref_box); cudaFree(ref_tri); cudaFree(leaf_box); cudaFree(node_box);
+    if (dev_ref_box && n_int) *dev_ref_box = leaf_box;                      // the GPU builder (lbvh_ploc_rebuild) works from these, on the device
+    else cudaFree(leaf_box);
+    cudaFree(ref_box); cudaFree(ref_tri); cudaFree(node_box);
     cudaFree(keys); cudaFree(vals); cudaFree(keys2); cudaFree(vals2); cudaFree(hist);
     cudaFree(left); cudaFree(right); cudaFree(parent_int); cudaFree(parent_leaf); cudaFree(flags); cudaFree(range);
 
