@@ -131,6 +131,25 @@ int32_t b200pt_instance_count(b200pt_handle h, uint32_t *out);
 int32_t b200pt_get_instance_transforms(b200pt_handle h, float *transforms, uint32_t count);
 #define B200PT_REBUILD_GPU 2
 int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *transforms, uint32_t count, int32_t rebuild);
+/* ---- mesh vertices (no reference equivalent: its BLAS are built once in SetScene) ----
+ * One call replaces the whole vertex array (position, normal, UV) of each listed mesh; every instance of an updated mesh changes.  Indices and
+ * vertex counts stay: vertex_count must equal the mesh's count.  The batch gets one tree update: rebuild has the meaning it has in
+ * b200pt_update_instance_transforms (0 refits, B200PT_REBUILD_GPU builds on the GPU, any other value builds what set_scene builds).  The
+ * update waits for the waves in flight and resets the accumulation (ResetPathTracing); camera, config, image size, partition, materials,
+ * volumes, environment and instance transforms stay.
+ * vertices_are_device != 0: every update's vertices pointer is device memory of the handle's GPU, read on the handle's stream.  The caller
+ * orders its own writes of those buffers before the call: by synchronising the stream that wrote them, or by writing them on the stream given
+ * to b200pt_set_stream.  The buffers are staged and checked on the device; nothing is committed before the check passes.
+ * WRONG_ARGUMENTS: a null pointer, n_updates == 0, a mesh index out of range or repeated, a count mismatch or a non-finite component;
+ * NO_SCENE without a scene.  A rejected call changes nothing.  A failed update restores the previous vertices: a failed rebuild keeps the
+ * previous tree, a failed refit refits the tree back (if that fails too, the handle reports NO_SCENE until the next set_scene).  The image
+ * equals that of a handle loaded with the deformed scene. */
+typedef struct { uint32_t mesh; uint32_t vertex_count; const b200pt_vertex *vertices; } b200pt_mesh_update;
+int32_t b200pt_mesh_count(b200pt_handle h, uint32_t *out);
+int32_t b200pt_mesh_vertex_count(b200pt_handle h, uint32_t mesh, uint32_t *out);
+int32_t b200pt_get_mesh_vertices(b200pt_handle h, uint32_t mesh, b200pt_vertex *out, uint32_t count);   /* count must equal the mesh's */
+int32_t b200pt_update_mesh_vertices(b200pt_handle h, const b200pt_mesh_update *updates, uint32_t n_updates,
+                                    int32_t vertices_are_device, int32_t rebuild);
 int32_t b200pt_set_camera(b200pt_handle h, const float view_inverse[16], const float projection_inverse[16]); /* SetCameraViewInverse/ProjectionInverse */
 int32_t b200pt_get_camera(b200pt_handle h, float view_inverse[16], float projection_inverse[16]);
 /* the Editor/FlyCamera round trip that produces the matrices the shader really sees (Editor.cpp:45-48,1042-1051; FlyCamera.cpp:84-140) */

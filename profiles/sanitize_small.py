@@ -80,4 +80,15 @@ def _update(name, inst, env=None):                                  # instance u
     for k in (env or {}): del os.environ[k]
     print(name, "instance updates ok")
 _update("cornell_box", 5); _update("cornell_box_glass", 6); _update("viking_room", 0, {"B200PT_WIDE": "1"})
+def _deform(name, mesh):                                            # mesh vertex updates: host input (refit), device input (k_flag_nonfinite, refit + k_refresh_shade)
+    import torch
+    T = util.product_tracer(name, 40, 30, MaxDepth=5)
+    T.path_trace(1, util.BASE_SEED)
+    v = T.get_mesh_vertices(mesh).view(np.float32).reshape(-1, 8).copy(); v[:, 0:3] *= 1.1
+    T.update_mesh_vertices({mesh: v}); T.path_trace(1, util.BASE_SEED)
+    v[:, 0:3] *= 0.9
+    T.update_mesh_vertices({mesh: torch.from_numpy(v).cuda(0)}); T.path_trace(1, util.BASE_SEED)
+    assert np.isfinite(T.get_hdr()).all()
+    print(name, "mesh updates ok")
+_deform("cornell_box_glass", 6)
 print("sanitize_small done")

@@ -45,6 +45,13 @@ class Instance(C.Structure):
     _fields_ = [("Transform", C.c_float * 16), ("MeshIndex", C.c_uint32), ("MaterialIndex", C.c_uint32)]
 
 
+class MeshUpdate(C.Structure):      # b200pt_mesh_update
+    _fields_ = [("mesh", C.c_uint32), ("vertex_count", C.c_uint32), ("vertices", C.c_void_p)]
+
+
+VERTEX_DTYPE = np.dtype([("pos", "<f4", 3), ("nrm", "<f4", 3), ("uv", "<f4", 2)])   # b200pt_vertex, the mesh arrays of load_gltf
+
+
 class Texture(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("channels", C.c_uint32), ("_pad", C.c_uint32), ("data", C.c_void_p)]
 
@@ -215,6 +222,9 @@ def lib():
             "b200pt_post_process_denoised": [C.c_void_p],
             "b200pt_instance_count": [C.c_void_p, C.POINTER(C.c_uint32)], "b200pt_get_instance_transforms": [C.c_void_p, C.c_void_p, C.c_uint32],
             "b200pt_update_instance_transforms": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32],
+            "b200pt_mesh_count": [C.c_void_p, C.POINTER(C.c_uint32)], "b200pt_mesh_vertex_count": [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)],
+            "b200pt_get_mesh_vertices": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32],
+            "b200pt_update_mesh_vertices": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.c_int32],
         }
         for name, args in sig.items():
             fn = getattr(L, name); fn.restype = C.c_int32; fn.argtypes = args
@@ -365,7 +375,7 @@ def load_gltf(path):
     r = lib().b200pt_load_gltf(path.encode(), C.byref(pd))
     if r != OK: raise B200ptError(r, lib().b200pt_last_error(None).decode(errors="replace"))
     d = pd.contents
-    vdt = np.dtype([("pos", "<f4", 3), ("nrm", "<f4", 3), ("uv", "<f4", 2)])
+    vdt = VERTEX_DTYPE
     meshes = []
     ms = C.cast(d.meshes, C.POINTER(Mesh))
     for i in range(d.mesh_count):
@@ -389,7 +399,7 @@ class PathTracer:
     """One GPU: the reference's PathTracer + PostProcessor behind the C-ABI."""
 
     def __init__(self, device=0):
-        self.L = lib(); self.h = C.c_void_p()
+        self.L = lib(); self.h = C.c_void_p(); self.device = device
         r = self.L.b200pt_create(device, C.byref(self.h))
         if r != OK: raise B200ptError(r, self.L.b200pt_last_error(None).decode(errors="replace"))
         self._keep = []
@@ -486,12 +496,57 @@ class PathTracer:
         """xf: (n, 16) column-major transforms, one per instance.  rebuild: False / 0 refits the tree in place; "gpu" / REBUILD_GPU (2, the C
         API's B200PT_REBUILD_GPU) builds a new tree on the GPU (PLOC, milliseconds); True / 1 builds the tree set_scene would build (host passes)."""
         xf = np.ascontiguousarray(xf, np.float32).reshape(-1, 16)
+        mode = self._rebuild_mode(rebuild)
+        self._ck(self.L.b200pt_update_instance_transforms(self.h, _p(xf), len(xf), mode))
+
+    def _rebuild_mode(self, rebuild):
         modes = {"gpu": self.REBUILD_GPU, self.REBUILD_GPU: self.REBUILD_GPU, True: 1, False: 0}   # True == 1, False == 0 as keys
         if isinstance(rebuild, (np.integer, np.bool_)): rebuild = rebuild.item()
         if not isinstance(rebuild, (str, bool, int)) or rebuild not in modes:
             raise ValueError(f"rebuild must be False / 0, True / 1 or 'gpu' / {self.REBUILD_GPU}, not {rebuild!r}")
-        mode = modes[rebuild]
-        self._ck(self.L.b200pt_update_instance_transforms(self.h, _p(xf), len(xf), mode))
+        return modes[rebuild]
+
+    # ---- mesh vertices (no reference equivalent) without reloading the scene
+    def mesh_count(self):
+        n = C.c_uint32(); self._ck(self.L.b200pt_mesh_count(self.h, C.byref(n))); return n.value
+
+    def get_mesh_vertices(self, mesh):
+        """the vertices of mesh `mesh` as a VERTEX_DTYPE array (pos / nrm / uv, as load_gltf returns them)"""
+        n = C.c_uint32(); self._ck(self.L.b200pt_mesh_vertex_count(self.h, int(mesh), C.byref(n)))
+        out = np.zeros(n.value, VERTEX_DTYPE)
+        self._ck(self.L.b200pt_get_mesh_vertices(self.h, int(mesh), _p(out), n.value)); return out
+
+    def update_mesh_vertices(self, updates, rebuild=False):
+        """updates: {mesh index: vertices}, each the mesh's whole vertex array, as a VERTEX_DTYPE array, an (n, 8) float32 array
+        (pos, nrm, uv) or a contiguous (n, 8) float32 CUDA tensor on this handle's device.  One call takes host arrays or tensors, not both.
+        rebuild: as update_instance_transforms.  Tensors are read on the handle's stream after torch's current stream is synchronised."""
+        mode = self._rebuild_mode(rebuild)
+        items = list(dict(updates).items())
+        if not items: raise ValueError("no mesh update")
+        on_dev = [hasattr(v, "data_ptr") for _, v in items]
+        if any(on_dev) and not all(on_dev): raise ValueError("one call takes host arrays or CUDA tensors, not both")
+        ups = (MeshUpdate * len(items))(); keep = []
+        for k, (m, v) in enumerate(items):
+            if on_dev[k]:
+                import torch
+                if (not v.is_cuda or v.device.index != self.device or v.dtype != torch.float32 or v.dim() != 2 or v.shape[1] != 8
+                        or not v.is_contiguous()):
+                    raise ValueError(f"mesh {m}: a CUDA tensor must be contiguous (n, 8) float32 on device {self.device}")
+                ptr, n = v.data_ptr(), v.shape[0]
+            else:
+                v = np.asarray(v)
+                if v.dtype.names is not None:
+                    if v.dtype != VERTEX_DTYPE: raise ValueError(f"mesh {m}: structured vertices must have dtype {VERTEX_DTYPE}")
+                    v = np.ascontiguousarray(v)
+                else:
+                    if v.ndim != 2 or v.shape[1] != 8: raise ValueError(f"mesh {m}: vertices must be (n, 8) float32 (pos, nrm, uv)")
+                    v = np.ascontiguousarray(v, np.float32)
+                keep.append(v); ptr, n = v.ctypes.data, len(v)
+            ups[k] = MeshUpdate(int(m), n, ptr)
+        if any(on_dev):
+            import torch
+            torch.cuda.current_stream(self.device).synchronize()
+        self._ck(self.L.b200pt_update_mesh_vertices(self.h, C.addressof(ups), len(items), 1 if any(on_dev) else 0, mode))
 
     def bvh2_ploc_build_query(self, ref_boxes):
         """b200pt_bvh2_ploc_build_query: the GPU builder and the GPU BVH4 collapse on reference boxes [n, 6] in the given order.

@@ -125,6 +125,31 @@ int32_t b200pt_update_instance_transforms(b200pt_handle h, const float *xf, uint
     if (!xf) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { e.update_instance_transforms(xf, count, rebuild); });
 }
+static const HostMesh &mesh_of(Engine &e, uint32_t mesh) {
+    if (!e.has_scene()) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (mesh >= e.scene().meshes.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "mesh index out of range" };
+    return e.scene().meshes[mesh];
+}
+int32_t b200pt_mesh_count(b200pt_handle h, uint32_t *out) {
+    if (!out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { if (!e.has_scene()) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" }; *out = (uint32_t)e.scene().meshes.size(); });
+}
+int32_t b200pt_mesh_vertex_count(b200pt_handle h, uint32_t mesh, uint32_t *out) {
+    if (!out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { *out = (uint32_t)mesh_of(e, mesh).vertices.size(); });
+}
+int32_t b200pt_get_mesh_vertices(b200pt_handle h, uint32_t mesh, b200pt_vertex *out, uint32_t count) {
+    if (!out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) {
+        const HostMesh &m = mesh_of(e, mesh);
+        if (count != m.vertices.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex count differs from the mesh's" };
+        if (count) memcpy(out, m.vertices.data(), (size_t)count * sizeof(b200pt_vertex));
+    });
+}
+int32_t b200pt_update_mesh_vertices(b200pt_handle h, const b200pt_mesh_update *updates, uint32_t n_updates, int32_t vertices_are_device, int32_t rebuild) {
+    if (!updates || n_updates == 0) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.update_mesh_vertices(updates, n_updates, vertices_are_device != 0, rebuild); });
+}
 int32_t b200pt_set_camera(b200pt_handle h, const float vi[16], const float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_camera(vi, pi); }); }
 int32_t b200pt_get_camera(b200pt_handle h, float vi[16], float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.get_camera(vi, pi); }); }
 int32_t b200pt_camera_from_view(const float view[16], float aspect, float vi[16], float pi[16]) {

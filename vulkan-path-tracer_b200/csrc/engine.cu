@@ -53,6 +53,7 @@ Engine::~Engine() {
     free_scene(); free_wave(); free_post(); free_adaptive(); free_denoise(); dfree(d_dn_img_);
     if (h_active_count_) cudaFreeHost(h_active_count_);
     if (h_small_) cudaFreeHost(h_small_);
+    dfree(d_scratch_);
     dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_); for (auto &l : d_luts_) dfree(l);
     dfree(d_image_); dfree(d_ctr_); dfree(d_volumes_); dfree(d_grids_); grids_.clear(); dfree(d_tri_class_);
     for (int c = 0; c < 2; c++) {
@@ -66,6 +67,16 @@ Engine::~Engine() {
     if (ev_[0]) cudaEventDestroy(ev_[0]); if (ev_[1]) cudaEventDestroy(ev_[1]);
     for (auto &e : prof_ev_) cudaEventDestroy(e);
     if (own_stream_) cudaStreamDestroy(own_stream_);
+}
+
+// Device scratch of the engine, grown on demand and kept: the per-frame updates allocate (and free, which synchronises the device) nothing.
+// Only valid until the next call; the caller has synchronised the work that used the previous contents.
+void *Engine::scratch(size_t bytes) {
+    if (bytes > scratch_bytes_) {
+        dfree(d_scratch_); scratch_bytes_ = 0;
+        CK(cudaMalloc(&d_scratch_, bytes)); scratch_bytes_ = bytes;
+    }
+    return d_scratch_;
 }
 
 void Engine::sync_all() {
@@ -236,6 +247,99 @@ void Engine::update_instance_transforms(const float *xf, uint32_t count, int reb
         LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
         try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
         catch (...) { lbvh_free(&fresh); apply(old); throw; }
+        lbvh_free(&bvh_); lbvh_refit_free(&refit_);
+        bvh_ = fresh; ds_ = ds; lc_ = lc;
+    }
+    reset();
+}
+
+// Mesh vertex update (no reference equivalent): the whole vertex array of each listed mesh replaced in d_verts_ and in the host mirror
+// scene_.meshes (rebuild_emissive, set_material, the instance update and get_mesh_vertices read it), the emissive records rebuilt from the
+// mirror, then the tree refit in place with the shading records of the changed meshes' instances rewritten (rebuild == 0), or built anew as
+// update_instance_transforms builds it; then ResetPathTracing.  What stays and how a failure is undone: as update_instance_transforms.
+// Every argument is checked before anything changes; device input is staged in one buffer and checked there first.
+void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool device, int rebuild) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!u || n == 0) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no mesh update" };
+    std::vector<uint8_t> listed(scene_.meshes.size(), 0);
+    size_t total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (u[i].mesh >= scene_.meshes.size() || listed[u[i].mesh]) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "mesh index out of range or repeated" };
+        listed[u[i].mesh] = 1;
+        if (!u[i].vertices) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "null vertex pointer" };
+        if (u[i].vertex_count != scene_.meshes[u[i].mesh].vertices.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex count differs from the mesh's" };
+        total += u[i].vertex_count;
+    }
+    constexpr size_t VB = sizeof(b200pt_vertex), VF = VB / sizeof(float);
+    if (!device)
+        for (uint32_t i = 0; i < n; i++) {
+            const float *f = reinterpret_cast<const float *>(u[i].vertices);
+            for (size_t k = 0; k < (size_t)u[i].vertex_count * VF; k++) if (!std::isfinite(f[k])) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex component is not finite" };
+        }
+    sync_all();                                                 // the waves in flight neither read half-updated records nor resolve into the new accumulation
+    b200pt_vertex *stage = nullptr;                             // device input: [update 0 | update 1 | ... | flag word]
+    if (device) {
+        stage = static_cast<b200pt_vertex *>(scratch(total * VB + 16));
+        size_t o = 0;
+        for (uint32_t i = 0; i < n; o += u[i].vertex_count, i++)
+            if (u[i].vertex_count) CK(cudaMemcpyAsync(stage + o, u[i].vertices, u[i].vertex_count * VB, cudaMemcpyDeviceToDevice, stream_));
+        bool bad = false;
+        const int r = any_nonfinite(reinterpret_cast<const float *>(stage), total * VF, reinterpret_cast<uint32_t *>(stage + total), h_small_, stream_, &bad);
+        if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("any_nonfinite failed: ") + cudaGetErrorString((cudaError_t)r) };
+        if (bad) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex component is not finite" };
+    }
+    std::vector<std::vector<b200pt_vertex>> old(n);
+    for (uint32_t i = 0; i < n; i++) old[i] = scene_.meshes[u[i].mesh].vertices;
+    auto restore = [&]() {
+        for (uint32_t i = 0; i < n; i++) {
+            std::vector<b200pt_vertex> &mv = scene_.meshes[u[i].mesh].vertices;
+            mv = old[i];
+            if (!mv.empty()) CK(cudaMemcpyAsync(d_verts_ + h_meshes_[u[i].mesh].vbase, mv.data(), mv.size() * VB, cudaMemcpyHostToDevice, stream_));
+        }
+        CK(cudaStreamSynchronize(stream_));
+        rebuild_emissive();
+    };
+    try {
+        size_t o = 0;
+        for (uint32_t i = 0; i < n; o += u[i].vertex_count, i++) {
+            std::vector<b200pt_vertex> &mv = scene_.meshes[u[i].mesh].vertices;
+            b200pt_vertex *dst = d_verts_ + h_meshes_[u[i].mesh].vbase;
+            const size_t bytes = mv.size() * VB;
+            if (!bytes) continue;
+            if (device) {
+                CK(cudaMemcpyAsync(dst, stage + o, bytes, cudaMemcpyDeviceToDevice, stream_));
+                CK(cudaMemcpyAsync(mv.data(), stage + o, bytes, cudaMemcpyDeviceToHost, stream_));   // the mirror: the updated ranges only
+            } else {
+                memcpy(mv.data(), u[i].vertices, bytes);
+                CK(cudaMemcpyAsync(dst, mv.data(), bytes, cudaMemcpyHostToDevice, stream_));
+            }
+        }
+        CK(cudaStreamSynchronize(stream_));
+        rebuild_emissive();                                     // the world-space EmTri, from the mirror
+    } catch (...) {
+        try { restore(); } catch (...) { has_scene_ = false; }
+        throw;
+    }
+    if (!rebuild) {
+        std::vector<uint32_t> changed;                          // instances of the updated meshes: their shading records are rewritten
+        for (size_t a = 0; a < h_instances_.size(); a++) if (listed[h_instances_[a].mesh]) changed.push_back((uint32_t)a);
+        uint32_t *const d_list = static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
+        auto refit = [&]() {
+            int r = lbvh_refit(&bvh_, &refit_, d_verts_, d_indices_, d_meshes_, d_instances_, (uint32_t)h_instances_.size(), stream_);
+            if (r == 0) r = lbvh_refresh_shade(&bvh_, d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), changed.data(),
+                                               (uint32_t)changed.size(), d_list, stream_);
+            return r;
+        };
+        const int r = refit();
+        if (r != 0) {                                           // back to the previous vertices, and the tree refit to them
+            try { restore(); if (refit() != 0) has_scene_ = false; } catch (...) { has_scene_ = false; }
+            throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refit failed: ") + cudaGetErrorString((cudaError_t)r) };
+        }
+    } else {
+        LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
+        try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
+        catch (...) { lbvh_free(&fresh); try { restore(); } catch (...) { has_scene_ = false; } throw; }
         lbvh_free(&bvh_); lbvh_refit_free(&refit_);
         bvh_ = fresh; ds_ = ds; lc_ = lc;
     }

@@ -23,6 +23,8 @@ public:
     // TLAS::Update: count x 16 floats (b200pt_instance::Transform); rebuild: 0 refits in place, B200PT_REBUILD_GPU builds on the device (PLOC),
     // any other value builds the tree set_scene would build
     void update_instance_transforms(const float *transforms, uint32_t count, int rebuild);
+    // the whole vertex array of each listed mesh (host or device memory), one refit / rebuild for the batch; rebuild as above
+    void update_mesh_vertices(const b200pt_mesh_update *updates, uint32_t n, bool device, int rebuild);
     // PathTracer::AddVolume / SetVolume / RemoveVolume / SetPhaseFunction / AddDensityDataToVolume / RemoveDensityDataFromVolume (volumes.cuh)
     uint32_t add_volume(const b200pt_volume &v);
     void set_volume(uint32_t idx, const b200pt_volume &v);
@@ -151,6 +153,8 @@ private:
     LbvhResult bvh_{};
     LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
     uint32_t *h_small_ = nullptr;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
+    void *d_scratch_ = nullptr; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices
+    void *scratch(size_t bytes);
     LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
     uint8_t *d_tri_class_ = nullptr; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c

@@ -179,6 +179,13 @@ struct LbvhRefit { uint32_t *slot_jk = nullptr; float *slot_box = nullptr, *node
 int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
                uint32_t n_instances, cudaStream_t st);
 void lbvh_refit_free(LbvhRefit *s);
+// After the vertices of some meshes changed (d_verts holds them) and lbvh_refit ran: r->shade of every triangle of instances insts[0, m) is
+// rewritten as lbvh_build writes it.  Both rebuilds recompute r->shade themselves.  d_list: device scratch of at least 2 m + 1 words.
+// Returns cudaError_t as int.
+int lbvh_refresh_shade(LbvhResult *r, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+                       const DevInstance *h_instances, const DevMesh *h_meshes, const uint32_t *insts, uint32_t m, uint32_t *d_list, cudaStream_t st);
+// *any = some float of d_v[0, n) is not finite.  d_flag: one device word of scratch; h_small: pinned host word for the readback.  Returns cudaError_t as int.
+int any_nonfinite(const float *d_v, size_t n, uint32_t *d_flag, uint32_t *h_small, cudaStream_t st, bool *any);
 
 // ---- post chain (post_kernels.cu) ----
 struct PostParams { float Exposure, Gamma, BloomThreshold, BloomStrength, FalloffRange; };

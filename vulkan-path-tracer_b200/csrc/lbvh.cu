@@ -74,6 +74,19 @@ __device__ __forceinline__ BvhTri world_tri(const DevInstance &in, uint32_t a, u
     bb[2] = fminf(v0.z, fminf(v1.z, v2.z)); bb[5] = fmaxf(v0.z, fmaxf(v1.z, v2.z));
     return t;
 }
+// The shading record of triangle prim of instance a: object-space positions, normals and UVs (a transform never changes it, a vertex update
+// does).  k_world_tris and the vertex-update refresh (k_refresh_shade) both call this.
+__device__ __forceinline__ ShadeTri shade_tri(uint32_t a, uint32_t prim, uint32_t material, const b200pt_vertex &A, const b200pt_vertex &B, const b200pt_vertex &C) {
+    ShadeTri sh;
+    sh.r[0] = make_float4(A.Position[0], A.Position[1], A.Position[2], __uint_as_float(a));
+    sh.r[1] = make_float4(B.Position[0], B.Position[1], B.Position[2], __uint_as_float(prim));
+    sh.r[2] = make_float4(C.Position[0], C.Position[1], C.Position[2], __uint_as_float(material));
+    sh.r[3] = make_float4(A.Normal[0], A.Normal[1], A.Normal[2], A.TexCoord[0]);
+    sh.r[4] = make_float4(B.Normal[0], B.Normal[1], B.Normal[2], A.TexCoord[1]);
+    sh.r[5] = make_float4(C.Normal[0], C.Normal[1], C.Normal[2], B.TexCoord[0]);
+    sh.r[6] = make_float4(B.TexCoord[1], C.TexCoord[0], C.TexCoord[1], 0.0f);
+    return sh;
+}
 __device__ __forceinline__ void reduce_bounds(float lo[3], float hi[3], float *bounds) {   // warp-reduce, then one atomic per warp (whole warps call it)
     for (int k = 0; k < 3; k++) {
         for (int o = 16; o > 0; o >>= 1) { lo[k] = fminf(lo[k], __shfl_down_sync(0xFFFFFFFFu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_down_sync(0xFFFFFFFFu, hi[k], o)); }
@@ -94,15 +107,7 @@ __global__ void k_world_tris(const b200pt_vertex *__restrict__ verts, const uint
         const b200pt_vertex &A = verts[m.vbase + ix[0]], &B = verts[m.vbase + ix[1]], &C = verts[m.vbase + ix[2]];
         float bb[6];
         tmp[gid] = world_tri(in, a, gid, prim, A, B, C, bb);
-        ShadeTri sh;
-        sh.r[0] = make_float4(A.Position[0], A.Position[1], A.Position[2], __uint_as_float(a));
-        sh.r[1] = make_float4(B.Position[0], B.Position[1], B.Position[2], __uint_as_float(prim));
-        sh.r[2] = make_float4(C.Position[0], C.Position[1], C.Position[2], __uint_as_float(in.material));
-        sh.r[3] = make_float4(A.Normal[0], A.Normal[1], A.Normal[2], A.TexCoord[0]);
-        sh.r[4] = make_float4(B.Normal[0], B.Normal[1], B.Normal[2], A.TexCoord[1]);
-        sh.r[5] = make_float4(C.Normal[0], C.Normal[1], C.Normal[2], B.TexCoord[0]);
-        sh.r[6] = make_float4(B.TexCoord[1], C.TexCoord[0], C.TexCoord[1], 0.0f);
-        shade[gid] = sh;
+        shade[gid] = shade_tri(a, prim, in.material, A, B, C);
         for (int k = 0; k < 3; k++) { lo[k] = bb[k]; hi[k] = bb[3 + k]; }
         for (int k = 0; k < 6; k++) cent[(size_t)gid * 6 + k] = bb[k];  // per-triangle AABB (unsorted)
     }
@@ -430,6 +435,29 @@ __global__ void k_refit_wide(const int32_t *__restrict__ src, uint32_t n4, const
     const float *lo = (s & 1) ? N.lo1 : N.lo0, *hi = (s & 1) ? N.hi1 : N.hi0;
     Bvh4Node &o = nodes4[i >> 2]; const uint32_t k = i & 3u;
     o.lox[k] = lo[0]; o.loy[k] = lo[1]; o.loz[k] = lo[2]; o.hix[k] = hi[0]; o.hiy[k] = hi[1]; o.hiz[k] = hi[2];
+}
+
+// ---- 9. after the mesh vertices changed (Engine::update_mesh_vertices without rebuild) ------------------------------------------------------
+// The refit above recomputes the slot records; the shading records (gid order) of the instances of the changed meshes are rewritten here with
+// shade_tri, as k_world_tris writes them.  list = [instance ids (m) | prefix of their triangle counts (m + 1)]: one thread per triangle.
+__global__ void k_refresh_shade(const b200pt_vertex *__restrict__ verts, const uint32_t *__restrict__ indices, const DevMesh *__restrict__ meshes,
+                                const DevInstance *__restrict__ inst, const uint32_t *__restrict__ list, uint32_t m, ShadeTri *__restrict__ shade) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t *off = list + m;
+    if (t >= off[m]) return;
+    uint32_t lo = 0, hi = m - 1;                                         // last range with off <= t
+    while (lo < hi) { const uint32_t mid = (lo + hi + 1) >> 1; if (off[mid] <= t) lo = mid; else hi = mid - 1; }
+    const uint32_t a = list[lo], prim = t - off[lo];
+    const DevInstance &in = inst[a];
+    const DevMesh msh = meshes[in.mesh];
+    const uint32_t *ix = indices + msh.ibase + (size_t)prim * 3;
+    shade[in.tri_base + prim] = shade_tri(a, prim, in.material, verts[msh.vbase + ix[0]], verts[msh.vbase + ix[1]], verts[msh.vbase + ix[2]]);
+}
+// *flag = 1 when any of v[0, n) is not finite (the caller zeroes it first).
+__global__ void k_flag_nonfinite(const float *__restrict__ v, size_t n, uint32_t *__restrict__ flag) {
+    bool bad = false;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) bad |= !isfinite(v[i]);
+    if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) *flag = 1u;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1077,6 +1105,32 @@ int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const 
     if (s->n4) k_refit_wide<<<(s->n4 * 4 + 255) / 256, 256, 0, st>>>(s->src4, s->n4, r->nodes, r->nodes4);
     LBVH_CHECK(cudaGetLastError());
     LBVH_CHECK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int lbvh_refresh_shade(LbvhResult *r, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+                       const DevInstance *h_instances, const DevMesh *h_meshes, const uint32_t *insts, uint32_t m, uint32_t *d_list, cudaStream_t st) {
+    if (!r->shade) return (int)cudaErrorInvalidValue;
+    if (m == 0) return 0;
+    std::vector<uint32_t> list(insts, insts + m);
+    uint64_t total = 0;
+    list.push_back(0u);
+    for (uint32_t i = 0; i < m; i++) { total += h_meshes[h_instances[insts[i]].mesh].tri_count; if (total > 0xFFFFFFFFull) return (int)cudaErrorInvalidValue; list.push_back((uint32_t)total); }
+    if (total == 0) return 0;
+    LBVH_CHECK(cudaMemcpyAsync(d_list, list.data(), list.size() * 4, cudaMemcpyHostToDevice, st));
+    k_refresh_shade<<<(uint32_t)((total + 255) / 256), 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, d_list, m, r->shade);
+    LBVH_CHECK(cudaGetLastError());
+    LBVH_CHECK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int any_nonfinite(const float *d_v, size_t n, uint32_t *d_flag, uint32_t *h_small, cudaStream_t st, bool *any) {
+    LBVH_CHECK(cudaMemsetAsync(d_flag, 0, 4, st));
+    if (n) k_flag_nonfinite<<<(uint32_t)std::min<size_t>((n + 255) / 256, 1024), 256, 0, st>>>(d_v, n, d_flag);
+    LBVH_CHECK(cudaGetLastError());
+    LBVH_CHECK(cudaMemcpyAsync(h_small, d_flag, 4, cudaMemcpyDeviceToHost, st));
+    LBVH_CHECK(cudaStreamSynchronize(st));
+    *any = h_small[0] != 0u;
     return 0;
 }
 
