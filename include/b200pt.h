@@ -429,9 +429,21 @@ int32_t b200pt_trace_query(b200pt_handle h, int32_t shape, int32_t kind, int32_t
 #define B200PT_SQ_USER_EVAL  82
 #define B200PT_SQ_RNG        86   /* sampler state after the step */
 #define B200PT_SQ_CLASS      87   /* material class whose instantiation ran */
-#define B200PT_SQ_STRIDE     88
+#define B200PT_SQ_POS        88   /* shading position (world) */
+#define B200PT_SQ_SKY_W      91   /* sky draw direction (world) */
+#define B200PT_SQ_LIGHT_W    94   /* light draw direction (world) */
+#define B200PT_SQ_STRIDE     97
 int32_t b200pt_shade_query(b200pt_handle h, int32_t force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv2,
                            const float *dir3, const float *org3, const float *pay_pdf, const uint32_t *rng, const float *L3, float *out);
+/* Miss shading test hook: what the renderer's miss kernel (k_shade_miss, SH/Miss.slang:8-76) gives a path whose segment missed, for n
+ * caller-given world directions dir3, path depths depth[i] and BSDF pdfs pay_pdf[i] of the missed segment, under the current config:
+ * the environment seen along the direction (inverse sky rotation, lat-long lookup) times the intensity, or the furnace's 1, MIS-weighted
+ * at depth > 0 against the sky sampler's pdf.  out: n records of B200PT_MQ_STRIDE floats.  B200PT_ERR_NO_SCENE without a scene or an
+ * environment map. */
+#define B200PT_MQ_RGB        0    /* emitted radiance */
+#define B200PT_MQ_PDF        3    /* sky sampler pdf of the direction (alpha of the lookup; 1 where no lookup is made) */
+#define B200PT_MQ_STRIDE     4
+int32_t b200pt_miss_query(b200pt_handle h, uint32_t n, const float *dir3, const uint32_t *depth, const float *pay_pdf, float *out);
 
 /* Energy-compensation lookup-table baker (SURVEY.md 8f row 2).
  * Replaces LookupTableCalculator::CalculateTable(tableSize, sampleCount) (PathTracer/LookupTableCalculator.h:8,

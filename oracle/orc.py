@@ -142,6 +142,8 @@ def lib():
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.orc_shade_query.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32] + [C.c_void_p] * 9
         L.orc_shade_query.restype = None
+        L.orc_miss_query.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32] + [C.c_void_p] * 4
+        L.orc_miss_query.restype = None
         L.orc_render.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.POINTER(OrcCounters)]
         L.orc_sample_pixel.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -346,7 +348,7 @@ class Scene:
         lib().orc_trace_closest(self.h, n, _p(org), _p(dirs), C.c_float(tmin), C.c_float(tmax), int(use_bvh), _p(t), _p(prim), _p(inst), _p(uv))
         return t, prim, inst, uv
 
-    def shade_query(self, cfg, inst, prim, uv, dirs, org, pay_pdf, rng, L=None, stride=88):
+    def shade_query(self, cfg, inst, prim, uv, dirs, org, pay_pdf, rng, L=None, stride=97):
         """orc_shade_query: [n, stride] float32 records laid out like B200PT_SQ_* (include/b200pt.h)"""
         inst = np.ascontiguousarray(inst, np.uint32).reshape(-1); n = len(inst)
         b = lambda a, dt, sh: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dt), sh))
@@ -355,6 +357,15 @@ class Scene:
         Lw = None if L is None else b(L, np.float32, (n, 3))
         out = np.zeros((n, stride), np.float32)
         lib().orc_shade_query(self.h, C.byref(cfg), n, _p(inst), _p(prim), _p(uv), _p(dirs), _p(org), _p(pay_pdf), _p(rng), None if Lw is None else _p(Lw), _p(out))
+        return out
+
+    def miss_query(self, cfg, dirs, depth, pay_pdf):
+        """orc_miss_query: [n, 4] float32 records laid out like B200PT_MQ_* (emitted RGB, env pdf)"""
+        dirs = np.ascontiguousarray(dirs, np.float32).reshape(-1, 3); n = len(dirs)
+        depth = np.ascontiguousarray(np.broadcast_to(np.asarray(depth, np.uint32), (n,)))
+        pay_pdf = np.ascontiguousarray(np.broadcast_to(np.asarray(pay_pdf, np.float32), (n,)))
+        out = np.zeros((n, 4), np.float32)
+        lib().orc_miss_query(self.h, C.byref(cfg), n, _p(dirs), _p(depth), _p(pay_pdf), _p(out))
         return out
 
     def render(self, cfg, W, H, nframes, base_seed, frame0=0, image=None, rank=0, world=1, band_rows=1, nthreads=0):

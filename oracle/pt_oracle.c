@@ -1592,12 +1592,13 @@ void orc_shade_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const
         lobe_probs(&m, &pm, &pd, &pg);
         o[ORC_SQ_AX] = m.Ax; o[ORC_SQ_AY] = m.Ay; o[ORC_SQ_ETA] = m.Eta; o[ORC_SQ_PM] = pm; o[ORC_SQ_PD] = pd; o[ORC_SQ_PG] = pg;
         put3(o + ORC_SQ_BASECOLOR, m.BaseColor); o[ORC_SQ_ROUGHNESS] = m.Roughness;
+        put3(o + ORC_SQ_POS, sf.WorldPos);
         put3(o + ORC_SQ_EMITTED, hit_emission(sc, cfg, inst[i], &sf, &m, isLight, 1u, V3(org3[3 * i], org3[3 * i + 1], org3[3 * i + 2]), pay_pdf[i]));
         const v3 V = surf_world_to_tangent(&sf, v3normalize(v3neg(rayDir)));
         if (cfg->EnableSkyMIS) {                                                /* :125-147 */
             v3 w; v4 lv;
             const v3 t = hit_sky_draw(sc, cfg, &sf, &r, &w, &lv);
-            put3(o + ORC_SQ_SKY_L, t); put3(o + ORC_SQ_SKY_LV, V3(lv.x, lv.y, lv.z)); o[ORC_SQ_SKY_LV + 3] = lv.w;
+            put3(o + ORC_SQ_SKY_L, t); put3(o + ORC_SQ_SKY_W, w); put3(o + ORC_SQ_SKY_LV, V3(lv.x, lv.y, lv.z)); o[ORC_SQ_SKY_LV + 3] = lv.w;
             if (lv.w > 0.0f) {
                 const Eval e = eval_bsdf(&m, sc, cfg, V, t);
                 put_eval(o + ORC_SQ_SKY_EVAL, e);
@@ -1608,6 +1609,7 @@ void orc_shade_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const
         if (cfg->EnableMeshMIS && !isLight) {                                   /* :154-184 */
             v3 w; v4 lv; uint32_t lt, li;
             sample_emissive(sc, &r, sf.WorldPos, &w, &lv, &lt, &li);
+            put3(o + ORC_SQ_LIGHT_W, w);
             o[ORC_SQ_LIGHT_LV] = lv.x; o[ORC_SQ_LIGHT_LV + 1] = lv.y; o[ORC_SQ_LIGHT_LV + 2] = lv.z; o[ORC_SQ_LIGHT_LV + 3] = lv.w;
             if (li != 0xFFFFFFFFu) put_bits(o + ORC_SQ_LIGHT_GID, sc->xf[li].tri_base + lt);
             if (lv.w > 0.0f) {
@@ -1637,21 +1639,37 @@ void orc_shade_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const
     }
 }
 
-/* Miss: SH/Miss.slang:8-76 */
-static void miss_shader(const OrcScene *sc, const OrcConfig *cfg, Payload *pl) {
-    if (cfg->EnableAtmosphere) { pl->Depth = ORC_MAX_DEPTH; return; }           /* :11-14: the sky is the in-scattered sun light, a miss emits nothing */
+/* Miss: SH/Miss.slang:8-76.  miss_emission is what miss_shader and orc_miss_query share: the emitted radiance of a miss along dir at Depth
+ * `depth` with BSDF pdf `pdf`, and in .w the sky sampler's pdf of the lookup (1 where none is made). */
+static v4 miss_emission(const OrcScene *sc, const OrcConfig *cfg, v3 dir, uint32_t depth, float pdf) {
     v4 c;
-    if (cfg->ShowEnvMapDirectly || pl->Depth > 0) {
+    if (cfg->EnableAtmosphere) { v4 z = { 0, 0, 0, 1 }; return z; }            /* :11-14: the sky is the in-scattered sun light, a miss emits nothing */
+    if (cfg->ShowEnvMapDirectly || depth > 0) {
         float az = cfg->SkyRotationAzimuth / 180.0f * ORC_PI, al = cfg->SkyRotationAltitude / 180.0f * ORC_PI;
-        v3 r = orc_rotate(pl->Direction, V3(1, 0, 0), -al);
+        v3 r = orc_rotate(dir, V3(1, 0, 0), -al);
         r = orc_rotate(r, V3(0, 1, 0), -az);
         float u, v; direction_to_uv(r, &u, &v);
         c = env_sample(sc, u, v);
     } else { v4 z = { 0, 0, 0, 1 }; c = z; }
-    pl->Emitted = V3(c.x * cfg->EnvironmentIntensity, c.y * cfg->EnvironmentIntensity, c.z * cfg->EnvironmentIntensity);
-    if (cfg->FurnaceTestMode) pl->Emitted = v3s(1.0f);
-    if (cfg->EnableSkyMIS && pl->Depth > 0) pl->Emitted = v3scale(pl->Emitted, power_heuristic(pl->PDF, c.w));
+    v3 e = V3(c.x * cfg->EnvironmentIntensity, c.y * cfg->EnvironmentIntensity, c.z * cfg->EnvironmentIntensity);
+    if (cfg->FurnaceTestMode) e = v3s(1.0f);
+    if (cfg->EnableSkyMIS && depth > 0) e = v3scale(e, power_heuristic(pdf, c.w));
+    v4 r = { e.x, e.y, e.z, c.w };
+    return r;
+}
+static void miss_shader(const OrcScene *sc, const OrcConfig *cfg, Payload *pl) {
+    if (!cfg->EnableAtmosphere) {
+        const v4 e = miss_emission(sc, cfg, pl->Direction, pl->Depth, pl->PDF);
+        pl->Emitted = V3(e.x, e.y, e.z);
+    }
     pl->Depth = ORC_MAX_DEPTH;
+}
+void orc_miss_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const float *dir3, const uint32_t *depth, const float *pay_pdf, float *out) {
+    for (uint32_t i = 0; i < n; i++) {
+        const v4 e = miss_emission(sc, cfg, V3(dir3[3 * i], dir3[3 * i + 1], dir3[3 * i + 2]), depth[i], pay_pdf[i]);
+        float *o = out + (size_t)i * ORC_MQ_STRIDE;
+        o[ORC_MQ_RGB] = e.x; o[ORC_MQ_RGB + 1] = e.y; o[ORC_MQ_RGB + 2] = e.z; o[ORC_MQ_PDF] = e.w;
+    }
 }
 
 /* ------------------------------------------------------------------------------------------------

@@ -210,9 +210,18 @@ void orc_trace_closest(const OrcScene *s, uint32_t n, const float *org3, const f
 #define ORC_SQ_USER_EVAL  82
 #define ORC_SQ_RNG        86
 #define ORC_SQ_CLASS      87   /* GPU only: the material class whose kernel ran */
-#define ORC_SQ_STRIDE     88
+#define ORC_SQ_POS        88   /* shading position, world */
+#define ORC_SQ_SKY_W      91   /* sky draw direction, world */
+#define ORC_SQ_LIGHT_W    94   /* light draw direction, world */
+#define ORC_SQ_STRIDE     97
 void orc_shade_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv2, const float *dir3,
                      const float *org3, const float *pay_pdf, const uint32_t *rng, const float *L3, float *out);
+/* Miss shading (miss_shader, SH/Miss.slang:8-76) for n world directions dir3 at path depth depth[i] with BSDF pdf pay_pdf[i]: out holds n records
+ * of ORC_MQ_STRIDE floats laid out like B200PT_MQ_* of include/b200pt.h (emitted RGB, sky sampler pdf of the lookup). */
+#define ORC_MQ_RGB        0
+#define ORC_MQ_PDF        3
+#define ORC_MQ_STRIDE     4
+void orc_miss_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const float *dir3, const uint32_t *depth, const float *pay_pdf, float *out);
 
 /* One reference dispatch sequence: frames [frame0, frame0+nframes) with Seed_f = PCG_HASH(base_seed + f)
  * (SURVEY 8d; the reference's own seed is wall-clock, PT/PathTracer.cpp:127-140), running-mean accumulate

@@ -66,8 +66,13 @@ def _shade(name):                                                   # b200pt_sha
     t, prim, inst, uv = S.trace_closest(o, d, 1e-3, 1e5); h = t > 0
     for general in (False, True):
         r = T.shade_query(inst[h], prim[h], uv[h], d[h], o[h], 0.5, np.arange(h.sum()), L=-d[h], force_general=general)
-        assert r.shape == (h.sum(), 88)
+        assert r.shape == (h.sum(), 97)
     print(name, "shade_query ok")
+    for kw in (dict(), dict(ShowEnvMapDirectly=0), dict(EnableSkyMIS=0, FurnaceTestMode=1)):   # b200pt_miss_query: every branch of miss_emission
+        T = util.product_tracer(name, 16, 16, SkyRotationAzimuth=70.0, SkyRotationAltitude=20.0, **kw)
+        r = T.miss_query(d, np.arange(300) % 2, 0.5)
+        assert r.shape == (300, 4) and np.isfinite(r).all()
+    print(name, "miss_query ok")
 _shade("cornell_box"); _shade("cornell_box_glass")
 def _update(name, inst, env=None):                                  # instance updates: k_refit_slots / k_refit_level (/ k_refit_wide), and the rebuild path
     for k, v in (env or {}).items(): os.environ[k] = v

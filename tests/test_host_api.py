@@ -39,6 +39,12 @@ def test_null_arguments_are_rejected_not_crashed():
     assert L.b200pt_add_volume(None, None) == pt.ERR_WRONG_ARGUMENTS      # homogeneous volumes are implemented: a null volume is a bad argument
     assert L.b200pt_add_density_data_to_volume(None, 0, None) == pt.ERR_NOT_IMPLEMENTED   # .vdb files need OpenVDB; density data goes in through b200pt_add_density_grid_to_volume
     assert L.b200pt_add_density_grid_to_volume(None, 0, None) == pt.ERR_WRONG_ARGUMENTS
+    buf = np.zeros(16, np.float32); u = np.zeros(4, np.uint32)
+    assert L.b200pt_miss_query(None, 1, buf.ctypes.data, u.ctypes.data, buf.ctypes.data, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_miss_query(None, 1, None, u.ctypes.data, buf.ctypes.data, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_miss_query(None, 1, buf.ctypes.data, None, buf.ctypes.data, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_miss_query(None, 1, buf.ctypes.data, u.ctypes.data, None, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_miss_query(None, 1, buf.ctypes.data, u.ctypes.data, buf.ctypes.data, None) == pt.ERR_WRONG_ARGUMENTS
     w, h, p = C.c_uint32(), C.c_uint32(), C.c_void_p()
     assert L.b200pt_decode_image_file(b"/nonexistent.png", C.byref(w), C.byref(h), C.byref(p)) == pt.ERR_INIT_FAILED
 
@@ -115,8 +121,12 @@ def test_hdr_decoder(tmp_path):
 
 
 def test_env_alias_table_bit_exact_vs_oracle():
-    for seed, (w, h) in [(3, (64, 32)), (4, (128, 64)), (5, (33, 17))]:
-        raw = gltf_ref.synthetic_env(w, h, seed)
+    hot = np.ones((19, 37, 4), np.float32); hot[..., :3] = 0.0; hot[0, 0, :3] = (50.0, 40.0, 30.0)      # one hot texel on the seam and the pole
+    half = gltf_ref.synthetic_env(37, 19, 9); half[19 // 2:, :, :3] = 0.0
+    const = np.ones((19, 37, 4), np.float32); const[..., :3] = 0.7
+    maps = [gltf_ref.synthetic_env(w, h, seed) for seed, (w, h) in [(3, (64, 32)), (4, (128, 64)), (5, (33, 17)), (6, (37, 19)), (7, (37, 1)), (8, (1, 19))]]
+    maps += [hot, half, const, gltf_ref.synthetic_env(4096, 2048, seed=3, sun=150000.0)]   # the last: the map bench.py renders with
+    for raw in maps:
         a_env, a_alias, a_sum = orc.build_env_alias(raw)
         b_env, b_alias, b_sum = pt.build_env_alias(raw)
         assert np.array_equal(a_env, b_env) and np.array_equal(a_alias, b_alias) and np.float32(a_sum) == np.float32(b_sum)

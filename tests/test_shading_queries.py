@@ -22,8 +22,8 @@ the surface frame and material (N, T, B, V, Ax, Ay, Eta, pm, pd, pg), which are 
 undecided share must stay under UNDECIDED_MAX per group.  The LUT texels are taken as exact (they are fp32 data).  Flags (validDir, refracted, entered,
 rejected) must be equal on decided records.  test_margin_is_tight shows that K / 10 rejects some GPU answer.
 
-Sky and light NEE, their terms c and the emission term are compared GPU against oracle only (the model has no env or emissive sampler);
-there a value the oracle computes as inf / NaN must be inf / NaN on the GPU too.  The class kernels are compared with the all-lobes kernel
+Sky and light NEE, their terms c and the emission term are compared GPU against oracle here; test_nee_queries.py checks them, and miss
+shading, against a float64 model of the samplers.  A value the oracle computes as inf / NaN must be inf / NaN on the GPU too.  The class kernels are compared with the all-lobes kernel
 (a class kernel must never be finite where the all-lobes one is not), and the per-material precompute with the per-hit texel path bit for bit.
 """
 import math
@@ -42,7 +42,8 @@ REL = 2.0 ** -23
 
 SQ = dict(N=0, T=3, B=6, NG=9, INSIDE=12, AX=13, AY=14, ETA=15, PM=16, PD=17, PG=18, BASECOLOR=19, ROUGHNESS=22, V=23, H=26, EMITTED=29,
           SKY_L=32, SKY_LV=35, SKY_EVAL=39, SKY_C=43, LIGHT_L=46, LIGHT_LV=49, LIGHT_EVAL=53, LIGHT_C=57, LIGHT_GID=60, BSDF_L=61, BSDF_EVAL=64,
-          VALID=68, SCATTER=69, SAMPLE=72, REFRACTED=76, ENTERED=77, REJECTED=78, USER_L=79, USER_EVAL=82, RNG=86, CLASS=87, STRIDE=88)
+          VALID=68, SCATTER=69, SAMPLE=72, REFRACTED=76, ENTERED=77, REJECTED=78, USER_L=79, USER_EVAL=82, RNG=86, CLASS=87, POS=88, SKY_W=91,
+          LIGHT_W=94, STRIDE=97)
 
 
 # ---------------------------------------------------------------- pcg_hash and its inverse (a bijection on 32-bit words)
@@ -282,6 +283,8 @@ def model_hit(inp, cfg, luts, draws):
         user = eval_bsdf(m, c, V, Lu, ec, br)
     out = dict(N=N, T=T, B=B, AX=m["Ax"], AY=m["Ay"], ETA=m["Eta"], PM=m["pm"], PD=m["pd"], PG=m["pg"], V=Vm, H=H, BSDF_L=Lv, BSDF_EVAL=ev,
                USER_EVAL=user, VALID=float(valid), REFRACTED=float(wr), ENTERED=float(wr and not inside), REJECTED=float(rej and valid), INSIDE=float(inside))
+    out["eval"] = lambda Lt, b: eval_bsdf(m, c, V, Lt, ec, b)             # the BSDF of this hit at a tangent-space direction (NEE draws)
+    out["GN"] = gn
     return out, br
 
 
@@ -506,12 +509,16 @@ def _q(T, R, **kw):
     return T.shade_query(R["inst"], R["prim"], R["uv"], R["dir"], R["org"], R["pdf"], R["rng"], R["L"], **kw)
 
 
-def test_record_layout_matches_header():
-    """the offsets the binding and this module use are the B200PT_SQ_* of the C header"""
+def test_shade_record_layout_matches_headers():
+    """the offsets the binding and this module use are the B200PT_SQ_* of the C header and the ORC_SQ_* of the oracle, with the world-space
+    NEE fields (shading position, sky and light directions) after the class"""
     import re
     import vpt_b200
     hdr = open(f"{util.ROOT}/include/b200pt.h").read()
     assert {m.group(1): int(m.group(2)) for m in re.finditer(r"#define B200PT_SQ_(\w+)\s+(\d+)", hdr)} == SQ == vpt_b200.SQ
+    ohdr = open(f"{util.ROOT}/oracle/pt_oracle.h").read()
+    assert {m.group(1): int(m.group(2)) for m in re.finditer(r"#define ORC_SQ_(\w+)\s+(\d+)", ohdr)} == SQ
+    assert (SQ["POS"], SQ["SKY_W"], SQ["LIGHT_W"], SQ["STRIDE"]) == (SQ["CLASS"] + 1, SQ["CLASS"] + 4, SQ["CLASS"] + 7, SQ["CLASS"] + 10)
 
 
 BITS = (SQ["LIGHT_GID"], SQ["RNG"], SQ["CLASS"])                          # u32 fields of the record

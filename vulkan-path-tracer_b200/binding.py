@@ -197,6 +197,7 @@ def lib():
             "b200pt_trace_stats": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p],
             "b200pt_trace_query": [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32] + [C.c_void_p] * 12,
             "b200pt_shade_query": [C.c_void_p, C.c_int32, C.c_uint32] + [C.c_void_p] * 9,
+            "b200pt_miss_query": [C.c_void_p, C.c_uint32] + [C.c_void_p] * 4,
             "b200pt_bake_lut": [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p],
             "b200pt_bake_luts_to_dir": [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32],
             "b200pt_decode_image_file": [C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_void_p)],
@@ -242,7 +243,10 @@ class Atmosphere(C.Structure):      # b200pt_atmosphere (include/b200pt.h)
 # record offsets of b200pt_shade_query (B200PT_SQ_* in include/b200pt.h; tests/test_shading_queries.py checks that they agree)
 SQ = dict(N=0, T=3, B=6, NG=9, INSIDE=12, AX=13, AY=14, ETA=15, PM=16, PD=17, PG=18, BASECOLOR=19, ROUGHNESS=22, V=23, H=26, EMITTED=29,
           SKY_L=32, SKY_LV=35, SKY_EVAL=39, SKY_C=43, LIGHT_L=46, LIGHT_LV=49, LIGHT_EVAL=53, LIGHT_C=57, LIGHT_GID=60, BSDF_L=61, BSDF_EVAL=64,
-          VALID=68, SCATTER=69, SAMPLE=72, REFRACTED=76, ENTERED=77, REJECTED=78, USER_L=79, USER_EVAL=82, RNG=86, CLASS=87, STRIDE=88)
+          VALID=68, SCATTER=69, SAMPLE=72, REFRACTED=76, ENTERED=77, REJECTED=78, USER_L=79, USER_EVAL=82, RNG=86, CLASS=87, POS=88, SKY_W=91,
+          LIGHT_W=94, STRIDE=97)
+# record offsets of b200pt_miss_query (B200PT_MQ_*)
+MQ = dict(RGB=0, PDF=3, STRIDE=4)
 
 
 def declared_symbols():
@@ -806,6 +810,15 @@ class PathTracer:
         out = np.zeros((n, SQ["STRIDE"]), np.float32)
         self._ck(self.L.b200pt_shade_query(self.h, int(bool(force_general)), n, _p(inst), _p(prim), _p(uv), _p(dirs), _p(org), _p(pay_pdf), _p(rng),
                                            None if Lw is None else _p(Lw), _p(out)))
+        return out
+
+    def miss_query(self, dirs, depth, pay_pdf):
+        """b200pt_miss_query: the renderer's miss shading per world direction.  Returns [n, B200PT_MQ_STRIDE] float32 records (emitted RGB, env pdf)."""
+        dirs = np.ascontiguousarray(dirs, np.float32).reshape(-1, 3); n = len(dirs)
+        depth = np.ascontiguousarray(np.broadcast_to(np.asarray(depth, np.uint32), (n,)))
+        pay_pdf = np.ascontiguousarray(np.broadcast_to(np.asarray(pay_pdf, np.float32), (n,)))
+        out = np.zeros((n, MQ["STRIDE"]), np.float32)
+        self._ck(self.L.b200pt_miss_query(self.h, n, _p(dirs), _p(depth), _p(pay_pdf), _p(out)))
         return out
 
     def scene_stats(self):

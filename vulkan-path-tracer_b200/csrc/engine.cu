@@ -1228,6 +1228,34 @@ void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, c
     for (void *p : bufs) cudaFree(p);
     CK(e); CK(cudaGetLastError());
 }
+void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, const float *pay_pdf, float *out) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "miss_query: no environment map" };
+    if (!n) return;
+    std::vector<void *> bufs;
+    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
+    auto dev = [&](size_t bytes, const void *src) -> void * {
+        void *p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) fail(e);
+        bufs.push_back(p);
+        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
+        return p;
+    };
+    MissQuery q{};
+    q.n = n;
+    q.dir = (const float *)dev((size_t)n * 12, dir); q.depth = (const uint32_t *)dev((size_t)n * 4, depth); q.pay_pdf = (const float *)dev((size_t)n * 4, pay_pdf);
+    const size_t out_bytes = (size_t)n * B200PT_MQ_STRIDE * sizeof(float);
+    q.out = (float *)dev(out_bytes, nullptr);
+    const int r = launch_miss_query(ds_, make_dev_config(), q, stream_);
+    if (r != 0) fail((cudaError_t)r);
+    cudaError_t e = cudaMemcpyAsync(out, q.out, out_bytes, cudaMemcpyDeviceToHost, stream_);
+    if (e != cudaSuccess) fail(e);
+    e = cudaStreamSynchronize(stream_);
+    for (void *p : bufs) cudaFree(p);
+    CK(e); CK(cudaGetLastError());
+}
 // LookupTableCalculator::CalculateTable (PT/LookupTableCalculator.cpp:44-157) on this engine's device and stream.
 // slices == 0 picks enough dispatch slices to give every SM ~2048 resident threads.
 void Engine::bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out_host, float *elapsed_ms) {

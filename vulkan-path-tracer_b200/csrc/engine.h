@@ -99,6 +99,8 @@ public:
     // b200pt_shade_query (host arrays; see include/b200pt.h)
     void shade_query(bool force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv, const float *dir, const float *org,
                      const float *pay_pdf, const uint32_t *rng, const float *L, float *out);
+    // b200pt_miss_query (host arrays; see include/b200pt.h)
+    void miss_query(uint32_t n, const float *dir, const uint32_t *depth, const float *pay_pdf, float *out);
     void scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const;
     // b200pt_bvh2_ploc_build_query (host arrays; see include/b200pt.h): the device builder and the device collapse on the caller's boxes
     void ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes_out, uint32_t *perm_out, uint32_t *n_out, int *depth_out,

@@ -125,6 +125,10 @@ struct ShadeQuery {                           // device arrays of n hits; L may 
     uint32_t n; bool force_general; const uint32_t *gid, *rng; const float *uv, *dir, *org, *pay_pdf, *L; float *out;
 };
 int launch_shade_query(const DevScene &sc, const DevConfig &cfg, const ShadeQuery &q, cudaStream_t st);   // cudaError_t as int
+struct MissQuery {                            // device arrays of n misses; out: n x B200PT_MQ_STRIDE floats (b200pt_miss_query)
+    uint32_t n; const float *dir; const uint32_t *depth; const float *pay_pdf; float *out;
+};
+int launch_miss_query(const DevScene &sc, const DevConfig &cfg, const MissQuery &q, cudaStream_t st);     // cudaError_t as int
 
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
 struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;

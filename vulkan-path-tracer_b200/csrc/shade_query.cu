@@ -1,8 +1,9 @@
-// shade_query.cu -- shading test hook (b200pt_shade_query): caller-given hits through one shading step of k_shade_hit.
-// Every step calls the __device__ functions k_shade_hit calls (surface_init, material_init, surface_rotate_tangents, bsdf_ctx_init,
-// sample_env_begin / _finish, sample_emissive, ggx_sample_vndf, sample_bsdf_direction, eval_bsdf), with the LOBES argument of the hit
-// triangle's class kernel, in k_shade_hit's draw order.  What k_shade_hit writes inline (the emission MIS term, the NEE term c, the
-// geometry-normal rejection) is repeated here in the same operation order; the image tests compare that composition with the oracle.
+// shade_query.cu -- shading test hooks: b200pt_shade_query runs caller-given hits through one shading step of k_shade_hit, b200pt_miss_query
+// caller-given directions through k_shade_miss's miss shading.
+// Every step calls the __device__ functions the renderer's kernels call (surface_init, material_init, surface_rotate_tangents, bsdf_ctx_init,
+// sample_env_begin / _finish, sample_emissive, ggx_sample_vndf, sample_bsdf_direction, eval_bsdf, hit_emission, nee_term, miss_emission), with
+// the LOBES argument of the hit triangle's class kernel, in k_shade_hit's draw order.  Only the geometry-normal rejection, a comparison k_shade_hit
+// writes inline, is repeated here.
 #include "shading.cuh"
 #include "kernels.h"
 #include <algorithm>
@@ -44,19 +45,8 @@ __device__ __forceinline__ void shade_one(const DevScene &sc, const DevConfig &c
     o[B200PT_SQ_AX] = m.Ax; o[B200PT_SQ_AY] = m.Ay; o[B200PT_SQ_ETA] = m.Eta; o[B200PT_SQ_PM] = m.pm; o[B200PT_SQ_PD] = m.pd; o[B200PT_SQ_PG] = m.pg;
     put3(o + B200PT_SQ_BASECOLOR, m.BaseColor); o[B200PT_SQ_ROUGHNESS] = m.Roughness;
 
-    float3 e0 = f3(0.0f);                                                   // emission :265-317, Depth != 0
-    if (cfg.EnableMeshMIS) {
-        if (isLight) {
-            const float3 w1 = xf_point(in.o2w, sf.P1), w2 = xf_point(in.o2w, sf.P2), w3 = xf_point(in.o2w, sf.P3);
-            const float area = length(cross(w2 - w1, w3 - w1)) * 0.5f;
-            const float3 dl = sf.WorldPos - payOrigin;
-            const float d2 = dot(dl, dl);
-            const float cosTheta = fabsf(dot(sf.Normal, normalize(payOrigin - sf.WorldPos)));
-            float lp = (1.0f / (float)sc.n_emissive) * (1.0f / (float)in.emissive_tri_count) * (1.0f / area) * (d2 / cosTheta);
-            lp = fmaxf(lp, cfg.EmissiveMeshSamplingPDFBias);
-            e0 = e0 + m.EmissiveColor * power_heuristic(payPDF, lp);
-        }
-    } else e0 = e0 + m.EmissiveColor;
+    put3(o + B200PT_SQ_POS, sf.WorldPos);
+    const float3 e0 = hit_emission(sc, cfg, in, sf, m, isLight, 1u, payOrigin, payPDF);   // emission :265-317, Depth != 0
     put3(o + B200PT_SQ_EMITTED, e0);
 
     float3 V = normalize(-rd);
@@ -75,11 +65,12 @@ __device__ __forceinline__ void shade_one(const DevScene &sc, const DevConfig &c
                 lv.x *= cfg.EnvironmentIntensity; lv.y *= cfg.EnvironmentIntensity; lv.z *= cfg.EnvironmentIntensity;   // Q7
                 dk = sf.world_to_tangent(toW);
                 need = lv.w > 0.0f;
-                put3(o + B200PT_SQ_SKY_L, dk);
+                put3(o + B200PT_SQ_SKY_L, dk); put3(o + B200PT_SQ_SKY_W, toW);
             }
         } else if (k == 1) {
             if (cfg.EnableMeshMIS && !isLight) {
                 sample_emissive(sc, rng, sf.WorldPos, toW, lv, lgid);
+                put3(o + B200PT_SQ_LIGHT_W, toW);
                 if (lv.w > 0.0f) { dk = sf.world_to_tangent(toW); need = true; put3(o + B200PT_SQ_LIGHT_L, dk); }
             }
         } else {
@@ -91,7 +82,7 @@ __device__ __forceinline__ void shade_one(const DevScene &sc, const DevConfig &c
         if (need) e = eval_bsdf<LOBES>(m, bc, cfg, V, dk);
         if (k == 2) { evS = e; break; }
         const bool contributes = need && e.PDF > 0.0f;
-        const float3 c = contributes ? (((e.BxDF * 1.0f) * f3(lv)) / lv.w) * power_heuristic(lv.w, e.PDF) : f3(0.0f);
+        const float3 c = contributes ? nee_term(e, lv) : f3(0.0f);
         const int base = k == 0 ? B200PT_SQ_SKY_LV : B200PT_SQ_LIGHT_LV;     // LV, EVAL and C follow each other for both draws
         o[base] = lv.x; o[base + 1] = lv.y; o[base + 2] = lv.z; o[base + 3] = lv.w;
         put_eval(o + base + 4, e); put3(o + base + 8, c);
@@ -131,7 +122,23 @@ __global__ void __launch_bounds__(THREADS) k_shade_query(DevScene sc, DevConfig 
     }
 }
 
+// k_shade_miss's miss shading (miss_emission) for caller-given directions, depths and BSDF pdfs: emitted RGB and the env pdf
+__global__ void __launch_bounds__(THREADS) k_miss_query(DevScene sc, DevConfig cfg, MissQuery q) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < q.n; i += gridDim.x * blockDim.x) {
+        const float4 r = miss_emission(sc, cfg, f3(q.dir[3 * i], q.dir[3 * i + 1], q.dir[3 * i + 2]), q.depth[i], q.pay_pdf[i]);
+        float *o = q.out + (size_t)i * B200PT_MQ_STRIDE;
+        put3(o + B200PT_MQ_RGB, f3(r)); o[B200PT_MQ_PDF] = r.w;
+    }
+}
+
 } // namespace
+
+int launch_miss_query(const DevScene &sc, const DevConfig &cfg, const MissQuery &q, cudaStream_t st) {
+    if (q.n == 0) return 0;
+    const int grid = (int)std::min<uint32_t>((q.n + THREADS - 1) / THREADS, 1024u);
+    k_miss_query<<<grid, THREADS, 0, st>>>(sc, cfg, q);
+    return (int)cudaGetLastError();
+}
 
 int launch_shade_query(const DevScene &sc, const DevConfig &cfg, const ShadeQuery &q, cudaStream_t st) {
     if (q.n == 0) return 0;

@@ -565,4 +565,44 @@ __device__ __forceinline__ void sample_emissive(const DevScene &sc, Rng &rng, fl
     colorPDF.x = mat.EmissiveColor[0] * te.x; colorPDF.y = mat.EmissiveColor[1] * te.y; colorPDF.z = mat.EmissiveColor[2] * te.z;
 }
 
+// ---------------------------------------------------------------- MIS terms (k_shade_hit, k_shade_miss and the test hooks call these)
+// Emission of a hit (SH/ClosestHit.slang:265-317) at Depth `depth`, reached from payOrigin with BSDF pdf payPDF: the emissive colour,
+// MIS-weighted at Depth > 0 against the light sampler's pdf of the same point, taken with the SHADING normal and floored by the bias.
+__device__ __forceinline__ float3 hit_emission(const DevScene &sc, const DevConfig &cfg, const DevInstance &in, const Surface &sf, const Mat &m, bool isLight,
+                                               uint32_t depth, float3 payOrigin, float payPDF) {
+    float3 e0 = f3(0.0f);
+    if (cfg.EnableMeshMIS) {
+        if (depth == 0 && isLight) e0 = e0 + m.EmissiveColor;
+        else if (isLight) {
+            const float3 w1 = xf_point(in.o2w, sf.P1), w2 = xf_point(in.o2w, sf.P2), w3 = xf_point(in.o2w, sf.P3);
+            const float area = length(cross(w2 - w1, w3 - w1)) * 0.5f;
+            const float3 dl = sf.WorldPos - payOrigin;
+            const float d2 = dot(dl, dl);
+            const float cosTheta = fabsf(dot(sf.Normal, normalize(payOrigin - sf.WorldPos)));
+            float lp = (1.0f / (float)sc.n_emissive) * (1.0f / (float)in.emissive_tri_count) * (1.0f / area) * (d2 / cosTheta);
+            lp = fmaxf(lp, cfg.EmissiveMeshSamplingPDFBias);
+            e0 = e0 + m.EmissiveColor * power_heuristic(payPDF, lp);
+        }
+    } else e0 = e0 + m.EmissiveColor;
+    return e0;
+}
+// One NEE term (SH/ClosestHit.slang:341-344, :366-369): BxDF * radiance / pdf, MIS-weighted against the BSDF pdf of the same direction
+__device__ __forceinline__ float3 nee_term(const Eval &e, float4 lv) { return (((e.BxDF * 1.0f) * f3(lv)) / lv.w) * power_heuristic(lv.w, e.PDF); }
+// What a path whose segment missed receives (SH/Miss.slang:8-76): the environment seen along dir (inverse sky rotation, then the
+// lat-long lookup), times the intensity, MIS-weighted at Depth > 0 against the sky sampler's pdf (.w of the lookup, returned in .w)
+__device__ __forceinline__ float4 miss_emission(const DevScene &sc, const DevConfig &cfg, float3 dir, uint32_t depth, float payPDF) {
+    float4 c;
+    if (cfg.EnableAtmosphere) c = make_float4(0, 0, 0, 1);                  // SH/Miss.slang:11-14: with the atmosphere a miss emits nothing
+    else if (cfg.ShowEnvMapDirectly || depth > 0) {
+        float3 r = rotate3_cs(dir, f3(1, 0, 0), cfg.cosAl, -cfg.sinAl);    // Rotate(dir, X, -altitude): cos is even, sin odd
+        r = rotate3_cs(r, f3(0, 1, 0), cfg.cosAz, -cfg.sinAz);
+        float u, v; direction_to_uv(r, u, v);
+        c = env_sample(sc, u, v);
+    } else c = make_float4(0, 0, 0, 1);
+    float3 em = f3(c.x * cfg.EnvironmentIntensity, c.y * cfg.EnvironmentIntensity, c.z * cfg.EnvironmentIntensity);
+    if (cfg.FurnaceTestMode && !cfg.EnableAtmosphere) em = f3(1.0f);
+    if (cfg.EnableSkyMIS && depth > 0 && !cfg.EnableAtmosphere) em = em * power_heuristic(payPDF, c.w);
+    return make_float4(em.x, em.y, em.z, c.w);
+}
+
 } // namespace b200pt

@@ -366,17 +366,7 @@ __device__ __forceinline__ void finish_missed_path(const DevScene &sc, const Dev
                                                    uint32_t flags, float4 *__restrict__ sample_buf, uint32_t *__restrict__ rng_carry) {
     const uint32_t depth = __float_as_uint(t4.w) & DEPTH_MASK;
     const int channel = dflags_channel(__float_as_uint(t4.w));
-    float4 c;
-    if (cfg.EnableAtmosphere) c = make_float4(0, 0, 0, 1);                  // SH/Miss.slang:11-14: with the atmosphere a miss emits nothing
-    else if (cfg.ShowEnvMapDirectly || depth > 0) {
-        float3 r = rotate3_cs(dir, f3(1, 0, 0), cfg.cosAl, -cfg.sinAl);    // Rotate(dir, X, -altitude): cos is even, sin odd
-        r = rotate3_cs(r, f3(0, 1, 0), cfg.cosAz, -cfg.sinAz);
-        float u, v; direction_to_uv(r, u, v);
-        c = env_sample(sc, u, v);
-    } else c = make_float4(0, 0, 0, 1);
-    float3 em = f3(c.x * cfg.EnvironmentIntensity, c.y * cfg.EnvironmentIntensity, c.z * cfg.EnvironmentIntensity);
-    if (cfg.FurnaceTestMode && !cfg.EnableAtmosphere) em = f3(1.0f);
-    if (cfg.EnableSkyMIS && depth > 0 && !cfg.EnableAtmosphere) em = em * power_heuristic(payPDF, c.w);
+    const float3 em = f3(miss_emission(sc, cfg, dir, depth, payPDF));
     // SH/RayGen.slang:92-102 with payload.Depth == MAX_DEPTH (!= 1): the contribution is always luminance-clamped (Q3)
     float3 contribution = em * f3(t4);
     const float lum = dot(contribution, f3(0.212671f, 0.715160f, 0.072169f));
@@ -558,21 +548,7 @@ __global__ void __launch_bounds__(FUSE ? 512 : 128, FUSE ? 1 : SHADE_MIN_BLOCKS)
             }
 
             // emission :265-317 (no RNG draws: evaluated before the NEE/BSDF loop so the corner positions and the ray origin die here)
-            float3 e0 = f3(0.0f);
-            if (cfg.EnableMeshMIS) {
-                if (depth == 0 && isLight) e0 = e0 + m.EmissiveColor;
-                else if (isLight) {
-                    const float3 w1 = xf_point(in.o2w, sf.P1), w2 = xf_point(in.o2w, sf.P2), w3 = xf_point(in.o2w, sf.P3);
-                    const float area = length(cross(w2 - w1, w3 - w1)) * 0.5f;
-                    const float3 dl = sf.WorldPos - payOrigin;
-                    const float d2 = dot(dl, dl);
-                    const float cosTheta = fabsf(dot(sf.Normal, normalize(payOrigin - sf.WorldPos)));
-                    float lp = (1.0f / (float)sc.n_emissive) * (1.0f / (float)in.emissive_tri_count) * (1.0f / area) * (d2 / cosTheta);
-                    lp = fmaxf(lp, cfg.EmissiveMeshSamplingPDFBias);
-                    e0 = e0 + m.EmissiveColor * power_heuristic(payPDF, lp);
-                }
-            } else e0 = e0 + m.EmissiveColor;
-            emitted = e0;
+            emitted = hit_emission(sc, cfg, in, sf, m, isLight, depth, payOrigin, payPDF);
 
             float3 V = normalize(-rd);
             V = sf.world_to_tangent(V);
@@ -617,7 +593,7 @@ __global__ void __launch_bounds__(FUSE ? 512 : 128, FUSE ? 1 : SHADE_MIN_BLOCKS)
                 // k_connect draws the transmittance walk whenever the sun is VISIBLE (SH/ClosestHit.slang:335-349 sits outside the pdf tests)
                 const bool contributes = need && e.PDF > 0.0f;
                 if (contributes || (k == 0 && (cfg.EnableAtmosphere || (VOL && sc.n_grids)) && cfg.EnableSkyMIS)) {   // grid volumes: same reason (:332-333)
-                    const float3 c = contributes ? (((e.BxDF * 1.0f) * f3(lv)) / lv.w) * power_heuristic(lv.w, e.PDF) : f3(0.0f);
+                    const float3 c = contributes ? nee_term(e, lv) : f3(0.0f);
                     // :139, :171 -- rounded like the unfused kernel, which stores the origin (product and sum apart, whatever the kernel around it)
                     const float3 ro = add_rn(sf.WorldPos, (k == 0) ? mul_rn(sf.Normal, f3(1e-5f)) : mul_rn(toW, f3(1e-2f)));
                     if (FUSE) {
@@ -681,7 +657,7 @@ __global__ void __launch_bounds__(FUSE ? 512 : 128, FUSE ? 1 : SHADE_MIN_BLOCKS)
                 ps.org_pdf[i] = make_float4(no.x, no.y, no.z, ss.PDF);
                 ps.dir_rng[i] = make_float4(scatterW.x, scatterW.y, scatterW.z, __uint_as_float(rng.s));
                 so.bxdf_pdf[i] = make_float4(ss.BxDF.x, ss.BxDF.y, ss.BxDF.z, ss.PDF);
-                so.e0[i] = make_float4(e0.x, e0.y, e0.z, __uint_as_float(newDepth | chanBits | (reqMask << 29) | (newInMedium ? 0x80000000u : 0u)));   // bits 29/30: stored shadow requests
+                so.e0[i] = make_float4(emitted.x, emitted.y, emitted.z, __uint_as_float(newDepth | chanBits | (reqMask << 29) | (newInMedium ? 0x80000000u : 0u)));   // bits 29/30: stored shadow requests
             }
         } while (false);
 
