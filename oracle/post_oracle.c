@@ -113,7 +113,7 @@ void orc_post_process(const float *hdr, uint32_t W, uint32_t H, const OrcPostCon
                 float bl = top + ay * (bot - top);
                 float cc = h4[k] + bl;
                 cc = cc * c->Exposure;
-                col[k] = powf(cc, invGamma);
+                col[k] = cc > 0.0f ? powf(cc, invGamma) : (cc == 0.0f ? 0.0f : NAN);   /* Q18: exp2(y log2 x): pow(0, y) = 0, pow(x < 0, y) = NaN */
             }
             float outc[3];
             orc_aces_fitted(col, outc);

@@ -96,4 +96,12 @@ def _deform(name, mesh):                                            # mesh verte
     assert np.isfinite(T.get_hdr()).all()
     print(name, "mesh updates ok")
 _deform("cornell_box_glass", 6)
+def _post_block():                                                  # fresh handle, unaligned row block, 2-level chain: k_bloom_down_first + k_bloom_final on rows
+    import vpt_b200 as pt
+    T = pt.PathTracer(0); T.set_scene(util.scene_dict("cornell_box")); T.resize(65, 37)
+    T.set_bloom(2.0, 1.0, 2, 5.0)
+    rng = np.random.default_rng(4); hdr = np.ones((37, 65, 4), np.float32); hdr[..., :3] = rng.random((37, 65, 3)) * 5
+    T.set_hdr(hdr); T.post_process_rows(9, 20); T.get_ldr_rows(9, 20)
+    print("post row block ok")
+_post_block()
 print("sanitize_small done")

@@ -249,7 +249,7 @@ def test_fused_post_chain_equals_pass_per_pass(pt, monkeypatch):
     kernel: PostProcessor.cpp:193-246 in 2 + 2(n-2) launches less traffic); B200PT_POST_FUSED=0 runs the reference's pass structure.
     Both must give the same RGBA8 image and the same mip 0, bit for bit, including odd sizes and image borders."""
     rng = np.random.default_rng(3)
-    for (W, H) in ((317, 203), (64, 33), (1280, 720)):
+    for (W, H) in ((317, 203), (64, 33), (1280, 720), (1, 1), (1, 37), (37, 1), (2, 2), (5, 3), (31, 7), (32, 8), (33, 9), (63, 17), (65, 15), (8, 8), (1023, 767)):
         hdr = np.ones((H, W, 4), np.float32); hdr[..., :3] = (np.exp(rng.normal(0, 1.5, (H, W, 3))) * 0.5).astype(np.float32)
         hdr[H // 3:H // 3 + 4, W // 2:W // 2 + 4, :3] = 500.0; hdr[0, 0, :3] = 300.0; hdr[H - 1, W - 1, :3] = 300.0
         out = {}
@@ -665,14 +665,14 @@ def test_volume_api_and_traversal_shapes(pt, monkeypatch):
     with pytest.raises(P.B200ptError): T.add_volume(**vol)
 
 
-@pytest.mark.parametrize("W,H,world", [(517, 389, 2), (640, 360, 3), (1280, 720, 8)])
+@pytest.mark.parametrize("W,H,world", [(517, 389, 2), (640, 360, 3), (1280, 720, 8), (33, 9, 2), (63, 17, 3), (65, 15, 2), (31, 7, 2), (1023, 767, 8)])
 def test_post_row_blocks_equal_the_full_image_pass(pt, W, H, world):
     """BASELINE config 5 on N GPUs: every rank post-processes one block of output rows (b200pt_post_process_rows) from the full HDR input,
     recomputing the halo rows of each bloom mip its block depends on.  The union of the blocks must equal b200pt_post_process bit for bit --
     including blocks whose boundaries are not multiples of the 8-row tiles, and mips so small that every block needs all of them."""
     rng = np.random.default_rng(11)
     hdr = np.ones((H, W, 4), np.float32); hdr[..., :3] = (np.exp(rng.normal(0, 1.5, (H, W, 3))) * 0.6).astype(np.float32)
-    for _ in range(12):
+    for _ in range(12 if W * H > 4096 else 1):                             # one hot block at the small sizes, which twelve would saturate
         y, x = rng.integers(0, H - 4), rng.integers(0, W - 4); hdr[y:y + 4, x:x + 4, :3] = 300.0
     T = util.product_tracer("cornell_box", W, H)
     T.set_hdr(hdr); T.post_process(); full = T.get_ldr().copy()
