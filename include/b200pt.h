@@ -444,6 +444,43 @@ int32_t b200pt_shade_query(b200pt_handle h, int32_t force_general, uint32_t n, c
 #define B200PT_MQ_PDF        3    /* sky sampler pdf of the direction (alpha of the lookup; 1 where no lookup is made) */
 #define B200PT_MQ_STRIDE     4
 int32_t b200pt_miss_query(b200pt_handle h, uint32_t n, const float *dir3, const uint32_t *depth, const float *pay_pdf, float *out);
+/* Bounce test hook: one non-primary bounce of the renderer (the extension ray, miss or hit shading, the NEE queries, the path epilogue and the
+ * compaction of the survivors) for n caller-given live paths, through the launch sequence and the kernels Engine::path_trace runs for the
+ * current scene and config.  in: n records of B200PT_BQ_IN_STRIDE floats; the sample slot of record i is i (IN_SLOT is ignored), IN_SAMPLE is
+ * the slot's value before the bounce.  DFLAGS = Depth | (colour channel + 1, 0 = unsplit) << 27 | InMedium << 31.  flags: B200PT_BQ_STORE
+ * (a path end stores its radiance instead of adding it to the slot), B200PT_BQ_CARRY (a path end stores its RNG state for a next sub-wave).
+ * out: n records of B200PT_BQ_OUT_STRIDE floats, record i for input i: the hit of the extension ray (ids 0xFFFFFFFF on a miss), ALIVE, the
+ * successor state in the input layout (ALIVE only; its medium fields only when InMedium), the slot value after the bounce and the carried
+ * RNG state (0 unless the path ended under B200PT_BQ_CARRY).  *survivors: the survivor count the kernels wrote.  Waits for the waves in
+ * flight; the accumulation, the dispatch counter and the adaptive state are not touched; the work counters are.  Throughput, radiance, pdf,
+ * medium and slot values may be anything.  B200PT_ERR_NO_SCENE without a scene, an environment map or the LUTs; B200PT_ERR_WRONG_ARGUMENTS
+ * for volumes or the atmosphere, a non-finite origin, a zero or non-finite direction, Depth >= MaxDepth, DFLAGS bits 29-30 set or unknown
+ * flag bits. */
+#define B200PT_BQ_STORE       2
+#define B200PT_BQ_CARRY       4
+#define B200PT_BQ_IN_ORG      0    /* origin, then the pdf of the segment's BSDF sample */
+#define B200PT_BQ_IN_PDF      3
+#define B200PT_BQ_IN_DIR      4    /* direction, then the sampler state (u32 bits) */
+#define B200PT_BQ_IN_RNG      7
+#define B200PT_BQ_IN_THR      8    /* throughput, then DFLAGS (u32 bits) */
+#define B200PT_BQ_IN_DFLAGS   11
+#define B200PT_BQ_IN_RAD      12   /* radiance gathered so far, then the sample slot (u32 bits) */
+#define B200PT_BQ_IN_SLOT     15
+#define B200PT_BQ_IN_MEDIUM   16   /* medium colour, density */
+#define B200PT_BQ_IN_MEDIUM_G 20   /* medium anisotropy */
+#define B200PT_BQ_IN_SAMPLE   21   /* sample slot value before the bounce (4 floats) */
+#define B200PT_BQ_IN_STRIDE   25
+#define B200PT_BQ_OUT_T       0
+#define B200PT_BQ_OUT_U       1
+#define B200PT_BQ_OUT_V       2
+#define B200PT_BQ_OUT_INST    3    /* u32 bits */
+#define B200PT_BQ_OUT_PRIM    4    /* u32 bits */
+#define B200PT_BQ_OUT_ALIVE   5
+#define B200PT_BQ_OUT_NEXT    6    /* B200PT_BQ_IN_SAMPLE floats in the input layout */
+#define B200PT_BQ_OUT_SAMPLE  27
+#define B200PT_BQ_OUT_CARRY   31   /* u32 bits */
+#define B200PT_BQ_OUT_STRIDE  32
+int32_t b200pt_bounce_query(b200pt_handle h, uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors);
 
 /* Energy-compensation lookup-table baker (SURVEY.md 8f row 2).
  * Replaces LookupTableCalculator::CalculateTable(tableSize, sampleCount) (PathTracer/LookupTableCalculator.h:8,

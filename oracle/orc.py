@@ -144,6 +144,8 @@ def lib():
         L.orc_shade_query.restype = None
         L.orc_miss_query.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32] + [C.c_void_p] * 4
         L.orc_miss_query.restype = None
+        L.orc_bounce_query.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]
+        L.orc_bounce_query.restype = None
         L.orc_render.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.POINTER(OrcCounters)]
         L.orc_sample_pixel.argtypes = [C.c_void_p, C.POINTER(OrcConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -367,6 +369,14 @@ class Scene:
         out = np.zeros((n, 4), np.float32)
         lib().orc_miss_query(self.h, C.byref(cfg), n, _p(dirs), _p(depth), _p(pay_pdf), _p(out))
         return out
+
+    def bounce_query(self, cfg, records, store=False, carry=False):
+        """orc_bounce_query: one path segment and the slot fold per [n, 25] record laid out like B200PT_BQ_IN_*.  Returns ([n, 32] float32
+        records laid out like B200PT_BQ_OUT_*, number alive)."""
+        rec = np.ascontiguousarray(records, np.float32).reshape(-1, 25); n = len(rec)
+        out = np.zeros((n, 32), np.float32); m = C.c_uint32()
+        lib().orc_bounce_query(self.h, C.byref(cfg), n, _p(rec), (2 if store else 0) | (4 if carry else 0), _p(out), C.byref(m))
+        return out, m.value
 
     def render(self, cfg, W, H, nframes, base_seed, frame0=0, image=None, rank=0, world=1, band_rows=1, nthreads=0):
         if image is None: image = np.zeros((H, W, 4), np.float32)

@@ -1675,6 +1675,43 @@ void orc_miss_query(const OrcScene *sc, const OrcConfig *cfg, uint32_t n, const 
 /* ------------------------------------------------------------------------------------------------
  * RayGen: SH/RayGen.slang:9-160  (ScatteredInVolume with VolumesCount==0 returns false, :162-263, Q5)
  * ---------------------------------------------------------------------------------------------- */
+/* One segment of the path loop (:66-113): trace, shade, clamp (Q3), throughput, Russian roulette (Q4).  Returns 0 when the path ends in the
+ * segment (below the planet, or the roulette), 1 otherwise; the loop condition Depth < MaxDepth is the caller's.  hit (optional): the
+ * segment's closest hit (hit = 0 on a miss or a volume event). */
+static int path_segment(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, v3 *throughput, v3 *pathLight, OrcCounters *cnt, Hit *hit) {
+    v3 ro = pl->Origin, rd = v3normalize(pl->Direction);
+    pl->Emitted = v3s(0.0f);
+    if (hit) memset(hit, 0, sizeof *hit);
+    if (cfg->EnableAtmosphere && atm_height(cfg, pl->Origin) < 0.0f) return 0;  /* :76-84: below the surface of the planet */
+    cnt->segments++;
+    if (!((cfg->VolumesCount || cfg->EnableAtmosphere) && scattered_in_volume(sc, cfg, pl, cnt))) {         /* :86-90 */
+        Hit h = trace_bvh(sc, ro, rd, 0.01f, 100000.0f);
+        if (hit) *hit = h;
+        if (h.hit) closest_hit(sc, cfg, pl, rd, &h, cnt);
+        else { miss_shader(sc, cfg, pl); cnt->misses++; }
+    }
+    v3 contribution = v3mul(pl->Emitted, *throughput);
+    if (pl->Depth != 1) {                                                       /* Q3 */
+        float lum = v3dot(contribution, V3(0.212671f, 0.715160f, 0.072169f));
+        float scale = cfg->MaxLuminance / fmaxf(lum, cfg->MaxLuminance);
+        contribution = v3scale(contribution, scale);
+    }
+    *pathLight = v3add(*pathLight, contribution);
+    *throughput = v3mul(*throughput, v3divs(pl->BxDF, pl->PDF));
+    float p = fmaxf(throughput->x, fmaxf(throughput->y, throughput->z));
+    p = fminf(p, 1.0f);
+    if (p < rng_f(&pl->Sampler)) return 0;                                      /* Q4 */
+    *throughput = v3divs(*throughput, p);
+    return 1;
+}
+
+/* :116-128: a finished sample's light is added to acc unless a component is NaN or Inf; a ray split by an atmosphere event carries one channel */
+static void fold_sample(v3 *acc, v3 l, int channel) {
+    if (isinf(l.x) || isinf(l.y) || isinf(l.z) || isnan(l.x) || isnan(l.y) || isnan(l.z)) return;
+    if (channel == -1) *acc = v3add(*acc, l);
+    else if (channel == 0) acc->x += l.x; else if (channel == 1) acc->y += l.y; else acc->z += l.z;
+}
+
 static v3 trace_one_sample(const OrcScene *sc, const OrcConfig *cfg, Payload *pl, uint32_t W, uint32_t H,
                            uint32_t px, uint32_t py, OrcCounters *cnt) {
     const float *VI = cfg->ViewInverse, *PI = cfg->ProjectionInverse;
@@ -1702,30 +1739,56 @@ static v3 trace_one_sample(const OrcScene *sc, const OrcConfig *cfg, Payload *pl
     pl->BxDF = v3s(1.0f); pl->PDF = 1.0f; pl->Emitted = v3s(0.0f); pl->InMedium = 0; pl->VolumeDepth = 0; pl->ColorChannel = -1;
     v3 throughput = v3s(1.0f), pathLight = v3s(0.0f);
     cnt->paths++;
-    while (pl->Depth < cfg->MaxDepth) {
-        v3 ro = pl->Origin, rd = v3normalize(pl->Direction);
-        pl->Emitted = v3s(0.0f);
-        if (cfg->EnableAtmosphere && atm_height(cfg, pl->Origin) < 0.0f) break;    /* :76-84: below the surface of the planet */
-        cnt->segments++;
-        if (!((cfg->VolumesCount || cfg->EnableAtmosphere) && scattered_in_volume(sc, cfg, pl, cnt))) {         /* :86-90 */
-            Hit h = trace_bvh(sc, ro, rd, 0.01f, 100000.0f);
-            if (h.hit) closest_hit(sc, cfg, pl, rd, &h, cnt);
-            else { miss_shader(sc, cfg, pl); cnt->misses++; }
-        }
-        v3 contribution = v3mul(pl->Emitted, throughput);
-        if (pl->Depth != 1) {                                                   /* Q3 */
-            float lum = v3dot(contribution, V3(0.212671f, 0.715160f, 0.072169f));
-            float scale = cfg->MaxLuminance / fmaxf(lum, cfg->MaxLuminance);
-            contribution = v3scale(contribution, scale);
-        }
-        pathLight = v3add(pathLight, contribution);
-        throughput = v3mul(throughput, v3divs(pl->BxDF, pl->PDF));
-        float p = fmaxf(throughput.x, fmaxf(throughput.y, throughput.z));
-        p = fminf(p, 1.0f);
-        if (p < rng_f(&pl->Sampler)) break;                                     /* Q4 */
-        throughput = v3divs(throughput, p);
-    }
+    while (pl->Depth < cfg->MaxDepth && path_segment(sc, cfg, pl, &throughput, &pathLight, cnt, NULL)) {}
     return pathLight;
+}
+
+void orc_bounce_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors) {
+    uint32_t alive_n = 0;
+    memset(out, 0, (size_t)n * ORC_BQ_OUT_STRIDE * sizeof(float));
+    for (uint32_t i = 0; i < n; i++) {
+        const float *r = in + (size_t)i * ORC_BQ_IN_STRIDE;
+        float *o = out + (size_t)i * ORC_BQ_OUT_STRIDE;
+        uint32_t dflags, seed; memcpy(&dflags, r + ORC_BQ_IN_DFLAGS, 4); memcpy(&seed, r + ORC_BQ_IN_RNG, 4);
+        Payload pl; memset(&pl, 0, sizeof(pl));
+        pl.Origin = V3(r[ORC_BQ_IN_ORG], r[ORC_BQ_IN_ORG + 1], r[ORC_BQ_IN_ORG + 2]); pl.PDF = r[ORC_BQ_IN_PDF];
+        pl.Direction = V3(r[ORC_BQ_IN_DIR], r[ORC_BQ_IN_DIR + 1], r[ORC_BQ_IN_DIR + 2]); pl.Sampler.seed = seed;
+        pl.Depth = dflags & 0x07FFFFFFu; pl.ColorChannel = (int)((dflags >> 27) & 3u) - 1; pl.InMedium = (int)(dflags >> 31);
+        pl.MediumColor = V3(r[ORC_BQ_IN_MEDIUM], r[ORC_BQ_IN_MEDIUM + 1], r[ORC_BQ_IN_MEDIUM + 2]);
+        pl.MediumDensity = r[ORC_BQ_IN_MEDIUM + 3]; pl.MediumAnisotropy = r[ORC_BQ_IN_MEDIUM_G];
+        v3 throughput = V3(r[ORC_BQ_IN_THR], r[ORC_BQ_IN_THR + 1], r[ORC_BQ_IN_THR + 2]);
+        v3 pathLight = V3(r[ORC_BQ_IN_RAD], r[ORC_BQ_IN_RAD + 1], r[ORC_BQ_IN_RAD + 2]);
+        OrcCounters c; memset(&c, 0, sizeof(c));
+        Hit h;
+        const int alive = path_segment(s, cfg, &pl, &throughput, &pathLight, &c, &h) && pl.Depth < cfg->MaxDepth;
+        uint32_t inst = 0xFFFFFFFFu, prim = 0xFFFFFFFFu;
+        if (h.hit) { inst = s->tris[h.tri].inst; prim = s->tris[h.tri].prim; o[ORC_BQ_OUT_T] = h.t; o[ORC_BQ_OUT_U] = h.u; o[ORC_BQ_OUT_V] = h.v; }
+        memcpy(o + ORC_BQ_OUT_INST, &inst, 4); memcpy(o + ORC_BQ_OUT_PRIM, &prim, 4);
+        o[ORC_BQ_OUT_ALIVE] = alive ? 1.0f : 0.0f;
+        memcpy(o + ORC_BQ_OUT_SAMPLE, r + ORC_BQ_IN_SAMPLE, 16);
+        if (alive) {
+            float *x = o + ORC_BQ_OUT_NEXT;
+            const uint32_t nd = pl.Depth | ((uint32_t)(pl.ColorChannel + 1) << 27) | (pl.InMedium ? 0x80000000u : 0u);
+            x[ORC_BQ_IN_ORG] = pl.Origin.x; x[ORC_BQ_IN_ORG + 1] = pl.Origin.y; x[ORC_BQ_IN_ORG + 2] = pl.Origin.z; x[ORC_BQ_IN_PDF] = pl.PDF;
+            x[ORC_BQ_IN_DIR] = pl.Direction.x; x[ORC_BQ_IN_DIR + 1] = pl.Direction.y; x[ORC_BQ_IN_DIR + 2] = pl.Direction.z;
+            memcpy(x + ORC_BQ_IN_RNG, &pl.Sampler.seed, 4);
+            x[ORC_BQ_IN_THR] = throughput.x; x[ORC_BQ_IN_THR + 1] = throughput.y; x[ORC_BQ_IN_THR + 2] = throughput.z; memcpy(x + ORC_BQ_IN_DFLAGS, &nd, 4);
+            x[ORC_BQ_IN_RAD] = pathLight.x; x[ORC_BQ_IN_RAD + 1] = pathLight.y; x[ORC_BQ_IN_RAD + 2] = pathLight.z; memcpy(x + ORC_BQ_IN_SLOT, &i, 4);
+            if (pl.InMedium) {
+                x[ORC_BQ_IN_MEDIUM] = pl.MediumColor.x; x[ORC_BQ_IN_MEDIUM + 1] = pl.MediumColor.y; x[ORC_BQ_IN_MEDIUM + 2] = pl.MediumColor.z;
+                x[ORC_BQ_IN_MEDIUM + 3] = pl.MediumDensity; x[ORC_BQ_IN_MEDIUM_G] = pl.MediumAnisotropy;
+            }
+            alive_n++;
+        } else {
+            float *acc4 = o + ORC_BQ_OUT_SAMPLE;
+            if (flags & ORC_BQ_STORE) memset(acc4, 0, 16);
+            v3 acc = V3(acc4[0], acc4[1], acc4[2]);
+            fold_sample(&acc, pathLight, pl.ColorChannel);
+            acc4[0] = acc.x; acc4[1] = acc.y; acc4[2] = acc.z;
+            if (flags & ORC_BQ_CARRY) memcpy(o + ORC_BQ_OUT_CARRY, &pl.Sampler.seed, 4);
+        }
+    }
+    *survivors = alive_n;
 }
 
 void orc_sample_pixel(const OrcScene *s, const OrcConfig *cfg, uint32_t W, uint32_t H,
@@ -1761,10 +1824,7 @@ static void *render_thread(void *arg) {
             v3 acc = v3s(0.0f);
             for (uint32_t i = 0; i < cfg->SampleCount; i++) {
                 v3 l = trace_one_sample(j->s, cfg, &pl, j->W, j->H, x, y, &j->cnt);
-                if (!isinf(l.x) && !isinf(l.y) && !isinf(l.z) && !isnan(l.x) && !isnan(l.y) && !isnan(l.z)) {   /* :116-128 */
-                    if (pl.ColorChannel == -1) acc = v3add(acc, l);
-                    else if (pl.ColorChannel == 0) acc.x += l.x; else if (pl.ColorChannel == 1) acc.y += l.y; else acc.z += l.z;   /* a split ray carries one channel */
-                }
+                fold_sample(&acc, l, pl.ColorChannel);
             }
             acc = v3divs(acc, (float)cfg->SampleCount);
             v3 color;

@@ -222,6 +222,35 @@ void orc_shade_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const 
 #define ORC_MQ_PDF        3
 #define ORC_MQ_STRIDE     4
 void orc_miss_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const float *dir3, const uint32_t *depth, const float *pay_pdf, float *out);
+/* One segment of the path loop (path_segment, SH/RayGen.slang:66-113) and the fold of a finished path into its sample slot (fold_sample,
+ * :116-128) for n caller-given paths, laid out like B200PT_BQ_* of include/b200pt.h: the sample slot of record i is i, flags ORC_BQ_STORE /
+ * ORC_BQ_CARRY as B200PT_BQ_STORE / CARRY.  Throughput and pathLight travel in the record.  *survivors: the number alive.  Scenes without
+ * volumes or the atmosphere. */
+#define ORC_BQ_STORE       2
+#define ORC_BQ_CARRY       4
+#define ORC_BQ_IN_ORG      0
+#define ORC_BQ_IN_PDF      3
+#define ORC_BQ_IN_DIR      4
+#define ORC_BQ_IN_RNG      7
+#define ORC_BQ_IN_THR      8
+#define ORC_BQ_IN_DFLAGS   11
+#define ORC_BQ_IN_RAD      12
+#define ORC_BQ_IN_SLOT     15
+#define ORC_BQ_IN_MEDIUM   16
+#define ORC_BQ_IN_MEDIUM_G 20
+#define ORC_BQ_IN_SAMPLE   21
+#define ORC_BQ_IN_STRIDE   25
+#define ORC_BQ_OUT_T       0
+#define ORC_BQ_OUT_U       1
+#define ORC_BQ_OUT_V       2
+#define ORC_BQ_OUT_INST    3
+#define ORC_BQ_OUT_PRIM    4
+#define ORC_BQ_OUT_ALIVE   5
+#define ORC_BQ_OUT_NEXT    6
+#define ORC_BQ_OUT_SAMPLE  27
+#define ORC_BQ_OUT_CARRY   31
+#define ORC_BQ_OUT_STRIDE  32
+void orc_bounce_query(const OrcScene *s, const OrcConfig *cfg, uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors);
 
 /* One reference dispatch sequence: frames [frame0, frame0+nframes) with Seed_f = PCG_HASH(base_seed + f)
  * (SURVEY 8d; the reference's own seed is wall-clock, PT/PathTracer.cpp:127-140), running-mean accumulate

@@ -74,6 +74,14 @@ def _shade(name):                                                   # b200pt_sha
         assert r.shape == (300, 4) and np.isfinite(r).all()
     print(name, "miss_query ok")
 _shade("cornell_box"); _shade("cornell_box_glass")
+def _bounce():                                                      # b200pt_bounce_query: one fused bounce of 33 paths (a partial second warp)
+    import test_bounce_queries as B
+    R = B.make_records(B.case_scene("classes"), 33, 4, 5)
+    T = util.product_tracer("cornell_box", 8, 8, scene=B.case_scene("classes"), MaxDepth=5)
+    out, m = T.bounce_query(R, store=True, carry=True)
+    assert out.shape == (33, B.BQ_OUT["STRIDE"]) and int(out[:, B.BQ_OUT["ALIVE"]].sum()) == m
+    print("bounce_query ok")
+_bounce()
 def _update(name, inst, env=None):                                  # instance updates: k_refit_slots / k_refit_level (/ k_refit_wide), and the rebuild path
     for k, v in (env or {}).items(): os.environ[k] = v
     T = util.product_tracer(name, 40, 30, MaxDepth=5)

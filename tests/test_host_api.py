@@ -45,6 +45,11 @@ def test_null_arguments_are_rejected_not_crashed():
     assert L.b200pt_miss_query(None, 1, buf.ctypes.data, None, buf.ctypes.data, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
     assert L.b200pt_miss_query(None, 1, buf.ctypes.data, u.ctypes.data, None, buf.ctypes.data) == pt.ERR_WRONG_ARGUMENTS
     assert L.b200pt_miss_query(None, 1, buf.ctypes.data, u.ctypes.data, buf.ctypes.data, None) == pt.ERR_WRONG_ARGUMENTS
+    m = C.c_uint32()
+    assert L.b200pt_bounce_query(None, 1, buf.ctypes.data, 0, buf.ctypes.data, C.byref(m)) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_bounce_query(None, 1, None, 0, buf.ctypes.data, C.byref(m)) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_bounce_query(None, 1, buf.ctypes.data, 0, None, C.byref(m)) == pt.ERR_WRONG_ARGUMENTS
+    assert L.b200pt_bounce_query(None, 1, buf.ctypes.data, 0, buf.ctypes.data, None) == pt.ERR_WRONG_ARGUMENTS
     w, h, p = C.c_uint32(), C.c_uint32(), C.c_void_p()
     assert L.b200pt_decode_image_file(b"/nonexistent.png", C.byref(w), C.byref(h), C.byref(p)) == pt.ERR_INIT_FAILED
 

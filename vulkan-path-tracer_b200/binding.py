@@ -198,6 +198,7 @@ def lib():
             "b200pt_trace_query": [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32] + [C.c_void_p] * 12,
             "b200pt_shade_query": [C.c_void_p, C.c_int32, C.c_uint32] + [C.c_void_p] * 9,
             "b200pt_miss_query": [C.c_void_p, C.c_uint32] + [C.c_void_p] * 4,
+            "b200pt_bounce_query": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
             "b200pt_bake_lut": [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p],
             "b200pt_bake_luts_to_dir": [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32],
             "b200pt_decode_image_file": [C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_void_p)],
@@ -247,6 +248,10 @@ SQ = dict(N=0, T=3, B=6, NG=9, INSIDE=12, AX=13, AY=14, ETA=15, PM=16, PD=17, PG
           LIGHT_W=94, STRIDE=97)
 # record offsets of b200pt_miss_query (B200PT_MQ_*)
 MQ = dict(RGB=0, PDF=3, STRIDE=4)
+# record layouts and flags of b200pt_bounce_query (B200PT_BQ_IN_*, B200PT_BQ_OUT_*, B200PT_BQ_STORE / CARRY)
+BQ_IN = dict(ORG=0, PDF=3, DIR=4, RNG=7, THR=8, DFLAGS=11, RAD=12, SLOT=15, MEDIUM=16, MEDIUM_G=20, SAMPLE=21, STRIDE=25)
+BQ_OUT = dict(T=0, U=1, V=2, INST=3, PRIM=4, ALIVE=5, NEXT=6, SAMPLE=27, CARRY=31, STRIDE=32)
+BQ_STORE, BQ_CARRY = 2, 4
 
 
 def declared_symbols():
@@ -820,6 +825,15 @@ class PathTracer:
         out = np.zeros((n, MQ["STRIDE"]), np.float32)
         self._ck(self.L.b200pt_miss_query(self.h, n, _p(dirs), _p(depth), _p(pay_pdf), _p(out)))
         return out
+
+    def bounce_query(self, records, store=False, carry=False):
+        """b200pt_bounce_query: one bounce of the renderer for [n, BQ_IN["STRIDE"]] float32 path records (u32 fields as their bits).
+        Returns ([n, BQ_OUT["STRIDE"]] float32 records, survivor count)."""
+        rec = np.ascontiguousarray(records, np.float32).reshape(-1, BQ_IN["STRIDE"]); n = len(rec)
+        out = np.zeros((n, BQ_OUT["STRIDE"]), np.float32)
+        m = C.c_uint32()
+        self._ck(self.L.b200pt_bounce_query(self.h, n, _p(rec), (BQ_STORE if store else 0) | (BQ_CARRY if carry else 0), _p(out), C.byref(m)))
+        return out, m.value
 
     def scene_stats(self):
         a, b, c, d = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()

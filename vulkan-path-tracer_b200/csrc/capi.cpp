@@ -321,6 +321,10 @@ int32_t b200pt_miss_query(b200pt_handle h, uint32_t n, const float *d, const uin
     if (n && (!d || !depth || !pay_pdf || !out)) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { e.miss_query(n, d, depth, pay_pdf, out); });
 }
+int32_t b200pt_bounce_query(b200pt_handle h, uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors) {
+    if (!survivors || (n && (!in || !out))) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { e.bounce_query(n, in, flags, out, survivors); });
+}
 int32_t b200pt_bake_lut(b200pt_handle h, int32_t kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t sample_count, uint32_t seed, uint32_t slices, float *out, float *elapsed_ms) {
     if (!out || kind < 0 || kind > 2 || !sx || !sy || !sz) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { e.bake_lut(kind, sx, sy, sz, sample_count, seed, slices, out, elapsed_ms); });

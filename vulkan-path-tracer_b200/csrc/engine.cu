@@ -585,6 +585,9 @@ void Engine::set_luts(const float *refl, const float *rout, const float *rin) {
 
 void Engine::set_config(const b200pt_config &c) {
     if (c.SamplesPerFrame == 0 || c.ScreenChunkCount == 0 || c.ScreenChunkCount > 64) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "SamplesPerFrame and ScreenChunkCount must be >= 1" };
+    // The clamp scales a contribution by MaxLuminance / max(lum, MaxLuminance): +inf gives inf / inf = NaN on every segment at Depth != 1, 0 gives
+    // 0 / 0 on every zero contribution and NaN gives NaN everywhere, and the sample rejection then discards the whole path (a black image).
+    if (!std::isfinite(c.MaxLuminance) || !(c.MaxLuminance > 0.0f)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "MaxLuminance must be finite and > 0" };
     if (c.ScreenChunkCount > 1 && world_ > 1) throw CudaError{ B200PT_ERR_NOT_IMPLEMENTED, "ScreenChunkCount > 1 cannot be combined with a multi-GPU partition" };
     if (c.ScreenChunkCount > 1 && adaptive_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "ScreenChunkCount > 1 cannot be combined with adaptive sampling" };
     if (c.ScreenChunkCount > 1 && track_variance_) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "ScreenChunkCount > 1 cannot be combined with per-pixel statistics" };
@@ -742,6 +745,26 @@ DevConfig Engine::make_dev_config() const {
     return d;
 }
 
+// Conservative: the device-side metallic value is Metallic * texel, so the constant factor alone cannot rule refraction out, and a negative
+// density (not validated by the reference either) scatters on every segment.  A false positive only costs a 4-byte read-back per 16 bounces.
+bool Engine::scene_has_media() const {
+    for (const auto &m : scene_.materials) if (m.Transmission > 0.0f && m.MediumDensity != 0.0f && m.MediumAnisotropy != 1.0f) return true;
+    return false;
+}
+
+// One bounce of path_trace's loop; bounce_query runs the same sequence on caller-given paths.
+uint64_t Engine::bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
+                        const std::function<void(int)> &mark) {
+    const uint32_t par = k & 1u;
+    const Queues q{ B.q_miss, B.q_hit, (uint32_t)wave_cap_ };
+    uint64_t launches = 0;
+    if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st);
+    if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); mark(1);
+    launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, flags, st); mark(2);
+    if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, flags, st); mark(3);
+    return launches;
+}
+
 // PathTracer::PathTrace x dispatches (PathTracer.cpp:122-156)
 bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     CK(cudaSetDevice(device_));
@@ -798,10 +821,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     const DevConfig dc = make_dev_config();
     auto pcg = [](uint32_t in) { uint32_t st = in * 747796405u + 2891336453u; uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; };
 
-    bool medium = false;                                      // can a path random-walk inside a mesh without gaining Depth?
-    // Conservative: the device-side metallic value is Metallic * texel, so the constant factor alone cannot rule refraction out, and a negative
-    // density (not validated by the reference either) scatters on every segment.  A false positive only costs a 4-byte read-back per 16 bounces.
-    for (const auto &m : scene_.materials) if (m.Transmission > 0.0f && m.MediumDensity != 0.0f && m.MediumAnisotropy != 1.0f) medium = true;
+    const bool medium = scene_has_media();
     const CallPlan cp = plan_call(lc_, ds_, dc, medium, class_mask_);
     ds_.pre_pass = cp.pre ? 1u : 0u;
     const uint32_t implied_flag = cp.implied ? WAVE_IMPLIED : 0u;   // per-launch flags: kernels.h
@@ -809,7 +829,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
 
     uint64_t launches = 0; uint32_t waves = 0, bounces_total = 0;
     std::vector<int> prof_kind; size_t prof_n = 0;            // kind: 0 raygen 1 extend 2 shade 3 connect 4 resolve
-    auto mark = [&](int kind) {
+    const std::function<void(int)> mark = [&](int kind) {
         if (!profiling_) return;
         if (prof_n >= prof_ev_.size()) { cudaEvent_t e; CK(cudaEventCreate(&e)); prof_ev_.push_back(e); }
         CK(cudaEventRecord(prof_ev_[prof_n++], stream_)); prof_kind.push_back(kind);
@@ -857,11 +877,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     if (!medium && cfg_.MaxDepth - std::min(cfg_.MaxDepth, k) < chunk) chunk = cfg_.MaxDepth - std::min(cfg_.MaxDepth, k);
                     if (chunk == 0) break;
                     for (uint32_t b = 0; b < chunk; b++, k++) {
-                        const uint32_t par = k & 1u, bflags = wflags | (k == 0 ? implied_flag : 0u);
-                        if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st);
-                        if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); mark(1);
-                        launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); mark(2);
-                        if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, bflags, st); mark(3);
+                        launches += bounce(cp, dc, B, pst, cur, k, wflags | (k == 0 ? implied_flag : 0u), st, mark);
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty
@@ -894,6 +910,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
         }
     }
     CK(cudaEventRecord(ev_[1], last_st));                     // ms_total: first kernel of the first wave .. resolve of the last (counters() synchronises before reading it)
+    timed_ = true;
     CK(cudaGetLastError());
     dispatch_count_ += todo;
     frame_count_ = (uint32_t)(dispatch_count_ / S2);                     // PathTracer.cpp:152
@@ -923,7 +940,9 @@ b200pt_counters Engine::counters() {
     b200pt_counters c = last_;
     c.paths = wc.paths; c.extend_rays = wc.extend_rays; c.shade_invocations = wc.shade_invocations; c.surface_hits = wc.surface_hits;
     c.misses = wc.misses; c.shadow_rays = wc.shadow_rays; c.medium_events = wc.medium_events;
-    float ms = 0.0f; if (cudaEventElapsedTime(&ms, ev_[0], ev_[1]) == cudaSuccess) c.ms_total = ms;
+    float ms = 0.0f;
+    if (timed_) CK(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));   // (querying never-recorded events would leave an error for the next call to find)
+    c.ms_total = ms;
     return c;
 }
 
@@ -1255,6 +1274,106 @@ void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, con
     e = cudaStreamSynchronize(stream_);
     for (void *p : bufs) cudaFree(p);
     CK(e); CK(cudaGetLastError());
+}
+void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!has_env_ || !has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "bounce_query: no environment map or no lookup tables" };
+    if (ds_.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: scenes with volumes or the atmosphere are not supported" };
+    static_assert(B200PT_BQ_STORE == WAVE_STORE && B200PT_BQ_CARRY == WAVE_CARRY, "bounce_query flags are the wave flags");
+    if (flags & ~(uint32_t)(B200PT_BQ_STORE | B200PT_BQ_CARRY)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: unknown flag bits" };
+    *survivors = 0;
+    if (!n) return;
+    constexpr uint32_t IN = B200PT_BQ_IN_STRIDE, OUT = B200PT_BQ_OUT_STRIDE;
+    std::vector<float4> org_pdf(n), dir_rng(n), thr_depth(n), rad_slot(n), medium(n), sample(n);
+    std::vector<float> medium_g(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const float *r = in + (size_t)i * IN;
+        const float *o = r + B200PT_BQ_IN_ORG, *d = r + B200PT_BQ_IN_DIR;
+        uint32_t dflags; memcpy(&dflags, r + B200PT_BQ_IN_DFLAGS, 4);
+        if (!std::isfinite(o[0]) || !std::isfinite(o[1]) || !std::isfinite(o[2])) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: non-finite origin" };
+        if (!std::isfinite(d[0]) || !std::isfinite(d[1]) || !std::isfinite(d[2]) || (d[0] == 0.0f && d[1] == 0.0f && d[2] == 0.0f))
+            throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: zero or non-finite direction" };
+        if ((dflags & 0x07FFFFFFu) >= cfg_.MaxDepth) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: Depth >= MaxDepth" };
+        if (dflags & (3u << 29)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: DFLAGS bits 29-30 set" };
+        org_pdf[i] = make_float4(o[0], o[1], o[2], r[B200PT_BQ_IN_PDF]);
+        dir_rng[i] = make_float4(d[0], d[1], d[2], r[B200PT_BQ_IN_RNG]);
+        thr_depth[i] = make_float4(r[B200PT_BQ_IN_THR], r[B200PT_BQ_IN_THR + 1], r[B200PT_BQ_IN_THR + 2], r[B200PT_BQ_IN_DFLAGS]);
+        float slot; memcpy(&slot, &i, 4);
+        rad_slot[i] = make_float4(r[B200PT_BQ_IN_RAD], r[B200PT_BQ_IN_RAD + 1], r[B200PT_BQ_IN_RAD + 2], slot);
+        memcpy(&medium[i], r + B200PT_BQ_IN_MEDIUM, 16); medium_g[i] = r[B200PT_BQ_IN_MEDIUM_G];
+        memcpy(&sample[i], r + B200PT_BQ_IN_SAMPLE, 16);
+    }
+    sync_all();                                               // the wave buffers of context 0 may still serve a wave in flight
+    ensure_wave(n, 1);
+    WaveBuf &B = wb_[0];
+    const PathState pst[2] = { { B.ps[0].org_pdf, B.ps[0].dir_rng, B.ps[0].thr_depth, B.ps[0].rad_slot, B.ps[0].medium, B.ps[0].medium_g, nullptr },
+                               { B.ps[1].org_pdf, B.ps[1].dir_rng, B.ps[1].thr_depth, B.ps[1].rad_slot, B.ps[1].medium, B.ps[1].medium_g, nullptr } };
+    const int cur = 1; const uint32_t k = 1;                  // a non-primary bounce: control word k & 1 holds the live count
+    const size_t b4 = (size_t)n * sizeof(float4);
+    CK(cudaMemcpyAsync(pst[cur].org_pdf, org_pdf.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(pst[cur].dir_rng, dir_rng.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(pst[cur].thr_depth, thr_depth.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(pst[cur].rad_slot, rad_slot.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(pst[cur].medium, medium.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(pst[cur].medium_g, medium_g.data(), (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(B.sample_buf, sample.data(), b4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemsetAsync(B.rng_carry, 0, (size_t)n * 4, stream_));
+    CK(cudaMemsetAsync(B.counts, 0, CTRL_WORDS * sizeof(uint32_t), stream_));
+    CK(cudaMemcpyAsync(B.counts + (k & 1u), &n, 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaStreamSynchronize(stream_));                       // (the pageable sources above are copied by now)
+
+    const DevConfig dc = make_dev_config();
+    const CallPlan cp = plan_call(lc_, ds_, dc, scene_has_media(), class_mask_);
+    ds_.pre_pass = 0u;
+    last_.kernel_launches += bounce(cp, dc, B, pst, cur, k, flags, stream_, [](int) {});
+
+    std::vector<float4> hit(n), nx_op(n), nx_dr(n), nx_td(n), nx_rs(n), nx_med(n);
+    std::vector<float> nx_g(n);
+    std::vector<uint32_t> carry(n), ctrl(CTRL_WORDS);
+    const PathState &dst = pst[cur ^ 1];
+    CK(cudaMemcpyAsync(ctrl.data(), B.counts, CTRL_WORDS * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(hit.data(), B.so.hit, b4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(sample.data(), B.sample_buf, b4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(carry.data(), B.rng_carry, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    const uint32_t m = ctrl[(k & 1u) ^ 1u];
+    *survivors = m;
+    if (m > n) throw CudaError{ B200PT_ERR_CUDA, "bounce_query: more survivors than paths" };
+    if (m) {
+        const size_t m4 = (size_t)m * sizeof(float4);
+        CK(cudaMemcpyAsync(nx_op.data(), dst.org_pdf, m4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(nx_dr.data(), dst.dir_rng, m4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(nx_td.data(), dst.thr_depth, m4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(nx_rs.data(), dst.rad_slot, m4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(nx_med.data(), dst.medium, m4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(nx_g.data(), dst.medium_g, (size_t)m * 4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));
+    }
+    CK(cudaGetLastError());
+    memset(out, 0, (size_t)n * OUT * sizeof(float));
+    for (uint32_t i = 0; i < n; i++) {
+        float *r = out + (size_t)i * OUT;
+        uint32_t gid; memcpy(&gid, &hit[i].w, 4);
+        uint32_t inst = 0xFFFFFFFFu, prim = 0xFFFFFFFFu;
+        if (gid < n_tris_) {                                  // instance-major triangle id -> (instance, primitive of its mesh)
+            const auto it = std::upper_bound(h_instances_.begin(), h_instances_.end(), gid, [](uint32_t g, const DevInstance &a) { return g < a.tri_base; });
+            inst = (uint32_t)(it - h_instances_.begin()) - 1u; prim = gid - h_instances_[inst].tri_base;
+        }
+        r[B200PT_BQ_OUT_T] = hit[i].x; r[B200PT_BQ_OUT_U] = hit[i].y; r[B200PT_BQ_OUT_V] = hit[i].z;
+        memcpy(r + B200PT_BQ_OUT_INST, &inst, 4); memcpy(r + B200PT_BQ_OUT_PRIM, &prim, 4);
+        memcpy(r + B200PT_BQ_OUT_SAMPLE, &sample[i], 16); memcpy(r + B200PT_BQ_OUT_CARRY, &carry[i], 4);
+    }
+    for (uint32_t j = 0; j < m; j++) {                        // the survivors in compacted order, each to the record of its slot
+        uint32_t slot; memcpy(&slot, &nx_rs[j].w, 4);
+        if (slot >= n) throw CudaError{ B200PT_ERR_CUDA, "bounce_query: a survivor carries a slot out of range" };
+        float *r = out + (size_t)slot * OUT, *s = r + B200PT_BQ_OUT_NEXT;
+        r[B200PT_BQ_OUT_ALIVE] += 1.0f;                       // (a slot written twice reads 2)
+        memcpy(s + B200PT_BQ_IN_ORG, &nx_op[j], 16); memcpy(s + B200PT_BQ_IN_DIR, &nx_dr[j], 16);
+        memcpy(s + B200PT_BQ_IN_THR, &nx_td[j], 16); memcpy(s + B200PT_BQ_IN_RAD, &nx_rs[j], 16);
+        uint32_t df; memcpy(&df, &nx_td[j].w, 4);
+        if (df >> 31) { memcpy(s + B200PT_BQ_IN_MEDIUM, &nx_med[j], 16); s[B200PT_BQ_IN_MEDIUM_G] = nx_g[j]; }
+    }
 }
 // LookupTableCalculator::CalculateTable (PT/LookupTableCalculator.cpp:44-157) on this engine's device and stream.
 // slices == 0 picks enough dispatch slices to give every SM ~2048 resident threads.

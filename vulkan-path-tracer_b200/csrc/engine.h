@@ -4,6 +4,7 @@
 #include "host_api.h"
 #include "kernels.h"
 #include <cuda_runtime.h>
+#include <functional>
 
 namespace b200pt {
 
@@ -101,6 +102,8 @@ public:
                      const float *pay_pdf, const uint32_t *rng, const float *L, float *out);
     // b200pt_miss_query (host arrays; see include/b200pt.h)
     void miss_query(uint32_t n, const float *dir, const uint32_t *depth, const float *pay_pdf, float *out);
+    // b200pt_bounce_query (host arrays; see include/b200pt.h): one bounce of path_trace's loop for caller-given paths
+    void bounce_query(uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors);
     void scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const;
     // b200pt_bvh2_ploc_build_query (host arrays; see include/b200pt.h): the device builder and the device collapse on the caller's boxes
     void ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes_out, uint32_t *perm_out, uint32_t *n_out, int *depth_out,
@@ -131,6 +134,7 @@ private:
     bool profiling_ = false;
     std::vector<cudaEvent_t> prof_ev_;
     cudaEvent_t ev_[2] = { nullptr, nullptr };
+    bool timed_ = false;                            // ev_ have been recorded (by a path_trace call that launched work)
 
     HostScene scene_;
     bool has_scene_ = false, has_env_ = false, has_luts_ = false;
@@ -185,6 +189,11 @@ private:
     void join_waves();                              // work enqueued on the caller's stream from here on sees every launched wave resolved into the image
     WaveCounters *d_ctr_ = nullptr;
     b200pt_counters last_{};
+    bool scene_has_media() const;                   // can a path random-walk inside a mesh without gaining Depth?
+    // bounce k of a sub-wave in context B: the paths of pst[cur] (control word k & 1) are traced and shaded, the survivors written to
+    // pst[cur ^ 1].  mark(kind) follows each launch group (profiling).  Returns the number of kernels enqueued on st.
+    uint64_t bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
+                    const std::function<void(int)> &mark);
 
     // adaptive sampling: allocated only while enabled.  The state is rebuilt lazily (prepare_adaptive) after every reset.
     b200pt_adaptive adaptive_{};
