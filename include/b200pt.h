@@ -348,6 +348,8 @@ int32_t b200pt_bloom_mip_sizes(uint32_t width, uint32_t height, uint32_t *wh_out
 int32_t b200pt_save_png(b200pt_handle h, const char *path);
 
 /* ---- fine-grained hooks used by the parity tests (closest-hit semantics of RTCommon.slang:47-117) ---- */
+/* b200pt_trace_query's closest-hit walk (tmin < t < tmax for every ray, subtract-then-multiply slabs) in the shape the renderer's one-ray-per-thread
+ * kernels take for the scene: B200PT_TRAV_FLAT or _SHARED when the BVH is staged in shared memory, _GLOBAL otherwise.  Outputs as there. */
 int32_t b200pt_trace_closest(b200pt_handle h, uint32_t n, const float *origins3, const float *directions3,
                              float tmin, float tmax, float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out2);
 /* the volume walks on given rays (parity hook; needs no scene): out_T[i] = Volume::CalculateVolumesTransmittance (SH/Volume.slang:419-446) from seeds[i],
@@ -355,7 +357,7 @@ int32_t b200pt_trace_closest(b200pt_handle h, uint32_t n, const float *origins3,
  * or -1) from the same seed, out_rng[2*i] / [2*i+1] = the sampler state after each -- the number of random numbers a walk consumed must match too */
 int32_t b200pt_volume_walks(b200pt_handle h, uint32_t n, const float *origins3, const float *directions3, const uint32_t *seeds, float ray_depth,
                             float *out_T, float *out_scatter, int32_t *out_volume, uint32_t *out_rng2);
-/* traversal cost of the same query: nodes_tris_out[2*i] = BVH nodes visited, [2*i+1] = triangles tested (measurement hook) */
+/* traversal cost of b200pt_trace_closest's walk: nodes_tris_out[2*i] = BVH nodes visited, [2*i+1] = triangles tested (measurement hook) */
 int32_t b200pt_trace_stats(b200pt_handle h, uint32_t n, const float *origins3, const float *directions3, float tmin, float tmax, uint32_t *nodes_tris_out);
 /* Traversal test hook: ray i (per-ray tmin[i] < t < tmax[i]) through one traversal shape the renderer can launch and one query kind.
  * shape: B200PT_TRAV_SHARED / _GLOBAL: BVH2 stack walk, one ray per thread, BVH staged in shared memory / read from global memory;

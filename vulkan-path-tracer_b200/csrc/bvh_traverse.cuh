@@ -65,7 +65,7 @@ template <bool SMEM> __device__ __forceinline__ float4 ld4(const float4 *p) {
 
 // Moeller-Trumbore with precomputed edges; the same formula as the oracle's tri_hit().
 // The products are written with explicit FMA / multiply intrinsics so that every kernel this is inlined into (k_extend, k_connect,
-// k_extend_dyn, k_shadow_dyn, k_trace_rays) rounds identically: the traversal shapes are interchangeable bit for bit (tested).
+// k_extend_dyn, k_shadow_dyn, k_trace_query) rounds identically: the traversal shapes are interchangeable bit for bit (tested).
 __device__ __forceinline__ float3 cross_fma(float3 a, float3 b) {          // a x b, each component fma(a1, b2, -(a2 * b1))
     return f3(__fmaf_rn(a.y, b.z, -__fmul_rn(a.z, b.y)), __fmaf_rn(a.z, b.x, -__fmul_rn(a.x, b.z)), __fmaf_rn(a.x, b.y, -__fmul_rn(a.y, b.x)));
 }

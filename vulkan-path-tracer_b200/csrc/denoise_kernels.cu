@@ -17,7 +17,7 @@ namespace b200pt {
 // ------------------------------------------------------------------------------------------------
 // k_features : FeatureSamples camera rays per local pixel from one PCG stream seeded y + W * x + seed0 (global pixel coordinates, so a tile
 // partition's rows equal the one-rank rows), each drawing its jitter and lens samples in camera_ray's order.  The closest hit of each ray
-// (k_trace_rays' query after k_extend's normalize_ray) gives albedo (pd + pm) * BaseColor + pg, the shading normal and the view depth;
+// (the walk of b200pt_trace_closest after k_extend's normalize_ray) gives albedo (pd + pm) * BaseColor + pg, the shading normal and the view depth;
 // a miss counts as albedo 1, normal 0.  Volumes and the atmosphere are not seen: the features are those of the first surface.
 // ------------------------------------------------------------------------------------------------
 template <bool SMEM>

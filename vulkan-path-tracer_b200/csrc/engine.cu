@@ -11,13 +11,43 @@
 
 namespace b200pt {
 
-void Engine::check(cudaError_t e, const char *what) const {
+static void check_cuda(cudaError_t e, const char *what) {
     if (e != cudaSuccess) throw CudaError{ (int)e, std::string(what) + ": " + cudaGetErrorString(e) };
 }
+void Engine::check(cudaError_t e, const char *what) const { check_cuda(e, what); }
 #define CK(x) check((x), #x)
 
 static const uint32_t kMaxDispatchTable = 1u << 16;
 template <class T> static void dfree(T *&p) { if (p) { cudaFree(p); p = nullptr; } }
+
+// The device arrays of one query-hook call, on the engine's stream.  Every block is freed when the object goes out of scope, also when an
+// allocation, a copy or the launch throws halfway (cudaFree waits for the work still using it).
+class HookArrays {
+public:
+    explicit HookArrays(cudaStream_t st) : st_(st) {}
+    ~HookArrays() { for (void *p : blocks_) cudaFree(p); }
+    HookArrays(const HookArrays &) = delete;
+    HookArrays &operator=(const HookArrays &) = delete;
+    template <class T> T *out(size_t count) {                 // uninitialised
+        void *p = nullptr;
+        blocks_.push_back(nullptr);                           // before the allocation: a full vector cannot lose the block
+        check_cuda(cudaMalloc(&p, count * sizeof(T)), "cudaMalloc");
+        blocks_.back() = p;
+        return static_cast<T *>(p);
+    }
+    template <class T> T *in(const T *src, size_t count) {    // filled from host memory
+        T *p = out<T>(count);
+        check_cuda(cudaMemcpyAsync(p, src, count * sizeof(T), cudaMemcpyHostToDevice, st_), "cudaMemcpyAsync");
+        return p;
+    }
+    template <class T> void get(T *dst, const T *src, size_t count) {
+        check_cuda(cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, st_), "cudaMemcpyAsync");
+    }
+    void sync() { check_cuda(cudaStreamSynchronize(st_), "cudaStreamSynchronize"); check_cuda(cudaGetLastError(), "cudaGetLastError"); }   // the first error
+private:
+    cudaStream_t st_;
+    std::vector<void *> blocks_;
+};
 
 Engine::Engine(int device) : device_(device) {
     int n = 0;
@@ -1144,69 +1174,42 @@ void Engine::volume_walks(uint32_t n, const float *org, const float *dir, const 
     CK(cudaSetDevice(device_));
     if (!n) return;
     sync_all();
-    float *d_o = nullptr, *d_d = nullptr, *d_T = nullptr, *d_s = nullptr; uint32_t *d_seed = nullptr, *d_r = nullptr; int32_t *d_v = nullptr;
-    CK(cudaMalloc(&d_o, (size_t)n * 12)); CK(cudaMalloc(&d_d, (size_t)n * 12)); CK(cudaMalloc(&d_seed, (size_t)n * 4)); CK(cudaMalloc(&d_T, (size_t)n * 4));
-    CK(cudaMalloc(&d_s, (size_t)n * 4)); CK(cudaMalloc(&d_v, (size_t)n * 4)); CK(cudaMalloc(&d_r, (size_t)n * 8));
-    CK(cudaMemcpyAsync(d_o, org, (size_t)n * 12, cudaMemcpyHostToDevice, stream_)); CK(cudaMemcpyAsync(d_d, dir, (size_t)n * 12, cudaMemcpyHostToDevice, stream_));
-    CK(cudaMemcpyAsync(d_seed, seeds, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
-    launch_volume_walks(ds_, n, d_o, d_d, d_seed, ray_depth, d_T, d_s, d_v, d_r, stream_);
-    CK(cudaMemcpyAsync(T, d_T, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_)); CK(cudaMemcpyAsync(scatter, d_s, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
-    CK(cudaMemcpyAsync(vol, d_v, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_)); CK(cudaMemcpyAsync(rng2, d_r, (size_t)n * 8, cudaMemcpyDeviceToHost, stream_));
-    cudaError_t e = cudaStreamSynchronize(stream_);
-    cudaFree(d_o); cudaFree(d_d); cudaFree(d_seed); cudaFree(d_T); cudaFree(d_s); cudaFree(d_v); cudaFree(d_r);
-    CK(e); CK(cudaGetLastError());
+    HookArrays a(stream_);
+    float *d_T = a.out<float>(n), *d_s = a.out<float>(n); int32_t *d_v = a.out<int32_t>(n); uint32_t *d_r = a.out<uint32_t>(2 * (size_t)n);
+    launch_volume_walks(ds_, n, a.in(org, 3 * (size_t)n), a.in(dir, 3 * (size_t)n), a.in(seeds, n), ray_depth, d_T, d_s, d_v, d_r, stream_);
+    a.get(T, d_T, n); a.get(scatter, d_s, n); a.get(vol, d_v, n); a.get(rng2, d_r, 2 * (size_t)n);
+    a.sync();
 }
+// The closest-hit walk of trace_query in the shape the render's one-ray-per-thread kernels take for this scene, with one [tmin, tmax] for all rays.
+// stats: nodes visited and triangles tested per ray.
 void Engine::trace_closest(uint32_t n, const float *org, const float *dir, float tmin, float tmax, float *t, uint32_t *prim, uint32_t *inst, float *uv, uint32_t *stats) {
-    CK(cudaSetDevice(device_));
-    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
-    if (!n) return;
-    float *d_o = nullptr, *d_d = nullptr, *d_t = nullptr, *d_uv = nullptr; uint32_t *d_p = nullptr, *d_i = nullptr;
-    CK(cudaMalloc(&d_o, (size_t)n * 12)); CK(cudaMalloc(&d_d, (size_t)n * 12)); CK(cudaMalloc(&d_t, (size_t)n * 4)); CK(cudaMalloc(&d_uv, (size_t)n * 8));
-    CK(cudaMalloc(&d_p, (size_t)n * 4)); CK(cudaMalloc(&d_i, (size_t)n * 4));
-    CK(cudaMemcpyAsync(d_o, org, (size_t)n * 12, cudaMemcpyHostToDevice, stream_)); CK(cudaMemcpyAsync(d_d, dir, (size_t)n * 12, cudaMemcpyHostToDevice, stream_));
-    uint32_t *d_st = nullptr; if (stats) CK(cudaMalloc(&d_st, (size_t)n * 8));
-    launch_trace_rays(lc_, ds_, n, d_o, d_d, tmin, tmax, d_t, d_p, d_i, d_uv, d_st, stream_);
-    if (stats) CK(cudaMemcpyAsync(stats, d_st, (size_t)n * 8, cudaMemcpyDeviceToHost, stream_));
-    CK(cudaMemcpyAsync(t, d_t, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_)); CK(cudaMemcpyAsync(prim, d_p, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
-    CK(cudaMemcpyAsync(inst, d_i, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_)); CK(cudaMemcpyAsync(uv, d_uv, (size_t)n * 8, cudaMemcpyDeviceToHost, stream_));
-    cudaError_t e = cudaStreamSynchronize(stream_);
-    cudaFree(d_o); cudaFree(d_d); cudaFree(d_t); cudaFree(d_uv); cudaFree(d_p); cudaFree(d_i); if (d_st) cudaFree(d_st);
-    CK(e); CK(cudaGetLastError());
+    const std::vector<float> lo(n, tmin), hi(n, tmax);
+    std::vector<uint32_t> st3(stats ? 3 * (size_t)n : 0);
+    const int shape = lc_.bvh_in_smem ? (ds_.n_flat ? TQ_FLAT : TQ_SHARED) : TQ_GLOBAL;
+    trace_query(shape, TQ_CLOSEST, false, n, org, dir, lo.data(), hi.data(), nullptr, nullptr, t, prim, inst, uv, nullptr, stats ? st3.data() : nullptr);
+    if (stats) for (size_t i = 0; i < n; i++) { stats[2 * i] = st3[3 * i]; stats[2 * i + 1] = st3[3 * i + 1]; }
 }
 void Engine::trace_query(int shape, int kind, bool fma, uint32_t n, const float *org, const float *dir, const float *tmin, const float *tmax, const uint32_t *target,
                          const float *tmax_test, float *t, uint32_t *prim, uint32_t *inst, float *uv, uint32_t *occluded, uint32_t *stats) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
     if (!n) return;
-    std::vector<void *> bufs;
-    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
-    auto dev = [&](size_t bytes, const void *src) -> void * {               // device buffer, filled from src when given
-        void *p = nullptr;
-        cudaError_t e = cudaMalloc(&p, bytes);
-        if (e != cudaSuccess) fail(e);
-        bufs.push_back(p);
-        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
-        return p;
-    };
+    HookArrays a(stream_);
     const bool any = kind != TQ_CLOSEST, tgt = kind == TQ_TARGET;
     TraceQuery q{};
     q.n = n;
-    q.org = (const float *)dev((size_t)n * 12, org); q.dir = (const float *)dev((size_t)n * 12, dir);
-    q.tmin = (const float *)dev((size_t)n * 4, tmin); q.tmax = (const float *)dev((size_t)n * 4, tmax);
-    if (tgt) { q.target = (const uint32_t *)dev((size_t)n * 4, target); q.tmax_test = (const float *)dev((size_t)n * 4, tmax_test); }
-    if (any) q.occluded = (uint32_t *)dev((size_t)n * 4, nullptr);
-    else { q.t = (float *)dev((size_t)n * 4, nullptr); q.prim = (uint32_t *)dev((size_t)n * 4, nullptr); q.inst = (uint32_t *)dev((size_t)n * 4, nullptr); q.uv = (float *)dev((size_t)n * 8, nullptr); }
-    if (stats) q.stats = (uint32_t *)dev((size_t)n * 12, nullptr);
+    q.org = a.in(org, 3 * (size_t)n); q.dir = a.in(dir, 3 * (size_t)n); q.tmin = a.in(tmin, n); q.tmax = a.in(tmax, n);
+    if (tgt) { q.target = a.in(target, n); q.tmax_test = a.in(tmax_test, n); }
+    if (any) q.occluded = a.out<uint32_t>(n);
+    else { q.t = a.out<float>(n); q.prim = a.out<uint32_t>(n); q.inst = a.out<uint32_t>(n); q.uv = a.out<float>(2 * (size_t)n); }
+    if (stats) q.stats = a.out<uint32_t>(3 * (size_t)n);
     const int r = launch_trace_query(lc_, ds_, bvh_.depth4, shape, kind, fma, q, stream_);
-    if (r == TQ_UNSUPPORTED) { for (void *p : bufs) cudaFree(p); throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "trace_query: the scene has no such traversal shape" }; }
-    if (r != 0) fail((cudaError_t)r);
-    auto get = [&](void *dst, const void *src, size_t bytes) { cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, stream_); if (e != cudaSuccess) fail(e); };
-    if (any) get(occluded, q.occluded, (size_t)n * 4);
-    else { get(t, q.t, (size_t)n * 4); get(prim, q.prim, (size_t)n * 4); get(inst, q.inst, (size_t)n * 4); get(uv, q.uv, (size_t)n * 8); }
-    if (stats) get(stats, q.stats, (size_t)n * 12);
-    const cudaError_t e = cudaStreamSynchronize(stream_);
-    for (void *p : bufs) cudaFree(p);
-    CK(e); CK(cudaGetLastError());
+    if (r == TQ_UNSUPPORTED) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "trace_query: the scene has no such traversal shape" };
+    CK((cudaError_t)r);
+    if (any) a.get(occluded, q.occluded, n);
+    else { a.get(t, q.t, n); a.get(prim, q.prim, n); a.get(inst, q.inst, n); a.get(uv, q.uv, 2 * (size_t)n); }
+    if (stats) a.get(stats, q.stats, 3 * (size_t)n);
+    a.sync();
 }
 void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, const uint32_t *prim, const float *uv, const float *dir, const float *org,
                          const float *pay_pdf, const uint32_t *rng, const float *L, float *out) {
@@ -1221,59 +1224,33 @@ void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, c
             throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: instance or primitive out of range" };
         gid[i] = h_instances_[inst[i]].tri_base + prim[i];
     }
-    std::vector<void *> bufs;
-    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
-    auto dev = [&](size_t bytes, const void *src) -> void * {
-        void *p = nullptr;
-        cudaError_t e = cudaMalloc(&p, bytes);
-        if (e != cudaSuccess) fail(e);
-        bufs.push_back(p);
-        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
-        return p;
-    };
+    HookArrays a(stream_);
     ShadeQuery q{};
     q.n = n; q.force_general = force_general;
-    q.gid = (const uint32_t *)dev((size_t)n * 4, gid.data()); q.rng = (const uint32_t *)dev((size_t)n * 4, rng);
-    q.uv = (const float *)dev((size_t)n * 8, uv); q.dir = (const float *)dev((size_t)n * 12, dir); q.org = (const float *)dev((size_t)n * 12, org);
-    q.pay_pdf = (const float *)dev((size_t)n * 4, pay_pdf);
-    if (L) q.L = (const float *)dev((size_t)n * 12, L);
-    const size_t out_bytes = (size_t)n * B200PT_SQ_STRIDE * sizeof(float);
-    q.out = (float *)dev(out_bytes, nullptr);
-    const int r = launch_shade_query(ds_, make_dev_config(), q, stream_);
-    if (r != 0) fail((cudaError_t)r);
-    cudaError_t e = cudaMemcpyAsync(out, q.out, out_bytes, cudaMemcpyDeviceToHost, stream_);
-    if (e != cudaSuccess) fail(e);
-    e = cudaStreamSynchronize(stream_);
-    for (void *p : bufs) cudaFree(p);
-    CK(e); CK(cudaGetLastError());
+    q.gid = a.in(gid.data(), n); q.rng = a.in(rng, n);
+    q.uv = a.in(uv, 2 * (size_t)n); q.dir = a.in(dir, 3 * (size_t)n); q.org = a.in(org, 3 * (size_t)n);
+    q.pay_pdf = a.in(pay_pdf, n);
+    if (L) q.L = a.in(L, 3 * (size_t)n);
+    const size_t out_count = (size_t)n * B200PT_SQ_STRIDE;
+    q.out = a.out<float>(out_count);
+    CK((cudaError_t)launch_shade_query(ds_, make_dev_config(), q, stream_));
+    a.get(out, q.out, out_count);
+    a.sync();
 }
 void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, const float *pay_pdf, float *out) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
     if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "miss_query: no environment map" };
     if (!n) return;
-    std::vector<void *> bufs;
-    auto fail = [&](cudaError_t e) { for (void *p : bufs) cudaFree(p); CK(e); };
-    auto dev = [&](size_t bytes, const void *src) -> void * {
-        void *p = nullptr;
-        cudaError_t e = cudaMalloc(&p, bytes);
-        if (e != cudaSuccess) fail(e);
-        bufs.push_back(p);
-        if (src && (e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, stream_)) != cudaSuccess) fail(e);
-        return p;
-    };
+    HookArrays a(stream_);
     MissQuery q{};
     q.n = n;
-    q.dir = (const float *)dev((size_t)n * 12, dir); q.depth = (const uint32_t *)dev((size_t)n * 4, depth); q.pay_pdf = (const float *)dev((size_t)n * 4, pay_pdf);
-    const size_t out_bytes = (size_t)n * B200PT_MQ_STRIDE * sizeof(float);
-    q.out = (float *)dev(out_bytes, nullptr);
-    const int r = launch_miss_query(ds_, make_dev_config(), q, stream_);
-    if (r != 0) fail((cudaError_t)r);
-    cudaError_t e = cudaMemcpyAsync(out, q.out, out_bytes, cudaMemcpyDeviceToHost, stream_);
-    if (e != cudaSuccess) fail(e);
-    e = cudaStreamSynchronize(stream_);
-    for (void *p : bufs) cudaFree(p);
-    CK(e); CK(cudaGetLastError());
+    q.dir = a.in(dir, 3 * (size_t)n); q.depth = a.in(depth, n); q.pay_pdf = a.in(pay_pdf, n);
+    const size_t out_count = (size_t)n * B200PT_MQ_STRIDE;
+    q.out = a.out<float>(out_count);
+    CK((cudaError_t)launch_miss_query(ds_, make_dev_config(), q, stream_));
+    a.get(out, q.out, out_count);
+    a.sync();
 }
 void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors) {
     CK(cudaSetDevice(device_));
@@ -1525,22 +1502,20 @@ void Engine::ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes
     *n_out = 0; *depth_out = 0; *n4_out = 0; *depth4_out = 0;
     for (size_t i = 0; i < (size_t)n; i++)
         for (int a = 0; a < 3; a++) if (!(ref_boxes[i * 6 + a] <= ref_boxes[i * 6 + 3 + a])) return;
-    struct Bufs { float *box = nullptr; BvhNode *nodes = nullptr; uint32_t *perm = nullptr; Bvh4Node *nodes4 = nullptr;
-                  ~Bufs() { dfree(box); dfree(nodes); dfree(perm); dfree(nodes4); } } b;
-    CK(cudaMalloc(&b.box, (size_t)n * 6 * sizeof(float))); CK(cudaMalloc(&b.nodes, (size_t)(n - 1) * sizeof(BvhNode))); CK(cudaMalloc(&b.perm, (size_t)n * 4));
-    CK(cudaMemcpyAsync(b.box, ref_boxes, (size_t)n * 6 * sizeof(float), cudaMemcpyHostToDevice, stream_));
+    HookArrays a(stream_);
+    const float *box = a.in(ref_boxes, (size_t)n * 6);
+    BvhNode *nodes = a.out<BvhNode>(n - 1); uint32_t *perm = a.out<uint32_t>(n);
     uint32_t n2 = 0; int d2 = 0;
-    int r = ploc_build(b.box, n, b.nodes, b.perm, &n2, &d2, h_small_, stream_);
+    int r = ploc_build(box, n, nodes, perm, &n2, &d2, h_small_, stream_);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("ploc_build failed: ") + cudaGetErrorString((cudaError_t)r) };
     if (n2 == 0) return;
-    CK(cudaMalloc(&b.nodes4, (size_t)n2 * sizeof(Bvh4Node)));
+    Bvh4Node *nodes4 = a.out<Bvh4Node>(n2);
     uint32_t n4 = 0; int d4 = 0;
-    r = bvh4_collapse_device(b.nodes, n2, 0, b.nodes4, &n4, &d4, h_small_, stream_);
+    r = bvh4_collapse_device(nodes, n2, 0, nodes4, &n4, &d4, h_small_, stream_);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("bvh4_collapse_device failed: ") + cudaGetErrorString((cudaError_t)r) };
-    CK(cudaMemcpyAsync(nodes_out, b.nodes, (size_t)n2 * sizeof(BvhNode), cudaMemcpyDeviceToHost, stream_));
-    CK(cudaMemcpyAsync(perm_out, b.perm, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
-    if (n4) CK(cudaMemcpyAsync(nodes4_out, b.nodes4, (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyDeviceToHost, stream_));
-    CK(cudaStreamSynchronize(stream_));
+    a.get(nodes_out, nodes, n2); a.get(perm_out, perm, n);
+    if (n4) a.get(nodes4_out, nodes4, n4);
+    a.sync();
     *n_out = n2; *depth_out = d2; *n4_out = n4; *depth4_out = d4;
 }
 

@@ -8,7 +8,7 @@ namespace b200pt {
 
 struct LaunchCfg {
     int grid_light;     // grid for streaming kernels (raygen / resolve / post)
-    int grid_trace;     // persistent grid for the ray-query test hook
+    int grid_volume_decide;   // persistent grid of k_volume_decide (256 threads per CTA)
     int grid_extend, grid_connect;   // persistent grids of the traversal kernels (SM count x resident CTAs of each kernel)
     int grid_shade;     // persistent grid for the shading kernel
     int max_stack;      // traversal stack entries (BVH depth + 2)
@@ -31,7 +31,7 @@ struct LaunchCfg {
     size_t smem_extend; // k_extend / k_extend_dyn, k_camera and the tracing k_connect (extend_threads per CTA)
     size_t smem_shadow; // k_shadow_dyn (256 threads, + its ray ring)
     size_t smem_bounce; // fused k_shade_hit (bounce_threads)
-    size_t smem_trace;  // k_trace_rays, k_volume_decide and k_features (256 threads)
+    size_t smem_trace;  // k_volume_decide and k_features (256 threads)
 };
 
 // Grids, CTA sizes and shared memory of every traversal launch for one scene, and the per-device shared-memory opt-in of every kernel the
@@ -102,8 +102,6 @@ void launch_resolve(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch
                     const float4 *sample_buf, float4 *image, cudaStream_t st);
 void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const float *dir, const uint32_t *seeds, float ray_depth,
                          float *T_out, float *scatter_out, int32_t *vol_out, uint32_t *rng_out, cudaStream_t st);
-int launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
-                      float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st);
 // Shared-memory stack entries of the BVH4 dynamic-fetch kernels for a BVH4 of the given depth with a shared column of at most `cap` entries
 // (the rest goes to the DYN_SPILL overflow array); 0 when even that cannot hold three pushes per level.
 constexpr int WIDE_STACK_DEFAULT = 24;

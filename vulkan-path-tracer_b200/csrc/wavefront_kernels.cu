@@ -1303,35 +1303,6 @@ __global__ void __launch_bounds__(256) k_adaptive_compact(const uint4 *__restric
 }
 
 // ------------------------------------------------------------------------------------------------
-// test hook: closest-hit for arbitrary rays (b200pt_trace_closest)
-// ------------------------------------------------------------------------------------------------
-template <bool SMEM>
-__global__ void __launch_bounds__(256) k_trace_rays(DevScene sc, uint32_t n, const float *__restrict__ org, const float *__restrict__ dir,
-                                                     float tmin, float tmax, float *t_out, uint32_t *prim_out, uint32_t *inst_out,
-                                                     float *uv_out, int max_stack, uint32_t *stats) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t bar;
-    int *stack = reinterpret_cast<int *>(smem) + threadIdx.x;
-    BvhView bv;
-    if (SMEM) bv = stage_bvh_smem(sc, smem + (size_t)max_stack * blockDim.x * sizeof(int), &bar);
-    else bv = global_bvh(sc);
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        HitRec h;
-        uint32_t nn = 0, nt = 0;
-        const bool f = stats ? bvh_trace<SMEM, false, true>(bv, f3(org[3 * i], org[3 * i + 1], org[3 * i + 2]), f3(dir[3 * i], dir[3 * i + 1], dir[3 * i + 2]),
-                                                            tmin, tmax, h, stack, (int)blockDim.x, max_stack, &nn, &nt)
-                             : bvh_trace<SMEM, false>(bv, f3(org[3 * i], org[3 * i + 1], org[3 * i + 2]), f3(dir[3 * i], dir[3 * i + 1], dir[3 * i + 2]),
-                                                      tmin, tmax, h, stack, (int)blockDim.x, max_stack);
-        if (stats) { stats[2 * i] = nn; stats[2 * i + 1] = nt; }
-        t_out[i] = f ? h.t : -1.0f;
-        uint32_t pi = 0xFFFFFFFFu, ii = 0xFFFFFFFFu;
-        if (f) { const float4 *tp = bv.tris + (size_t)h.slot * 3; ii = __float_as_uint(ld4<SMEM>(tp + 1).w); pi = __float_as_uint(ld4<SMEM>(tp + 2).w); }
-        prim_out[i] = pi; inst_out[i] = ii;
-        uv_out[2 * i] = f ? h.u : 0.0f; uv_out[2 * i + 1] = f ? h.v : 0.0f;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
 // kernel selectors: the instantiation each launch runs for its flags.  The launchers launch through them, and query_launch_cfg sizes the
 // grids of, checks big mode against and opts in the shared memory of exactly what they can return.
 // ------------------------------------------------------------------------------------------------
@@ -1366,7 +1337,6 @@ static auto connect_kernel(bool smem, bool trace, bool walks) {            // wi
     return walks ? k_connect<false, true, true> : k_connect<false, true, false>;
 }
 static auto volume_decide_kernel(bool smem) { return smem ? k_volume_decide<true> : k_volume_decide<false>; }
-static auto trace_rays_kernel(bool smem) { return smem ? k_trace_rays<true> : k_trace_rays<false>; }
 
 // ------------------------------------------------------------------------------------------------
 // launch configuration
@@ -1395,7 +1365,7 @@ static int opt_in_shared_memory() {
         const bool a = f & 1, b = f & 2, c = f & 4;
         optin(extend_kernel(a, b, c)); optin(extend_dyn_kernel(a, b, c)); optin(connect_kernel(a, b, c));
         optin(shadow_dyn_kernel(a, b)); optin(camera_kernel(a, b));
-        optin(volume_decide_kernel(a)); optin(trace_rays_kernel(a)); optin(features_kernel(a));
+        optin(volume_decide_kernel(a)); optin(features_kernel(a));
         for (uint32_t cls = 0; cls < MC_COUNT; cls++) optin(shade_kernel(cls, a, b));
     }
     cudaGetLastError();
@@ -1504,7 +1474,7 @@ int query_launch_cfg(const DevScene &sc, int bvh_max_depth, int bvh4_depth, Laun
     lc->grid_shade = sms * occ_s;
     lc->grid_bounce = sms * occ_b;
     lc->grid_camera = sms * std::max(1, occ_cam);
-    lc->grid_trace = sms * std::max(1, occupancy(trace_rays_kernel(smem), 256, lc->smem_trace));   // k_volume_decide runs on it too
+    lc->grid_volume_decide = sms * std::max(1, occupancy(volume_decide_kernel(smem), 256, lc->smem_trace));
     lc->grid_features = sms * std::max(1, occupancy(features_kernel(smem), 256, lc->smem_trace));
     lc->grid_light = sms * 8;
     if (getenv("B200PT_DEBUG"))
@@ -1581,7 +1551,7 @@ int launch_shade(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, co
 }
 int launch_volume_decide(const LaunchCfg &lc, const DevScene &sc, const DevConfig &cfg, PathState ps, ShadeOut so, const uint32_t *ctrl, uint32_t parity,
                          float4 *sample_buf, uint32_t *rng_carry, cudaStream_t st) {
-    volume_decide_kernel(lc.bvh_in_smem)<<<lc.grid_trace, 256, lc.smem_trace, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
+    volume_decide_kernel(lc.bvh_in_smem)<<<lc.grid_volume_decide, 256, lc.smem_trace, st>>>(sc, cfg, ps, so, ctrl, parity, lc.max_stack, sample_buf, rng_carry);
     return 1;
 }
 int launch_connect(const LaunchCfg &lc, const CallPlan &cp, const DevScene &sc, const DevConfig &cfg, PathState src, PathState dst, ShadeOut so,
@@ -1602,11 +1572,6 @@ void launch_resolve(const LaunchCfg &lc, const DevConfig &cfg, const DevDispatch
 void launch_volume_walks(const DevScene &sc, uint32_t n, const float *org, const float *dir, const uint32_t *seeds, float ray_depth,
                          float *T_out, float *scatter_out, int32_t *vol_out, uint32_t *rng_out, cudaStream_t st) {
     k_volume_walks<<<(n + 127u) / 128u, 128, 0, st>>>(sc, n, org, dir, seeds, ray_depth, T_out, scatter_out, vol_out, rng_out);
-}
-int launch_trace_rays(const LaunchCfg &lc, const DevScene &sc, uint32_t n, const float *org, const float *dir, float tmin, float tmax,
-                      float *t_out, uint32_t *prim_out, uint32_t *inst_out, float *uv_out, uint32_t *stats, cudaStream_t st) {
-    trace_rays_kernel(lc.bvh_in_smem)<<<lc.grid_trace, 256, lc.smem_trace, st>>>(sc, n, org, dir, tmin, tmax, t_out, prim_out, inst_out, uv_out, lc.max_stack, stats);
-    return 1;
 }
 
 } // namespace b200pt
