@@ -150,6 +150,33 @@ int32_t b200pt_mesh_vertex_count(b200pt_handle h, uint32_t mesh, uint32_t *out);
 int32_t b200pt_get_mesh_vertices(b200pt_handle h, uint32_t mesh, b200pt_vertex *out, uint32_t count);   /* count must equal the mesh's */
 int32_t b200pt_update_mesh_vertices(b200pt_handle h, const b200pt_mesh_update *updates, uint32_t n_updates,
                                     int32_t vertices_are_device, int32_t rebuild);
+/* ---- glTF animation: node animations, skins and morph targets posed on the GPU (no reference equivalent) ----
+ * A scene loaded from a glTF file keeps its node graph, skins (joints, inverseBindMatrices), the JOINTS_n / WEIGHTS_n sets and the morph
+ * targets (POSITION / NORMAL / TEXCOORD_0 deltas; TANGENT and COLOR_n are ignored) of its primitives, and its animations.  None of it changes
+ * what the load returns; malformed animation data never fails the load and is reported by the pose that needs it.
+ * b200pt_pose samples every channel of animation `animation` at `time` as glTF 2.0 Appendix C defines it (time clamped to each sampler's
+ * keys; STEP, LINEAR with slerp for rotations, CUBICSPLINE), in double rounded to float; animation == -1 is the rest pose (the nodes' own
+ * TRS, default morph weights: node.weights, else mesh.weights, else 0; skins applied).  Node world matrices use the loader's arithmetic, so a
+ * node no channel touches keeps its load-time instance transform bit for bit.  Skinned meshes follow the spec: the skinned node's transform
+ * is ignored, the vertices are posed in glTF world space (joint matrix = world(joint) x inverseBind) and their instances get the
+ * y flip diag(1, -1, 1, 1) as transform.  Vertices are computed from the rest data on the GPU, never from the previous pose, so a pose
+ * depends only on (file, animation, time).  Every instance transform and the vertices of every mesh some skin or morph target touches are
+ * replaced, whatever b200pt_update_instance_transforms / b200pt_update_mesh_vertices set before; other meshes keep theirs.  One tree update
+ * per pose, rebuild as in b200pt_update_instance_transforms; the pose waits for the waves in flight and resets the accumulation.
+ * WRONG_ARGUMENTS: an animation index out of range, a non-finite time, malformed animation data the pose needs (indices out of range, count
+ * mismatches, keys that do not increase, non-finite values, a non-finite posed vertex), or a mesh its instances would deform two ways
+ * (different skins or weights, or skinned and not); b200pt_last_error names the problem.  NO_SCENE without a scene, or for a scene without
+ * glTF node data (OBJ, b200pt_set_scene_arrays).  A rejected pose changes nothing; a failed update restores the previous state as
+ * b200pt_update_mesh_vertices does.  The image equals that of a handle loaded with the posed vertices and transforms. */
+int32_t b200pt_animation_count(b200pt_handle h, uint32_t *out);
+int32_t b200pt_get_animation(b200pt_handle h, uint32_t index, char *name, uint32_t name_len, float *t0, float *t1);   /* t0 / t1: first and last key time */
+int32_t b200pt_pose(b200pt_handle h, int32_t animation, float time, int32_t rebuild);
+/* host halves (test hooks, no GPU needed), on a glTF file: the animation count and, for index < count, its name and key range; and the
+ * pose's node world matrices (glTF world space, column-major, 16 floats per node) and per-node morph weights (weight_counts[node] floats each,
+ * concatenated in node order).  With world == NULL only node_count and weights_total are written. */
+int32_t b200pt_gltf_animation_info(const char *path, int32_t index, uint32_t *count, char *name, uint32_t name_len, float *t0, float *t1);
+int32_t b200pt_gltf_pose_nodes(const char *path, int32_t animation, float time, uint32_t *node_count, float *world, uint32_t *weight_counts,
+                               float *weights, uint32_t *weights_total);
 int32_t b200pt_set_camera(b200pt_handle h, const float view_inverse[16], const float projection_inverse[16]); /* SetCameraViewInverse/ProjectionInverse */
 int32_t b200pt_get_camera(b200pt_handle h, float view_inverse[16], float projection_inverse[16]);
 /* the Editor/FlyCamera round trip that produces the matrices the shader really sees (Editor.cpp:45-48,1042-1051; FlyCamera.cpp:84-140) */

@@ -112,4 +112,15 @@ def _post_block():                                                  # fresh hand
     T.set_hdr(hdr); T.post_process_rows(9, 20); T.get_ldr_rows(9, 20)
     print("post row block ok")
 _post_block()
+def _pose():                                                        # glTF pose: k_pose_vertices (palette in shared memory), k_pose_normals, refit
+    import tempfile, test_gltf_animation as ga
+    import vpt_b200 as pt
+    with tempfile.TemporaryDirectory() as d:
+        import pathlib
+        g, blobs, _ = ga.build_scene(); path = ga.write(pathlib.Path(d), g, blobs)
+        T = pt.PathTracer(0); T.set_scene_file(path); ga._configure(T); T.resize(40, 30)
+        T.path_trace(1, util.BASE_SEED); T.pose(1, 1.3); T.path_trace(1, util.BASE_SEED); T.pose(0, 0.7, rebuild="gpu")
+        assert np.isfinite(T.get_hdr()).all()
+    print("pose ok")
+_pose()
 print("sanitize_small done")

@@ -227,6 +227,11 @@ def lib():
             "b200pt_mesh_count": [C.c_void_p, C.POINTER(C.c_uint32)], "b200pt_mesh_vertex_count": [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)],
             "b200pt_get_mesh_vertices": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32],
             "b200pt_update_mesh_vertices": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.c_int32],
+            "b200pt_animation_count": [C.c_void_p, C.POINTER(C.c_uint32)],
+            "b200pt_get_animation": [C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_float), C.POINTER(C.c_float)],
+            "b200pt_pose": [C.c_void_p, C.c_int32, C.c_float, C.c_int32],
+            "b200pt_gltf_animation_info": [C.c_char_p, C.c_int32, C.POINTER(C.c_uint32), C.c_char_p, C.c_uint32, C.POINTER(C.c_float), C.POINTER(C.c_float)],
+            "b200pt_gltf_pose_nodes": [C.c_char_p, C.c_int32, C.c_float, C.POINTER(C.c_uint32), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)],
         }
         for name, args in sig.items():
             fn = getattr(L, name); fn.restype = C.c_int32; fn.argtypes = args
@@ -404,6 +409,32 @@ def load_gltf(path):
     return out
 
 
+def gltf_animations(path):
+    """b200pt_gltf_animation_info (host only): [(name, t0, t1)] of a glTF file's animations"""
+    L = lib(); n = C.c_uint32(); out = []
+    r = L.b200pt_gltf_animation_info(str(path).encode(), -1, C.byref(n), None, 0, None, None)
+    if r != OK: raise B200ptError(r, L.b200pt_last_error(None).decode(errors="replace"))
+    for i in range(n.value):
+        name = C.create_string_buffer(256); t0, t1 = C.c_float(), C.c_float()
+        r = L.b200pt_gltf_animation_info(str(path).encode(), i, C.byref(n), name, 256, C.byref(t0), C.byref(t1))
+        if r != OK: raise B200ptError(r, L.b200pt_last_error(None).decode(errors="replace"))
+        out.append((name.value.decode(errors="replace"), t0.value, t1.value))
+    return out
+
+
+def gltf_pose_nodes(path, animation, t):
+    """b200pt_gltf_pose_nodes (host only): (world [nodes, 16] column-major glTF world matrices, [per-node morph weights as float32 arrays])
+    of animation `animation` (-1: rest pose) at time t"""
+    L = lib(); n, nw = C.c_uint32(), C.c_uint32(); p = str(path).encode()
+    r = L.b200pt_gltf_pose_nodes(p, int(animation), C.c_float(t), C.byref(n), None, None, None, C.byref(nw))
+    if r != OK: raise B200ptError(r, L.b200pt_last_error(None).decode(errors="replace"))
+    world = np.zeros((n.value, 16), np.float32); counts = np.zeros(n.value, np.uint32); w = np.zeros(max(nw.value, 1), np.float32)
+    r = L.b200pt_gltf_pose_nodes(p, int(animation), C.c_float(t), C.byref(n), _p(world), _p(counts), _p(w), C.byref(nw))
+    if r != OK: raise B200ptError(r, L.b200pt_last_error(None).decode(errors="replace"))
+    offs = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    return world, [w[offs[i]:offs[i + 1]].copy() for i in range(n.value)]
+
+
 class PathTracer:
     """One GPU: the reference's PathTracer + PostProcessor behind the C-ABI."""
 
@@ -556,6 +587,21 @@ class PathTracer:
             import torch
             torch.cuda.current_stream(self.device).synchronize()
         self._ck(self.L.b200pt_update_mesh_vertices(self.h, C.addressof(ups), len(items), 1 if any(on_dev) else 0, mode))
+
+    # ---- glTF animation (no reference equivalent): node animations, skins and morph targets posed on the GPU
+    def animations(self):
+        """[(name, t0, t1)] of the loaded glTF scene's animations"""
+        n = C.c_uint32(); self._ck(self.L.b200pt_animation_count(self.h, C.byref(n))); out = []
+        for i in range(n.value):
+            name = C.create_string_buffer(256); t0, t1 = C.c_float(), C.c_float()
+            self._ck(self.L.b200pt_get_animation(self.h, i, name, 256, C.byref(t0), C.byref(t1)))
+            out.append((name.value.decode(errors="replace"), t0.value, t1.value))
+        return out
+
+    def pose(self, animation, t, rebuild=False):
+        """b200pt_pose: animation `animation` (-1: the rest pose) at time t; rebuild as update_instance_transforms"""
+        mode = self._rebuild_mode(rebuild)
+        self._ck(self.L.b200pt_pose(self.h, int(animation), C.c_float(t), mode))
 
     def bvh2_ploc_build_query(self, ref_boxes):
         """b200pt_bvh2_ploc_build_query: the GPU builder and the GPU BVH4 collapse on reference boxes [n, 6] in the given order.

@@ -6,6 +6,8 @@
 #include <cstring>
 #include <cstdlib>
 #include <new>
+#include <cmath>
+#include <functional>
 
 using namespace b200pt;
 
@@ -150,6 +152,26 @@ int32_t b200pt_update_mesh_vertices(b200pt_handle h, const b200pt_mesh_update *u
     if (!updates || n_updates == 0) return B200PT_ERR_WRONG_ARGUMENTS;
     return guard(h, [&](Engine &e) { e.update_mesh_vertices(updates, n_updates, vertices_are_device != 0, rebuild); });
 }
+static const HostAnimation &animation_of(Engine &e) {
+    if (!e.has_scene()) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!e.scene().animation) throw CudaError{ B200PT_ERR_NO_SCENE, "the scene has no glTF node data (loaded from OBJ or set through arrays)" };
+    return *e.scene().animation;
+}
+static void copy_name(const std::string &s, char *buf, uint32_t n) { if (buf && n) { strncpy(buf, s.c_str(), n - 1); buf[n - 1] = 0; } }
+int32_t b200pt_animation_count(b200pt_handle h, uint32_t *out) {
+    if (!out) return B200PT_ERR_WRONG_ARGUMENTS;
+    return guard(h, [&](Engine &e) { *out = (uint32_t)animation_of(e).clips.size(); });
+}
+int32_t b200pt_get_animation(b200pt_handle h, uint32_t index, char *name, uint32_t name_len, float *t0, float *t1) {
+    return guard(h, [&](Engine &e) {
+        const HostAnimation &a = animation_of(e);
+        if (index >= a.clips.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "animation index out of range" };
+        copy_name(a.clips[index].name, name, name_len);
+        if (t0) *t0 = a.clips[index].t0;
+        if (t1) *t1 = a.clips[index].t1;
+    });
+}
+int32_t b200pt_pose(b200pt_handle h, int32_t animation, float time, int32_t rebuild) { return guard(h, [&](Engine &e) { e.pose(animation, time, rebuild); }); }
 int32_t b200pt_set_camera(b200pt_handle h, const float vi[16], const float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.set_camera(vi, pi); }); }
 int32_t b200pt_get_camera(b200pt_handle h, float vi[16], float pi[16]) { if (!vi || !pi) return B200PT_ERR_WRONG_ARGUMENTS; return guard(h, [&](Engine &e) { e.get_camera(vi, pi); }); }
 int32_t b200pt_camera_from_view(const float view[16], float aspect, float vi[16], float pi[16]) {
@@ -190,6 +212,51 @@ int32_t b200pt_prepare_density_grid(const b200pt_density_grid *g, float *values,
         *max_density = p.max_density;
         return B200PT_OK;
     } catch (const CudaError &e) { return e.code; } catch (...) { return B200PT_ERR_UNKNOWN; }
+}
+static int32_t host_hook(const std::function<void()> &f) {       // the error text goes to b200pt_last_error(NULL)
+    try { f(); return B200PT_OK; }
+    catch (const CudaError &e) { g_err = e.what; return e.code < 0 ? e.code : B200PT_ERR_UNKNOWN; }
+    catch (const std::bad_alloc &) { g_err = "host out of memory"; return B200PT_ERR_OUT_OF_MEMORY; }
+    catch (...) { g_err = "unknown error"; return B200PT_ERR_UNKNOWN; }
+}
+static void load_for_hook(const char *path, HostScene &sc) {
+    std::string err;
+    if (!load_scene_file(path, sc, err)) throw CudaError{ B200PT_ERR_INIT_FAILED, "Failed to import scene: " + err };
+    if (!sc.animation) throw CudaError{ B200PT_ERR_NO_SCENE, "the scene has no glTF node data" };
+}
+int32_t b200pt_gltf_animation_info(const char *path, int32_t index, uint32_t *count, char *name, uint32_t name_len, float *t0, float *t1) {
+    if (!path || !count) return B200PT_ERR_WRONG_ARGUMENTS;
+    return host_hook([&] {
+        HostScene sc; load_for_hook(path, sc);
+        const auto &clips = sc.animation->clips;
+        *count = (uint32_t)clips.size();
+        if (index < 0) return;
+        if ((size_t)index >= clips.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "animation index out of range" };
+        copy_name(clips[index].name, name, name_len);
+        if (t0) *t0 = clips[index].t0;
+        if (t1) *t1 = clips[index].t1;
+    });
+}
+int32_t b200pt_gltf_pose_nodes(const char *path, int32_t animation, float time, uint32_t *node_count, float *world, uint32_t *weight_counts,
+                               float *weights, uint32_t *weights_total) {
+    if (!path || !node_count || !weights_total) return B200PT_ERR_WRONG_ARGUMENTS;
+    return host_hook([&] {
+        HostScene sc; load_for_hook(path, sc);
+        const HostAnimation &a = *sc.animation;
+        if (animation < -1 || animation >= (int)a.clips.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "animation index out of range" };
+        if (!std::isfinite(time)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "time is not finite" };
+        HostPose P; evaluate_pose(a, sc, animation, time, P);
+        *node_count = (uint32_t)P.world.size();
+        size_t nw = 0; for (const auto &w : P.weights) nw += w.size();
+        *weights_total = (uint32_t)nw;
+        if (!world) return;
+        for (size_t i = 0; i < P.world.size(); i++) m4_to_colmajor(P.world[i], world + i * 16);
+        size_t o = 0;
+        for (size_t i = 0; i < P.weights.size(); i++) {
+            if (weight_counts) weight_counts[i] = (uint32_t)P.weights[i].size();
+            if (weights) for (float x : P.weights[i]) weights[o++] = x;
+        }
+    });
 }
 int32_t b200pt_default_atmosphere(b200pt_atmosphere *a) {          // PathTracer.h:221-232
     if (!a) return B200PT_ERR_WRONG_ARGUMENTS;

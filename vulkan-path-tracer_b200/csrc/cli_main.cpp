@@ -60,13 +60,15 @@ static void usage() {
         "  --checkpoint FILE save the accumulation when done         --resume FILE  continue from a checkpoint\n"
         "  --preview-every K rewrite the output PNG after every K PathTrace calls (the editor's progressive view, Editor.cpp:83-121)\n"
         "  --bake-luts N     bake missing lookup tables into DIR with N samples per texel first (Application.cpp:35-72)\n"
+        "  --animation I --time T   pose the glTF scene at time T of animation I (-1: the rest pose) before rendering (b200pt_pose,\n"
+        "                    the tree set_scene builds)\n"
         "  --device K        CUDA device ordinal (default 0)         --quiet\n");
 }
 
 int main(int argc, char **argv) {
     std::string scene, env, luts, out, ckpt_out, ckpt_in;
     uint32_t W = 0, H = 0, spp = 64, depth = 200, seed = 0x1234ABCDu, chunks = 1, batch = 8, bake = 0, phase = 0, preview = 0;
-    int device = 0; bool quiet = false, atmosphere = false, sky = false; float sky_az = 0.0f, sky_al = 0.0f, sun[3] = { 1.0f, 1.0f, 1.0f };
+    int device = 0, animation = -2; float anim_time = 0.0f; bool quiet = false, atmosphere = false, sky = false; float sky_az = 0.0f, sky_al = 0.0f, sun[3] = { 1.0f, 1.0f, 1.0f };
     b200pt_tonemap tm{ 1.0f, 2.2f }; b200pt_bloom bl{ 2.0f, 1.0f, 10, 5.0f };
     std::vector<b200pt_volume> vols;
     b200pt_adaptive adaptive; b200pt_default_adaptive(&adaptive);
@@ -107,6 +109,8 @@ int main(int argc, char **argv) {
         }
         else if (a == "--checkpoint") { need(1); ckpt_out = argv[++i]; } else if (a == "--resume") { need(1); ckpt_in = argv[++i]; }
         else if (a == "--bake-luts") { need(1); bake = (uint32_t)atoi(argv[++i]); } else if (a == "--device") { need(1); device = atoi(argv[++i]); }
+        else if (a == "--animation") { need(1); animation = atoi(argv[++i]); if (animation < -1) { usage(); return 2; } }
+        else if (a == "--time") { need(1); anim_time = (float)atof(argv[++i]); }
         else if (a == "--quiet") quiet = true;
         else { usage(); return 2; }
     }
@@ -118,6 +122,7 @@ int main(int argc, char **argv) {
     CALL(b200pt_set_luts_dir(h, luts.c_str()));
     CALL(b200pt_set_env_map_file(h, env.c_str()));
     CALL(b200pt_set_scene_file(h, scene.c_str()));                         // also sizes the image to 1080*aspect x 1080 and installs the scene camera
+    if (animation >= -1) CALL(b200pt_pose(h, animation, anim_time, 1));
     if (W && H) CALL(b200pt_resize(h, W, H));
     CALL(b200pt_get_size(h, &W, &H));
     b200pt_config cfg; CALL(b200pt_get_config(h, &cfg));

@@ -123,6 +123,7 @@ void Engine::free_scene() {
     for (auto &p : d_texdata_) if (p) cudaFree(p);
     d_texdata_.clear();
     lbvh_free(&bvh_); lbvh_refit_free(&refit_);
+    free_pose_data();
     has_scene_ = false;
 }
 
@@ -185,6 +186,7 @@ void Engine::upload_scene() {
     rebuild_tri_class();
     ds_.textures = d_textures_; ds_.emissive = d_emissive_;
     build_bvh(&bvh_, &ds_, &lc_);
+    upload_pose_data();
 }
 
 // DevInstance of every instance from scene_.instances (o2w = rows 0-2 of the column-major Transform, w2o its inverse); emissive_tri_count is
@@ -256,31 +258,9 @@ void Engine::update_instance_transforms(const float *xf, uint32_t count, int reb
     if (!xf || count != scene_.instances.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform count differs from the instance count" };
     for (size_t i = 0; i < (size_t)count * 16; i++) if (!std::isfinite(xf[i])) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "transform entry is not finite" };
     sync_all();                                                 // the waves in flight neither read a half-updated tree nor resolve into the new accumulation
-    std::vector<b200pt_instance> old = scene_.instances;
-    auto apply = [&](const std::vector<b200pt_instance> &inst) {
-        scene_.instances = inst;
-        fill_instances();
-        rebuild_emissive();                                     // DevEmissive::xf, the world-space EmTri, and d_instances_ (o2w / w2o)
-    };
-    std::vector<b200pt_instance> moved = old;
+    std::vector<b200pt_instance> moved = scene_.instances;
     for (uint32_t i = 0; i < count; i++) memcpy(moved[i].Transform, xf + (size_t)i * 16, sizeof moved[i].Transform);
-    apply(moved);
-    if (!rebuild) {
-        auto refit = [&]() { return lbvh_refit(&bvh_, &refit_, d_verts_, d_indices_, d_meshes_, d_instances_, (uint32_t)h_instances_.size(), stream_); };
-        const int r = refit();
-        if (r != 0) {                                           // back to the previous transforms, and the tree refit to them
-            apply(old);
-            if (refit() != 0) has_scene_ = false;               // the tree matches neither: no render until set_scene
-            throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refit failed: ") + cudaGetErrorString((cudaError_t)r) };
-        }
-    } else {
-        LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
-        try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
-        catch (...) { lbvh_free(&fresh); apply(old); throw; }
-        lbvh_free(&bvh_); lbvh_refit_free(&refit_);
-        bvh_ = fresh; ds_ = ds; lc_ = lc;
-    }
-    reset();
+    commit({}, &moved, rebuild);
 }
 
 // Mesh vertex update (no reference equivalent): the whole vertex array of each listed mesh replaced in d_verts_ and in the host mirror
@@ -308,6 +288,7 @@ void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool 
             for (size_t k = 0; k < (size_t)u[i].vertex_count * VF; k++) if (!std::isfinite(f[k])) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex component is not finite" };
         }
     sync_all();                                                 // the waves in flight neither read half-updated records nor resolve into the new accumulation
+    std::vector<VertexSource> src(n);
     b200pt_vertex *stage = nullptr;                             // device input: [update 0 | update 1 | ... | flag word]
     if (device) {
         stage = static_cast<b200pt_vertex *>(scratch(total * VB + 16));
@@ -319,34 +300,51 @@ void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool 
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("any_nonfinite failed: ") + cudaGetErrorString((cudaError_t)r) };
         if (bad) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex component is not finite" };
     }
-    std::vector<std::vector<b200pt_vertex>> old(n);
-    for (uint32_t i = 0; i < n; i++) old[i] = scene_.meshes[u[i].mesh].vertices;
+    size_t o = 0;
+    for (uint32_t i = 0; i < n; o += u[i].vertex_count, i++) src[i] = { u[i].mesh, device ? stage + o : u[i].vertices, device };
+    commit(src, nullptr, rebuild);
+}
+
+// The listed vertex arrays replaced in d_verts_ and the host mirror scene_.meshes, and (instances != nullptr) every instance transform replaced
+// (d_instances_ / h_instances_ through fill_instances); the emissive records rebuilt from the mirror; then the tree refit in place, with the
+// shading records of the changed meshes' instances rewritten (rebuild == 0), built on the device (B200PT_REBUILD_GPU) or as set_scene would
+// build it (any other value); then ResetPathTracing.  The caller has checked everything and synchronised the waves in flight.  A failure
+// restores the previous vertices and transforms: a failed rebuild keeps the previous tree, a failed refit refits the tree back to them (and if
+// that fails too, the handle has no scene until the next set_scene).
+void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200pt_instance> *instances, int rebuild) {
+    constexpr size_t VB = sizeof(b200pt_vertex);
+    std::vector<uint8_t> listed(scene_.meshes.size(), 0);
+    for (const VertexSource &s : src) listed[s.mesh] = 1;
+    std::vector<std::vector<b200pt_vertex>> old(src.size());
+    for (size_t i = 0; i < src.size(); i++) old[i] = scene_.meshes[src[i].mesh].vertices;
+    const std::vector<b200pt_instance> old_instances = instances ? scene_.instances : std::vector<b200pt_instance>();
     auto restore = [&]() {
-        for (uint32_t i = 0; i < n; i++) {
-            std::vector<b200pt_vertex> &mv = scene_.meshes[u[i].mesh].vertices;
+        for (size_t i = 0; i < src.size(); i++) {
+            std::vector<b200pt_vertex> &mv = scene_.meshes[src[i].mesh].vertices;
             mv = old[i];
-            if (!mv.empty()) CK(cudaMemcpyAsync(d_verts_ + h_meshes_[u[i].mesh].vbase, mv.data(), mv.size() * VB, cudaMemcpyHostToDevice, stream_));
+            if (!mv.empty()) CK(cudaMemcpyAsync(d_verts_ + h_meshes_[src[i].mesh].vbase, mv.data(), mv.size() * VB, cudaMemcpyHostToDevice, stream_));
         }
+        if (instances) { scene_.instances = old_instances; fill_instances(); }
         CK(cudaStreamSynchronize(stream_));
-        rebuild_emissive();
+        rebuild_emissive();                                     // DevEmissive::xf, the world-space EmTri, and d_instances_ (o2w / w2o)
     };
     try {
-        size_t o = 0;
-        for (uint32_t i = 0; i < n; o += u[i].vertex_count, i++) {
-            std::vector<b200pt_vertex> &mv = scene_.meshes[u[i].mesh].vertices;
-            b200pt_vertex *dst = d_verts_ + h_meshes_[u[i].mesh].vbase;
+        for (const VertexSource &s : src) {
+            std::vector<b200pt_vertex> &mv = scene_.meshes[s.mesh].vertices;
+            b200pt_vertex *dst = d_verts_ + h_meshes_[s.mesh].vbase;
             const size_t bytes = mv.size() * VB;
             if (!bytes) continue;
-            if (device) {
-                CK(cudaMemcpyAsync(dst, stage + o, bytes, cudaMemcpyDeviceToDevice, stream_));
-                CK(cudaMemcpyAsync(mv.data(), stage + o, bytes, cudaMemcpyDeviceToHost, stream_));   // the mirror: the updated ranges only
+            if (s.device) {
+                CK(cudaMemcpyAsync(dst, s.data, bytes, cudaMemcpyDeviceToDevice, stream_));
+                CK(cudaMemcpyAsync(mv.data(), s.data, bytes, cudaMemcpyDeviceToHost, stream_));   // the mirror: the updated ranges only
             } else {
-                memcpy(mv.data(), u[i].vertices, bytes);
+                memcpy(mv.data(), s.data, bytes);
                 CK(cudaMemcpyAsync(dst, mv.data(), bytes, cudaMemcpyHostToDevice, stream_));
             }
         }
+        if (instances) { scene_.instances = *instances; fill_instances(); }
         CK(cudaStreamSynchronize(stream_));
-        rebuild_emissive();                                     // the world-space EmTri, from the mirror
+        rebuild_emissive();                                     // the world-space EmTri, from the mirror; d_instances_
     } catch (...) {
         try { restore(); } catch (...) { has_scene_ = false; }
         throw;
@@ -354,15 +352,16 @@ void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool 
     if (!rebuild) {
         std::vector<uint32_t> changed;                          // instances of the updated meshes: their shading records are rewritten
         for (size_t a = 0; a < h_instances_.size(); a++) if (listed[h_instances_[a].mesh]) changed.push_back((uint32_t)a);
-        uint32_t *const d_list = static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
+        uint32_t *const d_list = src.empty() ? nullptr : static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
         auto refit = [&]() {
             int r = lbvh_refit(&bvh_, &refit_, d_verts_, d_indices_, d_meshes_, d_instances_, (uint32_t)h_instances_.size(), stream_);
-            if (r == 0) r = lbvh_refresh_shade(&bvh_, d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), changed.data(),
-                                               (uint32_t)changed.size(), d_list, stream_);
+            if (r == 0 && !src.empty())
+                r = lbvh_refresh_shade(&bvh_, d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), changed.data(),
+                                       (uint32_t)changed.size(), d_list, stream_);
             return r;
         };
         const int r = refit();
-        if (r != 0) {                                           // back to the previous vertices, and the tree refit to them
+        if (r != 0) {                                           // back to the previous state, and the tree refit to it
             try { restore(); if (refit() != 0) has_scene_ = false; } catch (...) { has_scene_ = false; }
             throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refit failed: ") + cudaGetErrorString((cudaError_t)r) };
         }
@@ -374,6 +373,103 @@ void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool 
         bvh_ = fresh; ds_ = ds; lc_ = lc;
     }
     reset();
+}
+
+// The rest data of the deformable meshes (HostAnimation::deformable), in device memory until the next set_scene: rest vertices, joints and
+// weights of every set, morph deltas as planes (PoseMesh), the last face of each vertex of generated-normal meshes, and room for one pose's
+// joint palettes and morph weights.  Scenes without deformable meshes allocate nothing.
+void Engine::upload_pose_data() {
+    pose_meshes_.clear(); pose_grid_ = pose_max_joints_ = pose_vertices_ = pose_palette_floats_ = pose_morph_floats_ = 0; pose_gen_normals_ = false;
+    if (!scene_.animation || scene_.animation->deformable.empty()) return;
+    const HostAnimation &A = *scene_.animation;
+    size_t nv = 0, njw = 0, ndelta = 0;
+    std::vector<uint32_t> block_mesh;
+    for (int p : A.deformable) {
+        const AnimPrim &ap = A.prims[p];
+        PoseMesh m{};
+        const int skin = A.prim_skin[p];
+        const bool ok = ap.err.empty() && !ap.rest.empty();    // a mesh with bad data is never posed (evaluate_pose rejects it): no rest data
+        m.vbase = (uint32_t)nv; m.count = ok ? ap.count : 0; m.block0 = (uint32_t)block_mesh.size();
+        m.flags = (skin >= 0 ? POSE_SKINNED : 0) | (!ap.dpos.empty() ? POSE_DPOS : 0) | (!ap.dnrm.empty() ? POSE_DNRM : 0) | (!ap.duv.empty() ? POSE_DUV : 0) |
+                  (ap.gen_normals ? POSE_GEN_NORMALS : 0);
+        m.sets = skin >= 0 ? ap.sets : 0; m.jw_base = (uint32_t)njw;
+        m.n_joints = skin >= 0 ? (uint32_t)A.skins[skin].joints.size() : 0; m.palette_base = pose_palette_floats_ / 12;
+        m.targets = ap.targets; m.morph_base = pose_morph_floats_; m.ibase = h_meshes_[p].ibase; m.delta_base = ndelta;
+        pose_meshes_.push_back(m);
+        for (uint32_t b = 0; b < (m.count + POSE_BLOCK - 1) / POSE_BLOCK; b++) block_mesh.push_back((uint32_t)pose_meshes_.size() - 1);
+        nv += m.count; njw += (size_t)m.count * 4 * m.sets; ndelta += (size_t)m.count * 8 * (m.flags & (POSE_DPOS | POSE_DNRM | POSE_DUV) ? m.targets : 0);
+        pose_palette_floats_ += m.n_joints * 12; pose_morph_floats_ += m.targets;
+        pose_max_joints_ = std::max(pose_max_joints_, m.n_joints);
+        if (m.flags & POSE_GEN_NORMALS) pose_gen_normals_ = true;
+    }
+    if (nv > 0xFFFFFFFFull / 8) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "too many deformable vertices" };
+    std::vector<float> rest(nv * 8), weights(njw), deltas(ndelta, 0.0f);
+    std::vector<uint32_t> joints(njw), last_face(nv, UINT32_MAX);
+    for (size_t d = 0; d < pose_meshes_.size(); d++) {
+        const PoseMesh &m = pose_meshes_[d]; const AnimPrim &ap = A.prims[A.deformable[d]];
+        if (!m.count) continue;
+        std::copy(ap.rest.begin(), ap.rest.end(), rest.begin() + (size_t)m.vbase * 8);
+        if (m.sets) { std::copy(ap.joints.begin(), ap.joints.end(), joints.begin() + m.jw_base); std::copy(ap.weights.begin(), ap.weights.end(), weights.begin() + m.jw_base); }
+        if (m.flags & POSE_GEN_NORMALS) std::copy(ap.last_face.begin(), ap.last_face.end(), last_face.begin() + m.vbase);
+        struct { uint32_t flag, c0, nc; const std::vector<float> *src; } planes[3] = { { POSE_DPOS, 0, 3, &ap.dpos }, { POSE_DNRM, 3, 3, &ap.dnrm }, { POSE_DUV, 6, 2, &ap.duv } };
+        for (auto &P : planes) if (m.flags & P.flag)
+            for (uint32_t t = 0; t < m.targets; t++) for (uint32_t c = 0; c < P.nc; c++) for (uint32_t i = 0; i < m.count; i++)
+                deltas[m.delta_base + ((size_t)t * 8 + P.c0 + c) * m.count + i] = (*P.src)[((size_t)t * m.count + i) * P.nc + c];
+    }
+    auto up = [&](const void *src, size_t bytes) -> void * {
+        void *p = nullptr;
+        d_pose_blocks_.push_back(nullptr);
+        CK(cudaMalloc(&p, std::max<size_t>(bytes, 16))); d_pose_blocks_.back() = p;
+        if (src && bytes) CK(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice));
+        return p;
+    };
+    pose_dev_.meshes = static_cast<const PoseMesh *>(up(pose_meshes_.data(), pose_meshes_.size() * sizeof(PoseMesh)));
+    pose_dev_.block_mesh = static_cast<const uint32_t *>(up(block_mesh.data(), block_mesh.size() * 4));
+    pose_dev_.rest = static_cast<const float *>(up(rest.data(), rest.size() * 4));
+    pose_dev_.joints = static_cast<const uint32_t *>(up(joints.data(), joints.size() * 4));
+    pose_dev_.weights = static_cast<const float *>(up(weights.data(), weights.size() * 4));
+    pose_dev_.deltas = static_cast<const float *>(up(deltas.data(), deltas.size() * 4));
+    pose_dev_.last_face = static_cast<const uint32_t *>(up(pose_gen_normals_ ? last_face.data() : nullptr, pose_gen_normals_ ? last_face.size() * 4 : 0));
+    pose_dev_.indices = d_indices_;
+    pose_dev_.palette = static_cast<const float *>(up(nullptr, (size_t)pose_palette_floats_ * 4));
+    pose_dev_.morph = static_cast<const float *>(up(nullptr, (size_t)pose_morph_floats_ * 4));
+    pose_grid_ = (uint32_t)block_mesh.size(); pose_vertices_ = (uint32_t)nv;
+}
+
+void Engine::free_pose_data() {
+    for (void *p : d_pose_blocks_) if (p) cudaFree(p);
+    d_pose_blocks_.clear(); pose_dev_ = PoseDev{}; pose_meshes_.clear(); pose_grid_ = pose_vertices_ = 0;
+}
+
+// glTF pose (DESIGN §15): arguments checked, the waves in flight finished, the pose evaluated on the host (animation.cpp), its joint
+// palettes and morph weights uploaded, the deformable meshes' vertices posed from the rest data into the staging buffer and checked there,
+// then committed with every instance transform and one refit / rebuild.  A rejected pose changes nothing.
+void Engine::pose(int animation, float t, int rebuild) {
+    CK(cudaSetDevice(device_));
+    if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
+    if (!scene_.animation) throw CudaError{ B200PT_ERR_NO_SCENE, "the scene has no glTF node data (loaded from OBJ or set through arrays)" };
+    if (animation < -1 || animation >= (int)scene_.animation->clips.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "animation index out of range" };
+    if (!std::isfinite(t)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "time is not finite" };
+    sync_all();
+    HostPose P;
+    evaluate_pose(*scene_.animation, scene_, animation, t, P);
+    std::vector<VertexSource> src;
+    if (pose_vertices_) {
+        if (P.palette.size() != pose_palette_floats_ || P.morph.size() != pose_morph_floats_) throw CudaError{ B200PT_ERR_UNKNOWN, "pose layout mismatch" };
+        b200pt_vertex *stage = static_cast<b200pt_vertex *>(scratch((size_t)pose_vertices_ * sizeof(b200pt_vertex) + 16));
+        uint32_t *flag = reinterpret_cast<uint32_t *>(stage + pose_vertices_);
+        if (!P.palette.empty()) CK(cudaMemcpyAsync(const_cast<float *>(pose_dev_.palette), P.palette.data(), P.palette.size() * 4, cudaMemcpyHostToDevice, stream_));
+        if (!P.morph.empty()) CK(cudaMemcpyAsync(const_cast<float *>(pose_dev_.morph), P.morph.data(), P.morph.size() * 4, cudaMemcpyHostToDevice, stream_));
+        CK(cudaMemsetAsync(flag, 0, 4, stream_));
+        const int r = launch_pose(pose_dev_, pose_grid_, pose_max_joints_, pose_gen_normals_, stage, flag, stream_);
+        if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("launch_pose failed: ") + cudaGetErrorString((cudaError_t)r) };
+        CK(cudaMemcpyAsync(h_small_, flag, 4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));                     // also: P's host arrays are no longer read
+        if (h_small_[0]) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "a posed vertex component is not finite" };
+        for (size_t d = 0; d < pose_meshes_.size(); d++)
+            src.push_back({ (uint32_t)scene_.animation->deformable[d], stage + pose_meshes_[d].vbase, true });
+    }
+    commit(src, &P.instances, rebuild);
 }
 
 // 1x1 textures (the defaults of PathTracer.cpp:1557-1621, or any constant texture) are resolved to their texel value here

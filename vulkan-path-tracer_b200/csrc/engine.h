@@ -26,6 +26,9 @@ public:
     void update_instance_transforms(const float *transforms, uint32_t count, int rebuild);
     // the whole vertex array of each listed mesh (host or device memory), one refit / rebuild for the batch; rebuild as above
     void update_mesh_vertices(const b200pt_mesh_update *updates, uint32_t n, bool device, int rebuild);
+    // glTF pose (DESIGN §15): the scene's nodes, skins and morph targets at time t of an animation (-1: the rest pose); the posed vertices of
+    // the deformable meshes and every instance transform committed with one refit / rebuild (rebuild as above)
+    void pose(int animation, float t, int rebuild);
     // PathTracer::AddVolume / SetVolume / RemoveVolume / SetPhaseFunction / AddDensityDataToVolume / RemoveDensityDataFromVolume (volumes.cuh)
     uint32_t add_volume(const b200pt_volume &v);
     void set_volume(uint32_t idx, const b200pt_volume &v);
@@ -159,8 +162,20 @@ private:
     LbvhResult bvh_{};
     LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
     uint32_t *h_small_ = nullptr;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
-    void *d_scratch_ = nullptr; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices
+    void *d_scratch_ = nullptr; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices and pose
     void *scratch(size_t bytes);
+    // the commit of update_instance_transforms, update_mesh_vertices and pose: the listed meshes' whole vertex arrays (host memory, or device
+    // memory on the stream) and, when given, every instance transform; one refit / rebuild; ResetPathTracing.  A failure restores both.
+    struct VertexSource { uint32_t mesh; const b200pt_vertex *data; bool device; };
+    void commit(const std::vector<VertexSource> &src, const std::vector<b200pt_instance> *instances, int rebuild);
+    // rest data of the deformable meshes of a glTF scene (pose_kernels.cu), uploaded by set_scene; nothing for other scenes
+    void upload_pose_data();
+    void free_pose_data();
+    std::vector<void *> d_pose_blocks_;             // every device allocation behind pose_dev_
+    PoseDev pose_dev_{};
+    std::vector<PoseMesh> pose_meshes_;             // HostAnimation::deformable order
+    uint32_t pose_grid_ = 0, pose_max_joints_ = 0, pose_vertices_ = 0, pose_palette_floats_ = 0, pose_morph_floats_ = 0;
+    bool pose_gen_normals_ = false;
     LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
     uint8_t *d_tri_class_ = nullptr; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c

@@ -189,6 +189,31 @@ int lbvh_refresh_shade(LbvhResult *r, const b200pt_vertex *d_verts, const uint32
 // *any = some float of d_v[0, n) is not finite.  d_flag: one device word of scratch; h_small: pinned host word for the readback.  Returns cudaError_t as int.
 int any_nonfinite(const float *d_v, size_t n, uint32_t *d_flag, uint32_t *h_small, cudaStream_t st, bool *any);
 
+// ---- glTF pose (pose_kernels.cu): skinned / morphed vertices from the rest data, written as b200pt_vertex records ----
+// One descriptor per deformable mesh.  Its vertices are [vbase, vbase + count) of the rest data and of the output; its blocks of
+// POSE_BLOCK threads start at block0.  Morph deltas are planes of count floats: for target t, plane (delta_base + (t * 8 + c) * count),
+// c = 0..2 position, 3..5 normal, 6..7 uv.  Joints / weights: [vertex][4 * sets] from jw_base.
+constexpr uint32_t POSE_BLOCK = 256;
+constexpr uint32_t POSE_SMEM_JOINTS = 512;          // joint palettes up to this size are staged in shared memory (48 B per joint)
+enum PoseFlags : uint32_t { POSE_SKINNED = 1, POSE_DPOS = 2, POSE_DNRM = 4, POSE_DUV = 8, POSE_GEN_NORMALS = 16 };
+struct PoseMesh {
+    uint32_t vbase, count, block0, flags;
+    uint32_t sets, jw_base, n_joints, palette_base;   // palette_base: first joint of the mesh's palette (12 floats each)
+    uint32_t targets, morph_base, ibase, _pad;        // morph_base: first weight; ibase: first index in the scene's index buffer
+    size_t delta_base;
+};
+struct PoseDev {                                      // device arrays of the rest data, uploaded once per scene
+    const PoseMesh *meshes; const uint32_t *block_mesh;
+    const float *rest;                                // [vertex][8] position, NORMAL as stored, uv
+    const uint32_t *joints; const float *weights; const float *deltas;
+    const uint32_t *last_face;                        // per vertex (UINT32_MAX: none); generated-normal meshes only
+    const uint32_t *indices;                          // the scene's index buffer
+    const float *palette, *morph;                     // per pose
+};
+// out: vertex records at [vbase, ...), flag: set to 1 when a posed component is not finite (normals the loader leaves non-finite excepted).
+// gen_normals: the second pass over the meshes loaded without NORMAL runs.  max_joints: the largest palette of a skinned mesh.  cudaError_t as int.
+int launch_pose(const PoseDev &d, uint32_t n_blocks, uint32_t max_joints, bool gen_normals, b200pt_vertex *out, uint32_t *flag, cudaStream_t st);
+
 // ---- post chain (post_kernels.cu) ----
 struct PostParams { float Exposure, Gamma, BloomThreshold, BloomStrength, FalloffRange; };
 void launch_accumulate(const float4 *frame, float4 *image, uint32_t first, uint32_t count, uint32_t frame_index, int grid, cudaStream_t st);   // running mean of pixels [first, first + count)

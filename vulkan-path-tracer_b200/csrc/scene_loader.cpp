@@ -95,11 +95,26 @@ struct JParser {
     }
 };
 
-struct M4 { float m[4][4]; };   // row-major m[r][c]
+// untrusted JSON: a short or missing array leaves the default (*err names the field)
+NodeTRS node_trs(const JVal &n, std::string *err) {
+    NodeTRS o;
+    auto vec = [&](const char *key, float *dst, size_t k) {
+        const JVal *v = n.get(key); if (!v) return false;
+        if (v->size() < k) { if (err) *err = std::string("node ") + key + " has fewer than " + std::to_string(k) + " numbers"; return false; }
+        for (size_t i = 0; i < k; i++) dst[i] = (float)(*v)[i].n;
+        return true;
+    };
+    float mm[16];
+    if (vec("matrix", mm, 16)) { o.has_matrix = true; for (int c = 0; c < 4; c++) for (int rr = 0; rr < 4; rr++) o.matrix.m[rr][c] = mm[c * 4 + rr]; }
+    vec("translation", o.t, 3); vec("rotation", o.r, 4); vec("scale", o.s, 3);
+    return o;
+}
+} // namespace
+
 M4 m4_identity() { M4 r; memset(&r, 0, sizeof r); for (int i = 0; i < 4; i++) r.m[i][i] = 1.0f; return r; }
 M4 m4_mul(const M4 &a, const M4 &b) { M4 r; for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) { float s = 0.0f; for (int k = 0; k < 4; k++) s += a.m[i][k] * b.m[k][j]; r.m[i][j] = s; } return r; }
 void m4_to_colmajor(const M4 &a, float out[16]) { for (int c = 0; c < 4; c++) for (int r = 0; r < 4; r++) out[c * 4 + r] = a.m[r][c]; }
-bool m4_inverse_d(const M4 &a, M4 &out) {   // Gauss-Jordan in double
+static bool m4_inverse_d(const M4 &a, M4 &out) {   // Gauss-Jordan in double
     double w[4][8];
     for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) { w[i][j] = a.m[i][j]; w[i][4 + j] = i == j ? 1.0 : 0.0; }
     for (int c = 0; c < 4; c++) {
@@ -112,20 +127,18 @@ bool m4_inverse_d(const M4 &a, M4 &out) {   // Gauss-Jordan in double
     for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) out.m[i][j] = (float)w[i][4 + j];
     return true;
 }
-M4 node_local(const JVal &n) {
-    if (const JVal *mm = n.get("matrix")) { M4 r; for (int c = 0; c < 4; c++) for (int rr = 0; rr < 4; rr++) r.m[rr][c] = (float)(*mm)[c * 4 + rr].n; return r; }
+// a rotation (0, 0, 0, 1) yields the identity bit for bit, so T * R * S equals the product without the rotation factor
+M4 node_local(const NodeTRS &n) {
+    if (n.has_matrix) return n.matrix;
     M4 t = m4_identity(), r = m4_identity(), s = m4_identity();
-    if (const JVal *v = n.get("translation")) for (int i = 0; i < 3; i++) t.m[i][3] = (float)(*v)[i].n;
-    if (const JVal *q = n.get("rotation")) {
-        float x = (float)(*q)[0].n, y = (float)(*q)[1].n, z = (float)(*q)[2].n, w = (float)(*q)[3].n;
-        r.m[0][0] = 1 - 2 * (y * y + z * z); r.m[0][1] = 2 * (x * y - z * w); r.m[0][2] = 2 * (x * z + y * w);
-        r.m[1][0] = 2 * (x * y + z * w); r.m[1][1] = 1 - 2 * (x * x + z * z); r.m[1][2] = 2 * (y * z - x * w);
-        r.m[2][0] = 2 * (x * z - y * w); r.m[2][1] = 2 * (y * z + x * w); r.m[2][2] = 1 - 2 * (x * x + y * y);
-    }
-    if (const JVal *v = n.get("scale")) for (int i = 0; i < 3; i++) s.m[i][i] = (float)(*v)[i].n;
+    for (int i = 0; i < 3; i++) t.m[i][3] = n.t[i];
+    const float x = n.r[0], y = n.r[1], z = n.r[2], w = n.r[3];
+    r.m[0][0] = 1 - 2 * (y * y + z * z); r.m[0][1] = 2 * (x * y - z * w); r.m[0][2] = 2 * (x * z + y * w);
+    r.m[1][0] = 2 * (x * y + z * w); r.m[1][1] = 1 - 2 * (x * x + z * z); r.m[1][2] = 2 * (y * z - x * w);
+    r.m[2][0] = 2 * (x * z - y * w); r.m[2][1] = 2 * (y * z + x * w); r.m[2][2] = 1 - 2 * (x * x + y * y);
+    for (int i = 0; i < 3; i++) s.m[i][i] = n.s[i];
     return m4_mul(m4_mul(t, r), s);
 }
-} // namespace
 
 static bool read_all(const std::string &path, std::vector<uint8_t> &out) {
     FILE *f = fopen(path.c_str(), "rb");
@@ -266,6 +279,79 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
         return true;
     };
 
+    // Accessors of the animation data (skins, JOINTS_n / WEIGHTS_n, morph targets, animations).  Unlike the geometry's accessor above, these
+    // may be sparse or have no bufferView (zeros), and a failure only sets aerr: animation data never fails a load.  Values are decoded as the
+    // accessor says (float, or normalized integers); expect != SIZE_MAX: the element count the caller needs.
+    auto elems = [&](double bvd, double offd, int ct, int nc, size_t count, bool norm, double *out, std::string &aerr) -> bool {
+        auto to_sz = [](double v) { return (v >= 0.0 && v < 4294967296.0) ? (size_t)v : (size_t)-1; };
+        if (!views || !(bvd >= 0.0 && bvd < (double)views->size())) { aerr = "bad bufferView index"; return false; }
+        const JVal &bv = (*views)[(size_t)bvd];
+        const size_t off_v = to_sz(bv.num("byteOffset", 0)), off_a = to_sz(offd);
+        if (off_v == (size_t)-1 || off_a == (size_t)-1) { aerr = "bad byteOffset"; return false; }
+        const size_t off = off_v + off_a;
+        const int csz = (ct == 5120 || ct == 5121) ? 1 : (ct == 5122 || ct == 5123) ? 2 : (ct == 5125 || ct == 5126) ? 4 : 0;
+        if (!csz) { aerr = "bad componentType"; return false; }
+        const size_t elem = (size_t)csz * nc;
+        size_t stride = to_sz(bv.num("byteStride", 0)); if (!stride) stride = elem;
+        if (stride < elem || stride > 4096) { aerr = "bad byteStride"; return false; }
+        const double bid = bv.num("buffer", 0);
+        if (!(bid >= 0.0 && bid < (double)buffers.size())) { aerr = "bad buffer index"; return false; }
+        const std::vector<uint8_t> &buf = buffers[(size_t)bid];
+        if (count && (off > buf.size() || elem > buf.size() - off || count - 1 > (buf.size() - off - elem) / stride)) { aerr = "accessor out of range"; return false; }
+        for (size_t i = 0; i < count; i++) for (int c = 0; c < nc; c++) {
+            const uint8_t *p = &buf[off + i * stride + (size_t)c * csz];
+            double v = 0;
+            switch (ct) {
+            case 5120: { int8_t x; memcpy(&x, p, 1); v = norm ? std::max(x / 127.0, -1.0) : x; } break;
+            case 5121: { uint8_t x = *p; v = norm ? x / 255.0 : x; } break;
+            case 5122: { int16_t x; memcpy(&x, p, 2); v = norm ? std::max(x / 32767.0, -1.0) : x; } break;
+            case 5123: { uint16_t x; memcpy(&x, p, 2); v = norm ? x / 65535.0 : x; } break;
+            case 5125: { uint32_t x; memcpy(&x, p, 4); v = x; } break;
+            case 5126: { float x; memcpy(&x, p, 4); v = x; } break;
+            }
+            out[i * nc + c] = v;
+        }
+        return true;
+    };
+    auto anim_accessor = [&](const JVal *idxv, int want_comps, size_t expect, std::vector<double> &out, size_t &count, std::string &aerr,
+                             int *ct_out = nullptr, bool *norm_out = nullptr) -> bool {
+        if (!idxv || idxv->t != JVal::Num || !accs || !(idxv->n >= 0.0 && idxv->n < (double)accs->size())) { aerr = "bad accessor index"; return false; }
+        const JVal &a = (*accs)[(size_t)idxv->n];
+        const double cd = a.num("count", -1.0);
+        if (!(cd >= 1.0 && cd <= (double)(1u << 26)) || cd != std::floor(cd)) { aerr = "bad accessor count"; return false; }
+        count = (size_t)cd;
+        if (expect != (size_t)-1 && count != expect) { aerr = "accessor count mismatch"; return false; }
+        const JVal *ty = a.get("type"); const std::string ts = ty && ty->t == JVal::Str ? ty->s : "";
+        const int nc = ts == "SCALAR" ? 1 : ts == "VEC2" ? 2 : ts == "VEC3" ? 3 : ts == "VEC4" ? 4 : ts == "MAT4" ? 16 : 0;
+        if (!nc || nc != want_comps) { aerr = "unexpected accessor type " + ts; return false; }
+        const int ct = (int)a.num("componentType", 0);
+        const bool norm = a.get("normalized") && a.get("normalized")->b;
+        if (ct_out) *ct_out = ct;
+        if (norm_out) *norm_out = norm;
+        const JVal *bvv = a.get("bufferView"), *sp = a.get("sparse");
+        if (!bvv && !sp) { aerr = "accessor without bufferView or sparse"; return false; }
+        out.assign(count * nc, 0.0);
+        if (bvv && !elems(bvv->n, a.num("byteOffset", 0), ct, nc, count, norm, out.data(), aerr)) return false;
+        if (sp) {                                                          // glTF 2.0 3.6.2.3: values replace the elements at the given indices
+            const double sc = sp->num("count", -1.0);
+            const JVal *si = sp->get("indices"), *sv = sp->get("values");
+            if (!(sc >= 1.0 && sc <= (double)count) || sc != std::floor(sc) || !si || !sv) { aerr = "bad sparse accessor"; return false; }
+            const size_t m = (size_t)sc;
+            const int ict = (int)si->num("componentType", 0);
+            if (ict != 5121 && ict != 5123 && ict != 5125) { aerr = "bad sparse index componentType"; return false; }
+            std::vector<double> ix(m), vals(m * nc);
+            if (!elems(si->num("bufferView", -1), si->num("byteOffset", 0), ict, 1, m, false, ix.data(), aerr)) return false;
+            if (!elems(sv->num("bufferView", -1), sv->num("byteOffset", 0), ct, nc, m, norm, vals.data(), aerr)) return false;
+            for (size_t k = 0; k < m; k++) {
+                if (!(ix[k] < (double)count)) { aerr = "sparse index out of range"; return false; }
+                for (int c = 0; c < nc; c++) out[(size_t)ix[k] * nc + c] = vals[k * nc + c];
+            }
+        }
+        for (double v : out) if (!std::isfinite(v) || std::fabs(v) > 3.4e38) { aerr = "non-finite value"; return false; }
+        return true;
+    };
+    auto anim = std::make_shared<HostAnimation>();
+
     // ---- meshes: one per primitive (AssetImporterImpl.cpp:121-218)
     std::vector<std::vector<uint32_t>> prims_of_mesh; std::vector<int> mesh_material;
     if (const JVal *ms = g.get("meshes")) for (size_t mi = 0; mi < ms->size(); mi++) {
@@ -318,6 +404,59 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
                 const float inv = 1.0f / sqrtf(nx * nx + ny * ny + nz * nz);              // glm::normalize (:165)
                 v.Normal[0] = nx * inv; v.Normal[1] = ny * inv; v.Normal[2] = nz * inv;
                 v.TexCoord[0] = has_uv ? uv[i * 2] : 0.0f; v.TexCoord[1] = has_uv ? uv[i * 2 + 1] : 0.0f;   // importer flip + FlipUVs = identity
+            }
+            {   // what a pose of this primitive needs (skins, morph targets); problems go to ap.err
+                AnimPrim ap; try { ap.gltf_mesh = (int)mi; ap.count = (uint32_t)n; ap.gen_normals = !has_nrm;
+                std::vector<std::vector<double>> js, ws;
+                for (uint32_t s = 0; s < 16 && ap.err.empty(); s++) {
+                    const std::string jn = "JOINTS_" + std::to_string(s), wn = "WEIGHTS_" + std::to_string(s);
+                    const JVal *ja = at->get(jn.c_str()), *wa = at->get(wn.c_str());
+                    if (!ja && !wa) break;
+                    std::vector<double> j, w; size_t c = 0; int ct = 0; bool nm = false;
+                    if (!ja || !wa) { ap.err = jn + " / " + wn + " not paired"; break; }
+                    if (!anim_accessor(ja, 4, n, j, c, ap.err, &ct)) { ap.err = jn + ": " + ap.err; break; }
+                    if (ct != 5121 && ct != 5123) { ap.err = jn + ": joints must be unsigned byte or unsigned short"; break; }
+                    if (!anim_accessor(wa, 4, n, w, c, ap.err, &ct, &nm)) { ap.err = wn + ": " + ap.err; break; }
+                    if (!(ct == 5126 || ((ct == 5121 || ct == 5123) && nm))) { ap.err = wn + ": weights must be float or normalized unsigned byte / short"; break; }
+                    js.push_back(std::move(j)); ws.push_back(std::move(w));
+                }
+                if (ap.err.empty() && !js.empty()) {
+                    ap.sets = (uint32_t)js.size();
+                    ap.joints.resize(n * 4 * ap.sets); ap.weights.resize(n * 4 * ap.sets);
+                    for (size_t i = 0; i < n; i++) for (uint32_t s = 0; s < ap.sets; s++) for (int k = 0; k < 4; k++) {
+                        ap.joints[(i * ap.sets + s) * 4 + k] = (uint32_t)js[s][i * 4 + k];
+                        ap.weights[(i * ap.sets + s) * 4 + k] = (float)ws[s][i * 4 + k];
+                    }
+                }
+                const JVal *tg = p.get("targets");
+                if (tg && tg->t == JVal::Arr && tg->size()) {
+                    ap.targets = (uint32_t)std::min<size_t>(tg->size(), 256);
+                    if (tg->size() > 256) ap.err = "more than 256 morph targets";
+                    struct { const char *key; int nc; std::vector<float> *dst; } attrs[3] = { { "POSITION", 3, &ap.dpos }, { "NORMAL", 3, &ap.dnrm }, { "TEXCOORD_0", 2, &ap.duv } };
+                    for (uint32_t t = 0; t < ap.targets && ap.err.empty(); t++) {
+                        const JVal &tj = (*tg)[t];
+                        for (auto &A : attrs) {
+                            const JVal *ix = tj.get(A.key); if (!ix) continue;         // TANGENT / COLOR_n: no field in b200pt_vertex
+                            std::vector<double> d; size_t c = 0;
+                            if (!anim_accessor(ix, A.nc, n, d, c, ap.err)) { ap.err = std::string("morph target ") + A.key + ": " + ap.err; break; }
+                            if (A.dst->empty()) A.dst->assign((size_t)ap.targets * n * A.nc, 0.0f);
+                            for (size_t k = 0; k < n * A.nc; k++) (*A.dst)[(size_t)t * n * A.nc + k] = (float)d[k];
+                        }
+                    }
+                }
+                if (ap.sets || ap.targets) {
+                    ap.rest.resize(n * 8);
+                    for (size_t i = 0; i < n; i++) {
+                        for (int k = 0; k < 3; k++) { ap.rest[i * 8 + k] = pos[i * 3 + k]; ap.rest[i * 8 + 3 + k] = has_nrm ? nrm[i * 3 + k] : 0.0f; }
+                        ap.rest[i * 8 + 6] = hm.vertices[i].TexCoord[0]; ap.rest[i * 8 + 7] = hm.vertices[i].TexCoord[1];
+                    }
+                    if (!has_nrm) {
+                        ap.last_face.assign(n, UINT32_MAX);
+                        for (size_t f = 0; f + 2 < hm.indices.size(); f += 3) for (int k = 0; k < 3; k++) ap.last_face[hm.indices[f + k]] = (uint32_t)(f / 3);
+                    }
+                }
+                } catch (const std::bad_alloc &) { ap = AnimPrim(); ap.gltf_mesh = (int)mi; ap.count = (uint32_t)n; ap.err = "out of memory reading the skin / morph data"; }
+                anim->prims.push_back(std::move(ap));
             }
             prims_of_mesh.back().push_back((uint32_t)sc.meshes.size());
             mesh_material.push_back(p.has("material") ? (int)p.num("material", 0) : -1);
@@ -381,7 +520,7 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
         auto [ni, parent] = stack.back(); stack.pop_back();
         if (!nodes || ni < 0 || (size_t)ni >= nodes->size() || ++guard > 10000000) { err = "bad node graph"; return false; }
         const JVal &n = (*nodes)[ni];
-        const M4 world = m4_mul(parent, node_local(n));
+        const M4 world = m4_mul(parent, node_local(node_trs(n, nullptr)));
         if (n.has("mesh")) {
             size_t mi = (size_t)n.num("mesh", 0);
             if (mi < prims_of_mesh.size()) for (uint32_t pm : prims_of_mesh[mi]) {
@@ -389,6 +528,7 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
                 in.MeshIndex = pm; in.MaterialIndex = mesh_material[pm] < 0 ? default_mat : (uint32_t)mesh_material[pm];
                 if (in.MaterialIndex >= sc.materials.size()) { err = "Mesh instance has invalid material index"; return false; }
                 sc.instances.push_back(in);
+                anim->instance_node.push_back(ni);
             }
         }
         if (n.has("camera") && !have_cam && (int)n.num("camera", -1) == 0 && cams && cams->size()) {
@@ -406,6 +546,116 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
         M4 v = m4_identity(); v.m[2][3] = -5.0f; m4_to_colmajor(v, sc.camera_view); sc.camera_aspect = 16.0f / 9.0f;
     }
     if (sc.instances.empty()) { err = "scene has no mesh instances"; return false; }
+
+    // ---- animation data: node graph, skins, morph weights, animations.  Nothing below fails the load.
+    HostAnimation &A = *anim;
+    try {
+        auto index = [](const JVal *v, size_t n) { return (v && v->t == JVal::Num && v->n >= 0.0 && v->n < (double)n && v->n == std::floor(v->n)) ? (int)v->n : -1; };
+        const size_t nn = nodes ? nodes->size() : 0, nskin = g.get("skins") ? g.get("skins")->size() : 0;
+        A.roots = roots;
+        A.nodes.resize(nn);
+        const JVal *ms = g.get("meshes");
+        A.mesh_weights.resize(prims_of_mesh.size()); A.mesh_targets.assign(prims_of_mesh.size(), 0);
+        for (size_t mi = 0; mi < prims_of_mesh.size(); mi++) {
+            for (size_t k = 0; k < prims_of_mesh[mi].size(); k++) {
+                const AnimPrim &ap = A.prims[prims_of_mesh[mi][k]];
+                if (k == 0) A.mesh_targets[mi] = ap.targets;
+                else if (ap.targets != A.mesh_targets[mi] && A.err.empty()) A.err = "mesh " + std::to_string(mi) + ": primitives with different morph target counts";
+            }
+            if (const JVal *w = (*ms)[mi].get("weights")) for (size_t k = 0; k < w->size(); k++) A.mesh_weights[mi].push_back((float)(*w)[k].n);
+            if (!A.mesh_weights[mi].empty() && A.mesh_weights[mi].size() != A.mesh_targets[mi] && A.err.empty()) A.err = "mesh " + std::to_string(mi) + ": weights count differs from its morph targets";
+        }
+        for (size_t i = 0; i < nn; i++) {
+            const JVal &n = (*nodes)[i]; AnimNode &an = A.nodes[i];
+            std::string e; an.trs = node_trs(n, &e);
+            if (!e.empty() && A.err.empty()) A.err = "node " + std::to_string(i) + ": " + e;
+            if (const JVal *ch = n.get("children")) for (size_t c = 0; c < ch->size(); c++) {
+                const int ci = index(&(*ch)[c], nn);
+                if (ci < 0 && A.err.empty()) A.err = "node " + std::to_string(i) + ": child index out of range";
+                if (ci >= 0) an.children.push_back(ci);
+            }
+            if (n.has("mesh")) an.mesh = index(n.get("mesh"), prims_of_mesh.size());
+            if (n.has("skin")) { an.skin = index(n.get("skin"), nskin); if (an.skin < 0 && A.err.empty()) A.err = "node " + std::to_string(i) + ": skin index out of range"; }
+            if (const JVal *w = n.get("weights")) {
+                an.has_weights = true;
+                for (size_t k = 0; k < w->size(); k++) an.weights.push_back((float)(*w)[k].n);
+                if (an.mesh >= 0 && an.weights.size() != A.mesh_targets[an.mesh] && A.err.empty()) A.err = "node " + std::to_string(i) + ": weights count differs from its mesh's morph targets";
+            }
+        }
+        if (const JVal *sk = g.get("skins")) for (size_t s = 0; s < sk->size(); s++) {
+            AnimSkin S; const JVal &sj = (*sk)[s];
+            if (const JVal *js = sj.get("joints")) for (size_t k = 0; k < js->size(); k++) {
+                const int j = index(&(*js)[k], nn);
+                if (j < 0 && S.err.empty()) S.err = "skin " + std::to_string(s) + ": joint index out of range";
+                S.joints.push_back(j < 0 ? 0 : j);
+            }
+            if (S.joints.empty() && S.err.empty()) S.err = "skin " + std::to_string(s) + " has no joints";
+            S.inverse_bind.assign(S.joints.size(), m4_identity());
+            if (const JVal *ib = sj.get("inverseBindMatrices"); ib && S.err.empty()) {
+                std::vector<double> d; size_t c = 0; std::string e;
+                if (!anim_accessor(ib, 16, S.joints.size(), d, c, e)) S.err = "skin " + std::to_string(s) + " inverseBindMatrices: " + e;
+                else for (size_t k = 0; k < S.joints.size(); k++) for (int cc = 0; cc < 4; cc++) for (int r = 0; r < 4; r++) S.inverse_bind[k].m[r][cc] = (float)d[k * 16 + cc * 4 + r];
+            }
+            A.skins.push_back(std::move(S));
+        }
+        if (const JVal *as = g.get("animations")) for (size_t ai = 0; ai < as->size(); ai++) {
+            const JVal &aj = (*as)[ai]; AnimClip C;
+            if (const JVal *nm = aj.get("name")) C.name = nm->s;
+            const JVal *smp = aj.get("samplers"), *chs = aj.get("channels");
+            const size_t nsmp = smp ? smp->size() : 0;
+            for (size_t si = 0; si < nsmp; si++) {
+                const JVal &s = (*smp)[si]; AnimSampler S; std::string e;
+                const JVal *ip = s.get("interpolation");
+                const std::string it = ip && ip->t == JVal::Str ? ip->s : "LINEAR";
+                S.interp = it == "STEP" ? INTERP_STEP : it == "CUBICSPLINE" ? INTERP_CUBIC : INTERP_LINEAR;
+                if (it != "STEP" && it != "LINEAR" && it != "CUBICSPLINE") e = "unknown interpolation " + it;
+                std::vector<double> in, out; size_t ni = 0, no = 0;
+                const JVal *oacc = (accs && s.get("output") && index(s.get("output"), accs->size()) >= 0) ? &(*accs)[(size_t)s.get("output")->n] : nullptr;
+                const JVal *oty = oacc ? oacc->get("type") : nullptr;
+                const std::string ots = oty && oty->t == JVal::Str ? oty->s : "";
+                const int onc = ots == "SCALAR" ? 1 : ots == "VEC3" ? 3 : ots == "VEC4" ? 4 : 0;
+                if (e.empty() && !anim_accessor(s.get("input"), 1, (size_t)-1, in, ni, e)) e = "input: " + e;
+                if (e.empty() && !onc) e = "output: unexpected accessor type " + ots;
+                if (e.empty() && !anim_accessor(s.get("output"), onc, (size_t)-1, out, no, e)) e = "output: " + e;
+                if (e.empty()) for (size_t k = 1; k < ni; k++) if (!(in[k] > in[k - 1])) { e = "input times do not increase"; break; }
+                if (e.empty()) {
+                    S.input.assign(in.begin(), in.end()); S.output.assign(out.begin(), out.end());
+                    for (size_t k = 1; k < ni && e.empty(); k++) if (!(S.input[k] > S.input[k - 1])) e = "input times do not increase in float";
+                    const size_t per_key = S.interp == INTERP_CUBIC ? 3 : 1;
+                    if (e.empty() && (no % (ni * per_key))) e = "output count is not a multiple of the input count";
+                    S.comps = e.empty() ? (uint32_t)(no / (ni * per_key) * onc) : 0;
+                }
+                if (!e.empty()) S.err = "sampler " + std::to_string(si) + ": " + e;
+                C.samplers.push_back(std::move(S));
+            }
+            if (chs) for (size_t ci = 0; ci < chs->size() && C.err.empty(); ci++) {
+                const JVal &c = (*chs)[ci]; const JVal *tg = c.get("target");
+                const JVal *pj = tg ? tg->get("path") : nullptr;
+                const std::string path = pj && pj->t == JVal::Str ? pj->s : "";
+                AnimChannel ch;
+                ch.path = path == "translation" ? PATH_T : path == "rotation" ? PATH_R : path == "scale" ? PATH_S : path == "weights" ? PATH_W : -1;
+                if (ch.path < 0) continue;                                 // KHR_animation_pointer and other extensions: not posed
+                if (!tg->has("node")) continue;                            // glTF 2.0 5.5.2.1: a channel without a node is ignored
+                ch.node = index(tg->get("node"), nn); ch.sampler = index(c.get("sampler"), nsmp);
+                const std::string where = "channel " + std::to_string(ci) + ": ";
+                if (ch.node < 0) { C.err = where + "target node out of range"; break; }
+                if (ch.sampler < 0) { C.err = where + "sampler index out of range"; break; }
+                const AnimSampler &S = C.samplers[ch.sampler];
+                if (!S.err.empty()) { C.err = where + S.err; break; }
+                const AnimNode &an = A.nodes[ch.node];
+                if (ch.path != PATH_W && an.trs.has_matrix) { C.err = where + "animates a node that has a matrix"; break; }
+                const uint32_t want = ch.path == PATH_R ? 4 : ch.path == PATH_W ? (an.mesh >= 0 ? A.mesh_targets[an.mesh] : 0) : 3;
+                if (!want || S.comps != want) { C.err = where + "output size does not match the path"; break; }
+                C.channels.push_back(ch);
+            }
+            animation_range(C, &C.t0, &C.t1);
+            A.clips.push_back(std::move(C));
+        }
+        finalize_animation(A, sc);
+    } catch (const std::bad_alloc &) {
+        if (A.err.empty()) A.err = "out of memory reading the animation data";
+    }
+    sc.animation = anim;
     return true;
 }
 
