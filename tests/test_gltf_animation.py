@@ -517,11 +517,11 @@ def _rows(v):
 DEFORMED = {3: "tube", 4: "tube8", 5: "morphbox", 6: "morphskin", 7: "nonormals", 8: "emissive"}   # mesh index: model key
 
 
-def _model_vertices(g, blobs, model, mesh, world, weights, wabs):
-    """float64 posed (positions, raw normals, uvs, abs-term sums for position / uv, cofactor abs-term sums) of one deformable mesh,
-    in the space its vertices are stored in"""
-    key = DEFORMED[mesh]; M = model[key]
-    prim = g["meshes"][mesh]["primitives"][0]; at = prim["attributes"]
+def _model_vertices(g, blobs, M, mesh, prim, world, weights, wabs):
+    """float64 posed (positions, raw normals, uvs, abs-term sums for position / uv, cofactor abs-term sums) of primitive `prim` of glTF
+    mesh `mesh`, in the space its vertices are stored in.  M: that primitive's influences (joints / weights [vertex, 4 * sets]) and morph
+    deltas per target (dpos / dnrm / duv, None where the target lacks the attribute)"""
+    prim = g["meshes"][mesh]["primitives"][prim]; at = prim["attributes"]
     p = _acc(g, blobs, at["POSITION"]); uv = _acc(g, blobs, at["TEXCOORD_0"])
     n = _acc(g, blobs, at["NORMAL"]) if "NORMAL" in at else np.zeros_like(p)
     pa, ua, na = np.abs(p), np.abs(uv), np.abs(n)
@@ -540,7 +540,8 @@ def _model_vertices(g, blobs, model, mesh, world, weights, wabs):
         Ma = np.einsum("vi,vijk->vjk", np.abs(M["weights"]), Jabs[M["joints"]])
         ph = np.concatenate([p, np.ones((len(p), 1))], 1); pah = np.concatenate([pa, np.ones((len(p), 1))], 1)
         p = np.einsum("vjk,vk->vj", Mv, ph)[:, :3]; pa = np.einsum("vjk,vk->vj", Ma, pah)[:, :3]
-        cof = np.stack([cofactor(m[:3, :3]) for m in Mv])
+        m3 = Mv[:, :3, :3]                                              # cofactor() of every vertex's matrix at once
+        cof = np.stack([np.cross(m3[:, :, 1], m3[:, :, 2]), np.cross(m3[:, :, 2], m3[:, :, 0]), np.cross(m3[:, :, 0], m3[:, :, 1])], axis=2)
         cof_abs = np.einsum("vjk,vk->vj", np.abs(cof), na) / np.maximum(np.linalg.norm(np.einsum("vjk,vk->vj", cof, n), axis=1, keepdims=True), 1e-300)
         n = np.einsum("vjk,vk->vj", cof, n)
     else:
@@ -553,7 +554,7 @@ def _check_pose(pt, T, path, g, blobs, model, a, t):
     d = pt.load_gltf(path); xf = T.get_instance_transforms()
     for mesh in DEFORMED:
         got = _rows(T.get_mesh_vertices(mesh)).astype(np.float64)
-        p, n, uv, pa, ua, na = _model_vertices(g, blobs, model, mesh, world, weights, wabs)
+        p, n, uv, pa, ua, na = _model_vertices(g, blobs, model[DEFORMED[mesh]], mesh, 0, world, weights, wabs)   # one primitive per mesh
         inst = next(i for i, (_, m, _) in enumerate(d["instances"]) if m == mesh)
         X = xf[inst].reshape(4, 4).T.astype(np.float64)
         skinned = "skin" in g["nodes"][next(i for i, nd in enumerate(g["nodes"]) if nd.get("mesh") == mesh)]

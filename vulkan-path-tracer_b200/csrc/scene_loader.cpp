@@ -420,6 +420,13 @@ bool load_gltf_scene(const std::string &path, HostScene &sc, std::string &err) {
                     if (!(ct == 5126 || ((ct == 5121 || ct == 5123) && nm))) { ap.err = wn + ": weights must be float or normalized unsigned byte / short"; break; }
                     js.push_back(std::move(j)); ws.push_back(std::move(w));
                 }
+                // a set the loop did not read (a 17th, or one after a gap in the numbering) would silently lose its influences
+                for (size_t k = 0; k < at->o.size() && ap.err.empty(); k++)
+                    for (const char *pre : { "JOINTS_", "WEIGHTS_" }) {
+                        const std::string &name = at->o[k].first;
+                        if (ap.err.empty() && !name.compare(0, strlen(pre), pre) && strtoul(name.c_str() + strlen(pre), nullptr, 10) >= js.size())
+                            ap.err = name + ": more than 16 JOINTS_n / WEIGHTS_n sets, or a gap in their numbering";
+                    }
                 if (ap.err.empty() && !js.empty()) {
                     ap.sets = (uint32_t)js.size();
                     ap.joints.resize(n * 4 * ap.sets); ap.weights.resize(n * 4 * ap.sets);
