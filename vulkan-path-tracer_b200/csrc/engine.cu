@@ -18,36 +18,17 @@ void Engine::check(cudaError_t e, const char *what) const { check_cuda(e, what);
 #define CK(x) check((x), #x)
 
 static const uint32_t kMaxDispatchTable = 1u << 16;
-template <class T> static void dfree(T *&p) { if (p) { cudaFree(p); p = nullptr; } }
 
-// The device arrays of one query-hook call, on the engine's stream.  Every block is freed when the object goes out of scope, also when an
-// allocation, a copy or the launch throws halfway (cudaFree waits for the work still using it).
-class HookArrays {
-public:
-    explicit HookArrays(cudaStream_t st) : st_(st) {}
-    ~HookArrays() { for (void *p : blocks_) cudaFree(p); }
-    HookArrays(const HookArrays &) = delete;
-    HookArrays &operator=(const HookArrays &) = delete;
-    template <class T> T *out(size_t count) {                 // uninitialised
-        void *p = nullptr;
-        blocks_.push_back(nullptr);                           // before the allocation: a full vector cannot lose the block
-        check_cuda(cudaMalloc(&p, count * sizeof(T)), "cudaMalloc");
-        blocks_.back() = p;
-        return static_cast<T *>(p);
-    }
-    template <class T> T *in(const T *src, size_t count) {    // filled from host memory
-        T *p = out<T>(count);
-        check_cuda(cudaMemcpyAsync(p, src, count * sizeof(T), cudaMemcpyHostToDevice, st_), "cudaMemcpyAsync");
-        return p;
-    }
-    template <class T> void get(T *dst, const T *src, size_t count) {
-        check_cuda(cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, st_), "cudaMemcpyAsync");
-    }
-    void sync() { check_cuda(cudaStreamSynchronize(st_), "cudaStreamSynchronize"); check_cuda(cudaGetLastError(), "cudaGetLastError"); }   // the first error
-private:
-    cudaStream_t st_;
-    std::vector<void *> blocks_;
-};
+static Event make_event(unsigned flags) {
+    cudaEvent_t e = nullptr;
+    check_cuda(cudaEventCreateWithFlags(&e, flags), "cudaEventCreateWithFlags");
+    return Event(e);
+}
+static Stream make_stream() {
+    cudaStream_t s = nullptr;
+    check_cuda(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), "cudaStreamCreateWithFlags");
+    return Stream(s);
+}
 
 Engine::Engine(int device) : device_(device) {
     int n = 0;
@@ -55,72 +36,57 @@ Engine::Engine(int device) : device_(device) {
     if (e != cudaSuccess || n == 0) throw CudaError{ B200PT_ERR_NO_DEVICE, "no CUDA device available (the product has no CPU fallback)" };
     if (device < 0 || device >= n) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "device ordinal out of range" };
     CK(cudaSetDevice(device_));
-    CK(cudaStreamCreateWithFlags(&own_stream_, cudaStreamNonBlocking)); stream_ = own_stream_;
-    CK(cudaEventCreate(&ev_[0])); CK(cudaEventCreate(&ev_[1]));
+    own_stream_ = make_stream(); stream_ = own_stream_.get();
+    ev_[0] = make_event(cudaEventDefault); ev_[1] = make_event(cudaEventDefault);
     b200pt_default_config(&cfg_);
     memset(view_inv_, 0, sizeof view_inv_); memset(proj_inv_, 0, sizeof proj_inv_);
     for (int i = 0; i < 4; i++) view_inv_[i * 5] = proj_inv_[i * 5] = 1.0f;
-    CK(cudaMalloc(&d_ctr_, sizeof(WaveCounters)));
-    CK(cudaMemset(d_ctr_, 0, sizeof(WaveCounters)));
+    CK(alloc(d_ctr_, sizeof(WaveCounters)));
+    CK(cudaMemset(d_ctr_.get(), 0, sizeof(WaveCounters)));
     for (int c = 0; c < 2; c++) {
-        CK(cudaMalloc(&wb_[c].counts, CTRL_WORDS * sizeof(uint32_t))); CK(cudaMallocHost(&wb_[c].h_count, 4 * sizeof(uint32_t)));
-        CK(cudaStreamCreateWithFlags(&aux_stream_[c], cudaStreamNonBlocking)); CK(cudaEventCreateWithFlags(&resolved_ev_[c], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&wb_[c].disp_ev, cudaEventDisableTiming));
-        CK(cudaMalloc(&wb_[c].d_disp, kMaxDispatchTable * sizeof(DevDispatch))); CK(cudaMallocHost(&wb_[c].h_disp, kMaxDispatchTable * sizeof(DevDispatch)));
+        CK(alloc(wb_[c].counts, CTRL_WORDS * sizeof(uint32_t))); CK(alloc(wb_[c].h_count, 4 * sizeof(uint32_t)));
+        aux_stream_[c] = make_stream(); resolved_ev_[c] = make_event(cudaEventDisableTiming);
+        wb_[c].disp_ev = make_event(cudaEventDisableTiming);
+        CK(alloc(wb_[c].d_disp, kMaxDispatchTable * sizeof(DevDispatch))); CK(alloc(wb_[c].h_disp, kMaxDispatchTable * sizeof(DevDispatch)));
     }
-    CK(cudaEventCreateWithFlags(&image_free_ev_, cudaEventDisableTiming));
-    CK(cudaMallocHost(&h_active_count_, sizeof(uint32_t)));
-    CK(cudaMallocHost(&h_small_, 4 * sizeof(uint32_t)));
+    image_free_ev_ = make_event(cudaEventDisableTiming);
+    CK(alloc(h_active_count_, sizeof(uint32_t)));
+    CK(alloc(h_small_, 4 * sizeof(uint32_t)));
     b200pt_default_adaptive(&adaptive_);
     b200pt_default_atmosphere(&atmosphere_);
     memset(&last_, 0, sizeof last_);
 }
 
+// The members release everything else after this body, the streams last.
 Engine::~Engine() {
     cudaSetDevice(device_);
-    for (auto &st : aux_stream_) if (st) cudaStreamSynchronize(st);
+    for (auto &st : aux_stream_) if (st) cudaStreamSynchronize(st.get());
     if (stream_) cudaStreamSynchronize(stream_);
-    free_scene(); free_wave(); free_post(); free_adaptive(); free_denoise(); dfree(d_dn_img_);
-    if (h_active_count_) cudaFreeHost(h_active_count_);
-    if (h_small_) cudaFreeHost(h_small_);
-    dfree(d_scratch_);
-    dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_); for (auto &l : d_luts_) dfree(l);
-    dfree(d_image_); dfree(d_ctr_); dfree(d_volumes_); dfree(d_grids_); grids_.clear(); dfree(d_tri_class_);
-    for (int c = 0; c < 2; c++) {
-        dfree(wb_[c].counts); if (wb_[c].h_count) cudaFreeHost(wb_[c].h_count);
-        if (aux_stream_[c]) { cudaStreamSynchronize(aux_stream_[c]); cudaStreamDestroy(aux_stream_[c]); }
-        if (resolved_ev_[c]) cudaEventDestroy(resolved_ev_[c]);
-        if (wb_[c].disp_ev) cudaEventDestroy(wb_[c].disp_ev);
-        dfree(wb_[c].d_disp); if (wb_[c].h_disp) cudaFreeHost(wb_[c].h_disp);
-    }
-    if (image_free_ev_) cudaEventDestroy(image_free_ev_);
-    if (ev_[0]) cudaEventDestroy(ev_[0]); if (ev_[1]) cudaEventDestroy(ev_[1]);
-    for (auto &e : prof_ev_) cudaEventDestroy(e);
-    if (own_stream_) cudaStreamDestroy(own_stream_);
+    lbvh_free(&bvh_); lbvh_refit_free(&refit_);
 }
 
 // Device scratch of the engine, grown on demand and kept: the per-frame updates allocate (and free, which synchronises the device) nothing.
 // Only valid until the next call; the caller has synchronised the work that used the previous contents.
 void *Engine::scratch(size_t bytes) {
     if (bytes > scratch_bytes_) {
-        dfree(d_scratch_); scratch_bytes_ = 0;
-        CK(cudaMalloc(&d_scratch_, bytes)); scratch_bytes_ = bytes;
+        scratch_bytes_ = 0;
+        CK(alloc(d_scratch_, bytes)); scratch_bytes_ = bytes;
     }
-    return d_scratch_;
+    return d_scratch_.get();
 }
 
 void Engine::sync_all() {
-    for (auto &st : aux_stream_) if (st) CK(cudaStreamSynchronize(st));
+    for (auto &st : aux_stream_) if (st) CK(cudaStreamSynchronize(st.get()));
     CK(cudaStreamSynchronize(stream_));
 }
 void Engine::join_waves() {
     if (wave_seq_ == 0) return;
-    for (auto &e : resolved_ev_) CK(cudaStreamWaitEvent(stream_, e, 0));    // an event that was never recorded counts as complete
+    for (auto &e : resolved_ev_) CK(cudaStreamWaitEvent(stream_, e.get(), 0));    // an event that was never recorded counts as complete
 }
 
 void Engine::free_scene() {
-    dfree(d_verts_); dfree(d_indices_); dfree(d_meshes_); dfree(d_instances_); dfree(d_materials_); dfree(d_textures_); dfree(d_emissive_); dfree(d_em_tris_); dfree(d_em_tri_base_); dfree(d_tri_class_);
-    for (auto &p : d_texdata_) if (p) cudaFree(p);
+    d_verts_.reset(); d_indices_.reset(); d_meshes_.reset(); d_instances_.reset(); d_materials_.reset(); d_textures_.reset(); d_emissive_.reset();
+    d_em_tris_.reset(); d_em_tri_base_.reset(); d_tri_class_.reset();
     d_texdata_.clear();
     lbvh_free(&bvh_); lbvh_refit_free(&refit_);
     free_pose_data();
@@ -156,35 +122,35 @@ void Engine::upload_scene() {
         memcpy(&verts[h_meshes_[i].vbase], scene_.meshes[i].vertices.data(), scene_.meshes[i].vertices.size() * sizeof(b200pt_vertex));
         memcpy(&idx[h_meshes_[i].ibase], scene_.meshes[i].indices.data(), scene_.meshes[i].indices.size() * 4);
     }
-    CK(cudaMalloc(&d_verts_, nv * sizeof(b200pt_vertex))); CK(cudaMemcpy(d_verts_, verts.data(), nv * sizeof(b200pt_vertex), cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&d_indices_, ni * 4)); CK(cudaMemcpy(d_indices_, idx.data(), ni * 4, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&d_meshes_, h_meshes_.size() * sizeof(DevMesh))); CK(cudaMemcpy(d_meshes_, h_meshes_.data(), h_meshes_.size() * sizeof(DevMesh), cudaMemcpyHostToDevice));
+    CK(alloc(d_verts_, nv * sizeof(b200pt_vertex))); CK(cudaMemcpy(d_verts_.get(), verts.data(), nv * sizeof(b200pt_vertex), cudaMemcpyHostToDevice));
+    CK(alloc(d_indices_, ni * 4)); CK(cudaMemcpy(d_indices_.get(), idx.data(), ni * 4, cudaMemcpyHostToDevice));
+    CK(alloc(d_meshes_, h_meshes_.size() * sizeof(DevMesh))); CK(cudaMemcpy(d_meshes_.get(), h_meshes_.data(), h_meshes_.size() * sizeof(DevMesh), cudaMemcpyHostToDevice));
     fill_instances();
-    CK(cudaMalloc(&d_instances_, h_instances_.size() * sizeof(DevInstance)));
+    CK(alloc(d_instances_, h_instances_.size() * sizeof(DevInstance)));
     {
         std::vector<DevMaterial> dm; dm.reserve(scene_.materials.size());
         for (const auto &m : scene_.materials) dm.push_back(make_dev_material(m));
-        CK(cudaMalloc(&d_materials_, dm.size() * sizeof(DevMaterial)));
-        CK(cudaMemcpy(d_materials_, dm.data(), dm.size() * sizeof(DevMaterial), cudaMemcpyHostToDevice));
-        launch_prepare_materials(d_materials_, 0, (uint32_t)dm.size(), stream_);
+        CK(alloc(d_materials_, dm.size() * sizeof(DevMaterial)));
+        CK(cudaMemcpy(d_materials_.get(), dm.data(), dm.size() * sizeof(DevMaterial), cudaMemcpyHostToDevice));
+        launch_prepare_materials(d_materials_.get(), 0, (uint32_t)dm.size(), stream_);
         CK(cudaStreamSynchronize(stream_));
     }
-    CK(cudaMalloc(&d_emissive_, std::max<size_t>(1, scene_.instances.size()) * sizeof(DevEmissive)));
+    CK(alloc(d_emissive_, std::max<size_t>(1, scene_.instances.size()) * sizeof(DevEmissive)));
     rebuild_emissive();
     // textures
     std::vector<DevTexture> dt(scene_.textures.size());
-    d_texdata_.assign(scene_.textures.size(), nullptr);
+    d_texdata_.resize(scene_.textures.size());
     for (size_t i = 0; i < scene_.textures.size(); i++) {
         const HostTexture &t = scene_.textures[i];
-        CK(cudaMalloc(&d_texdata_[i], std::max<size_t>(t.data.size(), 4)));
-        CK(cudaMemcpy(d_texdata_[i], t.data.data(), t.data.size(), cudaMemcpyHostToDevice));
-        dt[i] = { d_texdata_[i], t.width, t.height, t.channels, 0 };
+        CK(alloc(d_texdata_[i], std::max<size_t>(t.data.size(), 4)));
+        CK(cudaMemcpy(d_texdata_[i].get(), t.data.data(), t.data.size(), cudaMemcpyHostToDevice));
+        dt[i] = { d_texdata_[i].get(), t.width, t.height, t.channels, 0 };
     }
-    CK(cudaMalloc(&d_textures_, dt.size() * sizeof(DevTexture))); CK(cudaMemcpy(d_textures_, dt.data(), dt.size() * sizeof(DevTexture), cudaMemcpyHostToDevice));
-    ds_.verts = d_verts_; ds_.indices = d_indices_; ds_.meshes = d_meshes_; ds_.instances = d_instances_; ds_.materials = d_materials_;
-    CK(cudaMalloc(&d_tri_class_, std::max<size_t>(1, n_tris_)));
+    CK(alloc(d_textures_, dt.size() * sizeof(DevTexture))); CK(cudaMemcpy(d_textures_.get(), dt.data(), dt.size() * sizeof(DevTexture), cudaMemcpyHostToDevice));
+    ds_.verts = d_verts_.get(); ds_.indices = d_indices_.get(); ds_.meshes = d_meshes_.get(); ds_.instances = d_instances_.get(); ds_.materials = d_materials_.get();
+    CK(alloc(d_tri_class_, std::max<size_t>(1, n_tris_)));
     rebuild_tri_class();
-    ds_.textures = d_textures_; ds_.emissive = d_emissive_;
+    ds_.textures = d_textures_.get(); ds_.emissive = d_emissive_.get();
     build_bvh(&bvh_, &ds_, &lc_);
     upload_pose_data();
 }
@@ -216,12 +182,12 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_bu
     int sah_mode = 3;
     if (const char *e = getenv("B200PT_BVH_SAH")) sah_mode = (e[0] >= '0' && e[0] <= '5' && e[1] == 0) ? e[0] - '0' : 3;
     if (gpu_builder) sah_mode = 0;
-    float *d_ref_box = nullptr;
-    int r = lbvh_build(d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_, sah_mode == 2 || sah_mode == 3,
-                       gpu_builder ? &d_ref_box : nullptr);
+    DevPtr<float> ref_box;
+    int r = lbvh_build(d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_,
+                       sah_mode == 2 || sah_mode == 3, gpu_builder ? &ref_box : nullptr);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build failed: ") + cudaGetErrorString((cudaError_t)r) };
     if (gpu_builder) {
-        r = lbvh_ploc_rebuild(out, d_ref_box, h_small_, stream_);                      // frees d_ref_box
+        r = lbvh_ploc_rebuild(out, std::move(ref_box), h_small_.get(), stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_ploc_rebuild failed: ") + cudaGetErrorString((cudaError_t)r) };
     }
     if (sah_mode) {
@@ -234,7 +200,7 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_bu
     ds->n_tris = out->n_tris; ds->n_nodes = out->n_nodes; ds->root = out->root; ds->bvh_bytes = out->bytes <= 0xFFFFFFFFull ? (uint32_t)out->bytes : 0;
     ds->nodes4 = nullptr; ds->n_nodes4 = 0;
     if (out->bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
-        r = gpu_builder ? lbvh_build_wide_device(out, h_small_, stream_) : lbvh_build_wide(out, stream_);
+        r = gpu_builder ? lbvh_build_wide_device(out, h_small_.get(), stream_) : lbvh_build_wide(out, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build_wide failed: ") + cudaGetErrorString((cudaError_t)r) };
         ds->nodes4 = out->nodes4; ds->n_nodes4 = out->n_nodes4;
     }
@@ -296,7 +262,7 @@ void Engine::update_mesh_vertices(const b200pt_mesh_update *u, uint32_t n, bool 
         for (uint32_t i = 0; i < n; o += u[i].vertex_count, i++)
             if (u[i].vertex_count) CK(cudaMemcpyAsync(stage + o, u[i].vertices, u[i].vertex_count * VB, cudaMemcpyDeviceToDevice, stream_));
         bool bad = false;
-        const int r = any_nonfinite(reinterpret_cast<const float *>(stage), total * VF, reinterpret_cast<uint32_t *>(stage + total), h_small_, stream_, &bad);
+        const int r = any_nonfinite(reinterpret_cast<const float *>(stage), total * VF, reinterpret_cast<uint32_t *>(stage + total), h_small_.get(), stream_, &bad);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("any_nonfinite failed: ") + cudaGetErrorString((cudaError_t)r) };
         if (bad) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "vertex component is not finite" };
     }
@@ -322,7 +288,7 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         for (size_t i = 0; i < src.size(); i++) {
             std::vector<b200pt_vertex> &mv = scene_.meshes[src[i].mesh].vertices;
             mv = old[i];
-            if (!mv.empty()) CK(cudaMemcpyAsync(d_verts_ + h_meshes_[src[i].mesh].vbase, mv.data(), mv.size() * VB, cudaMemcpyHostToDevice, stream_));
+            if (!mv.empty()) CK(cudaMemcpyAsync(d_verts_.get() + h_meshes_[src[i].mesh].vbase, mv.data(), mv.size() * VB, cudaMemcpyHostToDevice, stream_));
         }
         if (instances) { scene_.instances = old_instances; fill_instances(); }
         CK(cudaStreamSynchronize(stream_));
@@ -331,7 +297,7 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
     try {
         for (const VertexSource &s : src) {
             std::vector<b200pt_vertex> &mv = scene_.meshes[s.mesh].vertices;
-            b200pt_vertex *dst = d_verts_ + h_meshes_[s.mesh].vbase;
+            b200pt_vertex *dst = d_verts_.get() + h_meshes_[s.mesh].vbase;
             const size_t bytes = mv.size() * VB;
             if (!bytes) continue;
             if (s.device) {
@@ -354,9 +320,9 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         for (size_t a = 0; a < h_instances_.size(); a++) if (listed[h_instances_[a].mesh]) changed.push_back((uint32_t)a);
         uint32_t *const d_list = src.empty() ? nullptr : static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
         auto refit = [&]() {
-            int r = lbvh_refit(&bvh_, &refit_, d_verts_, d_indices_, d_meshes_, d_instances_, (uint32_t)h_instances_.size(), stream_);
+            int r = lbvh_refit(&bvh_, &refit_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), stream_);
             if (r == 0 && !src.empty())
-                r = lbvh_refresh_shade(&bvh_, d_verts_, d_indices_, d_meshes_, d_instances_, h_instances_.data(), h_meshes_.data(), changed.data(),
+                r = lbvh_refresh_shade(&bvh_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), changed.data(),
                                        (uint32_t)changed.size(), d_list, stream_);
             return r;
         };
@@ -417,9 +383,7 @@ void Engine::upload_pose_data() {
                 deltas[m.delta_base + ((size_t)t * 8 + P.c0 + c) * m.count + i] = (*P.src)[((size_t)t * m.count + i) * P.nc + c];
     }
     auto up = [&](const void *src, size_t bytes) -> void * {
-        void *p = nullptr;
-        d_pose_blocks_.push_back(nullptr);
-        CK(cudaMalloc(&p, std::max<size_t>(bytes, 16))); d_pose_blocks_.back() = p;
+        void *p = pose_blocks_.out<uint8_t>(std::max<size_t>(bytes, 16));
         if (src && bytes) CK(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice));
         return p;
     };
@@ -430,15 +394,14 @@ void Engine::upload_pose_data() {
     pose_dev_.weights = static_cast<const float *>(up(weights.data(), weights.size() * 4));
     pose_dev_.deltas = static_cast<const float *>(up(deltas.data(), deltas.size() * 4));
     pose_dev_.last_face = static_cast<const uint32_t *>(up(pose_gen_normals_ ? last_face.data() : nullptr, pose_gen_normals_ ? last_face.size() * 4 : 0));
-    pose_dev_.indices = d_indices_;
+    pose_dev_.indices = d_indices_.get();
     pose_dev_.palette = static_cast<const float *>(up(nullptr, (size_t)pose_palette_floats_ * 4));
     pose_dev_.morph = static_cast<const float *>(up(nullptr, (size_t)pose_morph_floats_ * 4));
     pose_grid_ = (uint32_t)block_mesh.size(); pose_vertices_ = (uint32_t)nv;
 }
 
 void Engine::free_pose_data() {
-    for (void *p : d_pose_blocks_) if (p) cudaFree(p);
-    d_pose_blocks_.clear(); pose_dev_ = PoseDev{}; pose_meshes_.clear(); pose_grid_ = pose_vertices_ = 0;
+    pose_blocks_.clear(); pose_dev_ = PoseDev{}; pose_meshes_.clear(); pose_grid_ = pose_vertices_ = 0;
 }
 
 // glTF pose (DESIGN §15): arguments checked, the waves in flight finished, the pose evaluated on the host (animation.cpp), its joint
@@ -463,9 +426,9 @@ void Engine::pose(int animation, float t, int rebuild) {
         CK(cudaMemsetAsync(flag, 0, 4, stream_));
         const int r = launch_pose(pose_dev_, pose_grid_, pose_max_joints_, pose_gen_normals_, stage, flag, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("launch_pose failed: ") + cudaGetErrorString((cudaError_t)r) };
-        CK(cudaMemcpyAsync(h_small_, flag, 4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(h_small_.get(), flag, 4, cudaMemcpyDeviceToHost, stream_));
         CK(cudaStreamSynchronize(stream_));                     // also: P's host arrays are no longer read
-        if (h_small_[0]) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "a posed vertex component is not finite" };
+        if (*h_small_) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "a posed vertex component is not finite" };
         for (size_t d = 0; d < pose_meshes_.size(); d++)
             src.push_back({ (uint32_t)scene_.animation->deformable[d], stage + pose_meshes_[d].vbase, true });
     }
@@ -513,8 +476,8 @@ void Engine::rebuild_tri_class() {
         const uint32_t first = h_instances_[i].tri_base, cnt = h_meshes_[scene_.instances[i].MeshIndex].tri_count;
         if (cnt) { class_mask_ |= 1u << c; std::fill(tc.begin() + first, tc.begin() + first + cnt, c); }
     }
-    CK(cudaMemcpy(d_tri_class_, tc.data(), tc.size(), cudaMemcpyHostToDevice));
-    ds_.tri_class = d_tri_class_;
+    CK(cudaMemcpy(d_tri_class_.get(), tc.data(), tc.size(), cudaMemcpyHostToDevice));
+    ds_.tri_class = d_tri_class_.get();
     ds_.uniform_class = 0xFFu;
     for (uint32_t c = 0; c < MC_COUNT; c++) if (class_mask_ == (1u << c)) ds_.uniform_class = c;
 }
@@ -535,7 +498,7 @@ void Engine::rebuild_emissive() {
     }
     if (em.size() >= 10000) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "too many emissive meshes (MAX_EMISSIVE_MESHES)" };
     n_emissive_ = (uint32_t)em.size();
-    if (!em.empty()) CK(cudaMemcpy(d_emissive_, em.data(), em.size() * sizeof(DevEmissive), cudaMemcpyHostToDevice));
+    if (!em.empty()) CK(cudaMemcpy(d_emissive_.get(), em.data(), em.size() * sizeof(DevEmissive), cudaMemcpyHostToDevice));
     // world-space emissive triangles (SH/Sampler.slang:376-391: vertices fetched and transformed per sample in the reference)
     std::vector<EmTri> et; std::vector<uint32_t> base;
     for (const DevEmissive &e : em) {
@@ -556,12 +519,12 @@ void Engine::rebuild_emissive() {
             et.push_back(r);
         }
     }
-    dfree(d_em_tris_); dfree(d_em_tri_base_);
-    CK(cudaMalloc(&d_em_tris_, std::max<size_t>(1, et.size()) * sizeof(EmTri))); CK(cudaMalloc(&d_em_tri_base_, std::max<size_t>(1, base.size()) * sizeof(uint32_t)));
-    if (!et.empty()) CK(cudaMemcpy(d_em_tris_, et.data(), et.size() * sizeof(EmTri), cudaMemcpyHostToDevice));
-    if (!base.empty()) CK(cudaMemcpy(d_em_tri_base_, base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    ds_.em_tris = d_em_tris_; ds_.em_tri_base = d_em_tri_base_;
-    CK(cudaMemcpy(d_instances_, h_instances_.data(), h_instances_.size() * sizeof(DevInstance), cudaMemcpyHostToDevice));
+    d_em_tris_.reset(); d_em_tri_base_.reset();
+    CK(alloc(d_em_tris_, std::max<size_t>(1, et.size()) * sizeof(EmTri))); CK(alloc(d_em_tri_base_, std::max<size_t>(1, base.size()) * sizeof(uint32_t)));
+    if (!et.empty()) CK(cudaMemcpy(d_em_tris_.get(), et.data(), et.size() * sizeof(EmTri), cudaMemcpyHostToDevice));
+    if (!base.empty()) CK(cudaMemcpy(d_em_tri_base_.get(), base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    ds_.em_tris = d_em_tris_.get(); ds_.em_tri_base = d_em_tri_base_.get();
+    CK(cudaMemcpy(d_instances_.get(), h_instances_.data(), h_instances_.size() * sizeof(DevInstance), cudaMemcpyHostToDevice));
     ds_.n_emissive = n_emissive_;
 }
 
@@ -573,7 +536,7 @@ void Engine::set_material(uint32_t idx, const b200pt_material &m) {
     for (uint32_t t : tix) if (t >= scene_.textures.size()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "texture index out of range" };
     sync_all();
     scene_.materials[idx] = m;
-    { const DevMaterial dm = make_dev_material(m); CK(cudaMemcpy(d_materials_ + idx, &dm, sizeof dm, cudaMemcpyHostToDevice)); launch_prepare_materials(d_materials_, idx, 1, stream_); CK(cudaStreamSynchronize(stream_)); }
+    { const DevMaterial dm = make_dev_material(m); CK(cudaMemcpy(d_materials_.get() + idx, &dm, sizeof dm, cudaMemcpyHostToDevice)); launch_prepare_materials(d_materials_.get(), idx, 1, stream_); CK(cudaStreamSynchronize(stream_)); }
     rebuild_emissive();
     rebuild_tri_class();
     reset();
@@ -584,12 +547,11 @@ static void check_volume(const b200pt_volume &v) {
     for (int k = 0; k < 3; k++) if (!(v.CornerMin[k] <= v.CornerMax[k]) || !(v.Scale[k] >= 0.0f)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "volume AABB: CornerMin > CornerMax or negative Scale" };
     if (!(v.Density >= 0.0f)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "volume density must be >= 0" };
 }
-Engine::GridData::~GridData() { cudaFree(d_values); cudaFree(d_max_densities); }
 void Engine::upload_volumes() {
     CK(cudaSetDevice(device_));
     sync_all();
-    if (!d_volumes_) CK(cudaMalloc(&d_volumes_, B200PT_MAX_VOLUMES * sizeof(DevVolume)));
-    if (!d_grids_) CK(cudaMalloc(&d_grids_, B200PT_MAX_VOLUMES * sizeof(DevGrid)));
+    if (!d_volumes_) CK(alloc(d_volumes_, B200PT_MAX_VOLUMES * sizeof(DevVolume)));
+    if (!d_grids_) CK(alloc(d_grids_, B200PT_MAX_VOLUMES * sizeof(DevGrid)));
     std::vector<DevVolume> dv(volumes_.size());
     std::vector<DevGrid> dg;
     for (size_t i = 0; i < volumes_.size(); i++) {
@@ -607,16 +569,16 @@ void Engine::upload_volumes() {
         if (grids_[i]) {
             const GridData &G = *grids_[i];
             DevGrid g{};
-            g.values = G.d_values; g.max_densities = G.d_max_densities;
+            g.values = G.d_values.get(); g.max_densities = G.d_max_densities.get();
             for (int k = 0; k < 3; k++) { g.imin[k] = G.host.imin[k]; g.dim[k] = G.host.dim[k]; g.wmin[k] = G.host.wmin[k]; g.wext[k] = G.host.wext[k]; g.inv_vs[k] = G.host.inv_vs[k]; g.trans[k] = G.host.trans[k]; }
             slot = (uint32_t)dg.size(); dg.push_back(g);
         }
         dv[i].flags = make_uint4(v.ApproximatedScatteringForClouds, (uint32_t)(v.HasTemperatureData != 0), (uint32_t)(v.UseBlackbody != 0), slot);
     }
-    if (!dv.empty()) CK(cudaMemcpy(d_volumes_, dv.data(), dv.size() * sizeof(DevVolume), cudaMemcpyHostToDevice));
-    if (!dg.empty()) CK(cudaMemcpy(d_grids_, dg.data(), dg.size() * sizeof(DevGrid), cudaMemcpyHostToDevice));
-    ds_.volumes = d_volumes_; ds_.n_volumes = (uint32_t)dv.size(); ds_.phase_function = phase_function_;
-    ds_.grids = d_grids_; ds_.n_grids = (uint32_t)dg.size();
+    if (!dv.empty()) CK(cudaMemcpy(d_volumes_.get(), dv.data(), dv.size() * sizeof(DevVolume), cudaMemcpyHostToDevice));
+    if (!dg.empty()) CK(cudaMemcpy(d_grids_.get(), dg.data(), dg.size() * sizeof(DevGrid), cudaMemcpyHostToDevice));
+    ds_.volumes = d_volumes_.get(); ds_.n_volumes = (uint32_t)dv.size(); ds_.phase_function = phase_function_;
+    ds_.grids = d_grids_.get(); ds_.n_grids = (uint32_t)dg.size();
     reset();
 }
 // the three READ-ONLY members of b200pt_volume follow the density data attached to the index, whatever the caller's struct says
@@ -649,10 +611,10 @@ void Engine::add_density_grid(uint32_t idx, const b200pt_density_grid &g) {
     prepare_density_grid(g, G->host);
     CK(cudaSetDevice(device_));
     sync_all();
-    CK(cudaMalloc(&G->d_values, G->host.values.size() * sizeof(float)));
-    CK(cudaMalloc(&G->d_max_densities, G->host.max_densities.size() * sizeof(float)));
-    CK(cudaMemcpy(G->d_values, G->host.values.data(), G->host.values.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(G->d_max_densities, G->host.max_densities.data(), G->host.max_densities.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(alloc(G->d_values, G->host.values.size() * sizeof(float)));
+    CK(alloc(G->d_max_densities, G->host.max_densities.size() * sizeof(float)));
+    CK(cudaMemcpy(G->d_values.get(), G->host.values.data(), G->host.values.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(G->d_max_densities.get(), G->host.max_densities.data(), G->host.max_densities.size() * sizeof(float), cudaMemcpyHostToDevice));
     b200pt_volume &v = volumes_[idx];
     for (int k = 0; k < 3; k++) { v.CornerMin[k] = G->host.corner_min[k]; v.CornerMax[k] = G->host.corner_max[k]; }
     v.MaxDensityInTheGrid = G->host.max_density;
@@ -684,16 +646,16 @@ void Engine::set_env_map(uint32_t w, uint32_t h, const float *rgba) {
     std::vector<float> px(rgba, rgba + (size_t)w * h * 4);
     std::vector<uint2> alias((size_t)w * h);
     build_env_alias(px.data(), w, h, alias.data());
-    dfree(d_env_); dfree(d_alias_); dfree(d_env_row_cos_);
+    d_env_.reset(); d_alias_.reset(); d_env_row_cos_.reset();
     {   // SH/Sampler.slang:329-331: stepTheta = M_PI / height; theta0 = py * stepTheta; cos(theta0), cos(theta0 + stepTheta)
         std::vector<float2> rc(h); const float stepTheta = 3.1415926535897F / (float)h;
         for (uint32_t y = 0; y < h; y++) { const float t0 = (float)y * stepTheta; rc[y] = make_float2(cosf(t0), cosf(t0 + stepTheta)); }
-        CK(cudaMalloc(&d_env_row_cos_, rc.size() * sizeof(float2))); CK(cudaMemcpy(d_env_row_cos_, rc.data(), rc.size() * sizeof(float2), cudaMemcpyHostToDevice));
-        ds_.env_row_cos = d_env_row_cos_;
+        CK(alloc(d_env_row_cos_, rc.size() * sizeof(float2))); CK(cudaMemcpy(d_env_row_cos_.get(), rc.data(), rc.size() * sizeof(float2), cudaMemcpyHostToDevice));
+        ds_.env_row_cos = d_env_row_cos_.get();
     }
-    CK(cudaMalloc(&d_env_, px.size() * 4)); CK(cudaMemcpy(d_env_, px.data(), px.size() * 4, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&d_alias_, alias.size() * sizeof(uint2))); CK(cudaMemcpy(d_alias_, alias.data(), alias.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    ds_.env = d_env_; ds_.alias = d_alias_; ds_.envW = w; ds_.envH = h;
+    CK(alloc(d_env_, px.size() * 4)); CK(cudaMemcpy(d_env_.get(), px.data(), px.size() * 4, cudaMemcpyHostToDevice));
+    CK(alloc(d_alias_, alias.size() * sizeof(uint2))); CK(cudaMemcpy(d_alias_.get(), alias.data(), alias.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    ds_.env = d_env_.get(); ds_.alias = d_alias_.get(); ds_.envW = w; ds_.envH = h;
     has_env_ = true;
     reset();
 }
@@ -703,8 +665,8 @@ void Engine::set_luts(const float *refl, const float *rout, const float *rin) {
     if (!refl || !rout || !rin) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "null LUT" };
     sync_all();
     const size_t n[3] = { 64 * 64 * 32, 128 * 128 * 32, 128 * 128 * 32 }; const float *src[3] = { refl, rout, rin };
-    for (int i = 0; i < 3; i++) { dfree(d_luts_[i]); CK(cudaMalloc(&d_luts_[i], n[i] * 4)); CK(cudaMemcpy(d_luts_[i], src[i], n[i] * 4, cudaMemcpyHostToDevice)); }
-    ds_.lut_reflect = d_luts_[0]; ds_.lut_refract_out = d_luts_[1]; ds_.lut_refract_in = d_luts_[2];
+    for (int i = 0; i < 3; i++) { CK(alloc(d_luts_[i], n[i] * 4)); CK(cudaMemcpy(d_luts_[i].get(), src[i], n[i] * 4, cudaMemcpyHostToDevice)); }
+    ds_.lut_reflect = d_luts_[0].get(); ds_.lut_refract_out = d_luts_[1].get(); ds_.lut_refract_in = d_luts_[2].get();
     has_luts_ = true;
     reset();
 }
@@ -742,13 +704,13 @@ void Engine::set_track_variance(bool on) {
     reset();
 }
 void Engine::free_adaptive() {
-    dfree(d_px_state_); dfree(d_active_); dfree(d_tile_count_); dfree(d_active_count_);
+    d_px_state_.reset(); d_active_.reset(); d_tile_count_.reset(); d_active_count_.reset();
     adaptive_pixels_ = 0; adaptive_ready_ = false;
 }
 void Engine::update_active(bool decide, cudaStream_t st) {
     const uint32_t npix = (uint32_t)adaptive_pixels_;
-    launch_adaptive_update(d_px_state_, npix, adaptive_.Threshold, adaptive_.MinSamples, decide, d_tile_count_, d_active_, d_active_count_, st);
-    CK(cudaMemcpyAsync(h_active_count_, d_active_count_, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    launch_adaptive_update(d_px_state_.get(), npix, adaptive_.Threshold, adaptive_.MinSamples, decide, d_tile_count_.get(), d_active_.get(), d_active_count_.get(), st);
+    CK(cudaMemcpyAsync(h_active_count_.get(), d_active_count_.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     active_count_ = *h_active_count_;
 }
@@ -760,11 +722,11 @@ void Engine::prepare_adaptive() {
     if (npix != adaptive_pixels_ || !d_px_state_) {
         free_adaptive();
         const size_t n = std::max<size_t>(npix, 1), tiles = (n + ADAPTIVE_TILE - 1) / ADAPTIVE_TILE;
-        CK(cudaMalloc(&d_px_state_, n * sizeof(uint4))); CK(cudaMalloc(&d_active_, n * sizeof(uint32_t)));
-        CK(cudaMalloc(&d_tile_count_, tiles * sizeof(uint32_t))); CK(cudaMalloc(&d_active_count_, sizeof(uint32_t)));
+        CK(alloc(d_px_state_, n * sizeof(uint4))); CK(alloc(d_active_, n * sizeof(uint32_t)));
+        CK(alloc(d_tile_count_, tiles * sizeof(uint32_t))); CK(alloc(d_active_count_, sizeof(uint32_t)));
         adaptive_pixels_ = npix;
     }
-    CK(cudaMemsetAsync(d_px_state_, 0, std::max<size_t>(npix, 1) * sizeof(uint4), stream_));
+    CK(cudaMemsetAsync(d_px_state_.get(), 0, std::max<size_t>(npix, 1) * sizeof(uint4), stream_));
     update_active(false, stream_);
     adaptive_ready_ = true;
 }
@@ -784,7 +746,7 @@ void Engine::pixel_stats(uint32_t *counts, float *rel_error) {
     }
     sync_all();
     std::vector<uint4> st(npix);
-    CK(cudaMemcpy(st.data(), d_px_state_, npix * sizeof(uint4), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(st.data(), d_px_state_.get(), npix * sizeof(uint4), cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < npix; i++) {
         const uint32_t n = st[i].z;
         if (counts) counts[i] = n;
@@ -816,15 +778,14 @@ void Engine::set_partition(uint32_t rank, uint32_t world, uint32_t band) {
 }
 void Engine::ensure_image() {
     const size_t need = (size_t)W_ * std::max<uint32_t>(local_rows_, 1);
-    if (need != image_pixels_) { dfree(d_image_); CK(cudaMalloc(&d_image_, need * sizeof(float4))); image_pixels_ = need; }
-    CK(cudaMemsetAsync(d_image_, 0, image_pixels_ * sizeof(float4), stream_));
+    if (need != image_pixels_) { CK(alloc(d_image_, need * sizeof(float4))); image_pixels_ = need; }
+    CK(cudaMemsetAsync(d_image_.get(), 0, image_pixels_ * sizeof(float4), stream_));
 }
 
 void Engine::free_wave() {
     for (auto &B : wb_) {
-        for (auto &p : B.ps) { dfree(p.org_pdf); dfree(p.dir_rng); dfree(p.thr_depth); dfree(p.rad_slot); dfree(p.medium); dfree(p.medium_g); dfree(p.vol_depth); }
-        dfree(B.so.hit); dfree(B.so.bxdf_pdf); dfree(B.so.e0); dfree(B.so.sky_o); dfree(B.so.sky_d); dfree(B.so.sky_c); dfree(B.so.lit_o); dfree(B.so.lit_d); dfree(B.so.lit_c);
-        dfree(B.sample_buf); dfree(B.rng_carry); dfree(B.q_hit); dfree(B.q_miss);
+        B.arrays.clear();
+        B.ps[0] = B.ps[1] = PathState{}; B.so = ShadeOut{}; B.sample_buf = nullptr; B.rng_carry = B.q_hit = B.q_miss = nullptr;
         B.cap = 0;
     }
     wave_cap_ = 0;
@@ -836,14 +797,14 @@ void Engine::ensure_wave(size_t cap, int contexts) {
     sync_all();
     cap = std::max(cap, wave_cap_);
     free_wave();
-    auto a4 = [&](float4 *&p) { CK(cudaMalloc(&p, cap * sizeof(float4))); };
     for (int c = 0; c < contexts; c++) {
         WaveBuf &B = wb_[c];
-        for (auto &p : B.ps) { a4(p.org_pdf); a4(p.dir_rng); a4(p.thr_depth); a4(p.rad_slot); a4(p.medium); CK(cudaMalloc(&p.medium_g, cap * sizeof(float))); CK(cudaMalloc(&p.vol_depth, cap * sizeof(uint32_t))); }
+        auto a4 = [&](float4 *&p) { p = B.arrays.out<float4>(cap); };
+        for (auto &p : B.ps) { a4(p.org_pdf); a4(p.dir_rng); a4(p.thr_depth); a4(p.rad_slot); a4(p.medium); p.medium_g = B.arrays.out<float>(cap); p.vol_depth = B.arrays.out<uint32_t>(cap); }
         a4(B.so.hit); a4(B.so.bxdf_pdf); a4(B.so.e0); a4(B.so.sky_o); a4(B.so.sky_d); a4(B.so.sky_c); a4(B.so.lit_o); a4(B.so.lit_d); a4(B.so.lit_c);
         a4(B.sample_buf);
-        CK(cudaMalloc(&B.rng_carry, cap * sizeof(uint32_t)));
-        CK(cudaMalloc(&B.q_hit, (size_t)MC_COUNT * cap * sizeof(uint32_t))); CK(cudaMalloc(&B.q_miss, cap * sizeof(uint32_t)));   // one hit queue per material class
+        B.rng_carry = B.arrays.out<uint32_t>(cap);
+        B.q_hit = B.arrays.out<uint32_t>((size_t)MC_COUNT * cap); B.q_miss = B.arrays.out<uint32_t>(cap);   // one hit queue per material class
         B.cap = cap;
     }
     wave_cap_ = cap;
@@ -884,10 +845,10 @@ uint64_t Engine::bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, con
     const uint32_t par = k & 1u;
     const Queues q{ B.q_miss, B.q_hit, (uint32_t)wave_cap_ };
     uint64_t launches = 0;
-    if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts, par, B.sample_buf, B.rng_carry, st);
-    if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts, par, q, d_ctr_, k == 0, st); mark(1);
-    launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, flags, st); mark(2);
-    if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts, par, q, B.sample_buf, B.rng_carry, d_ctr_, flags, st); mark(3);
+    if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts.get(), par, B.sample_buf, B.rng_carry, st);
+    if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts.get(), par, q, d_ctr_.get(), k == 0, st); mark(1);
+    launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(2);
+    if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(3);
     return launches;
 }
 
@@ -943,7 +904,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     const int n_ctx = overlap ? 2 : 1;
     ensure_wave((size_t)F * P, n_ctx);                        // adaptive: A <= P, so F * P is the worst case of every interval's waves too
     if (!overlap) join_waves();                               // single-stream mode runs on the caller's stream, behind whatever the internal streams still hold
-    else CK(cudaEventRecord(image_free_ev_, stream_));        // what the caller has enqueued on the image so far (gather copy, post chain, set_hdr) precedes this call's resolves
+    else CK(cudaEventRecord(image_free_ev_.get(), stream_));        // what the caller has enqueued on the image so far (gather copy, post chain, set_hdr) precedes this call's resolves
     const DevConfig dc = make_dev_config();
     auto pcg = [](uint32_t in) { uint32_t st = in * 747796405u + 2891336453u; uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; };
 
@@ -957,8 +918,8 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     std::vector<int> prof_kind; size_t prof_n = 0;            // kind: 0 raygen 1 extend 2 shade 3 connect 4 resolve
     const std::function<void(int)> mark = [&](int kind) {
         if (!profiling_) return;
-        if (prof_n >= prof_ev_.size()) { cudaEvent_t e; CK(cudaEventCreate(&e)); prof_ev_.push_back(e); }
-        CK(cudaEventRecord(prof_ev_[prof_n++], stream_)); prof_kind.push_back(kind);
+        if (prof_n >= prof_ev_.size()) prof_ev_.push_back(make_event(cudaEventDefault));
+        CK(cudaEventRecord(prof_ev_[prof_n++].get(), stream_)); prof_kind.push_back(kind);
     };
     mark(-1);
     cudaStream_t last_st = stream_;
@@ -966,7 +927,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     // interval's end k_adaptive_update runs behind the last resolve and A is read back (one host sync per interval).
     for (uint32_t s0 = 0; s0 < todo;) {
         uint32_t seg = todo - s0, Pw = P, Fw = F;
-        const uint32_t *const act = adaptive ? d_active_ : nullptr;
+        const uint32_t *const act = adaptive ? d_active_.get() : nullptr;
         if (adaptive) {
             seg = (uint32_t)std::min<uint64_t>(seg, adaptive_.Interval - (dispatch_count_ + s0) % adaptive_.Interval);
             Pw = active_count_;
@@ -976,26 +937,27 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             const uint32_t nd = std::min(Fw, s0 + seg - w0);
             const int ctx = overlap ? (int)(wave_seq_ & 1ull) : 0;
             WaveBuf &B = wb_[ctx];
-            cudaStream_t st = overlap ? aux_stream_[ctx] : stream_;
-            if (w0 == 0) CK(cudaEventRecord(ev_[0], st));
+            cudaStream_t st = overlap ? aux_stream_[ctx].get() : stream_;
+            if (w0 == 0) CK(cudaEventRecord(ev_[0].get(), st));
             // this wave's slice of the dispatch table (PathTracer.cpp:127-150: FrameCount, Seed = PCG(seed + dispatch), ChunkIndex) travels on the wave's own stream
-            CK(cudaEventSynchronize(B.disp_ev));                  // the pinned copy is reusable once ITS last upload has executed
+            CK(cudaEventSynchronize(B.disp_ev.get()));                  // the pinned copy is reusable once ITS last upload has executed
             for (uint32_t i = 0; i < nd; i++) {
                 const uint64_t d = dispatch_count_ + w0 + i;
-                B.h_disp[i].FrameCount = (uint32_t)(d / S2); B.h_disp[i].Seed = pcg(base_seed + (uint32_t)d); B.h_disp[i].ChunkIndex = (uint32_t)(d % S2); B.h_disp[i]._pad = 0;
+                DevDispatch &hd = B.h_disp.get()[i];
+                hd.FrameCount = (uint32_t)(d / S2); hd.Seed = pcg(base_seed + (uint32_t)d); hd.ChunkIndex = (uint32_t)(d % S2); hd._pad = 0;
             }
-            CK(cudaMemcpyAsync(B.d_disp, B.h_disp, nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
-            CK(cudaEventRecord(B.disp_ev, st));
+            CK(cudaMemcpyAsync(B.d_disp.get(), B.h_disp.get(), nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
+            CK(cudaEventRecord(B.disp_ev.get(), st));
             PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
             if (!ds_.n_volumes) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
             const Queues q{ B.q_miss, B.q_hit, qcap };
             for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
                 const uint32_t wflags = (s == 0 && cp.store ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
                 if (cp.camera) {
-                    CK(cudaMemsetAsync(B.counts, 0, CTRL_WORDS * sizeof(uint32_t), st));   // before any CTA appends to the parity-0 queues
-                    launches += launch_camera(lc_, cp, ds_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
-                                              B.counts, q, d_ctr_, st, act);
-                } else launches += launch_raygen(lc_, dc, B.d_disp, nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts, d_ctr_, st, act);
+                    CK(cudaMemsetAsync(B.counts.get(), 0, CTRL_WORDS * sizeof(uint32_t), st));   // before any CTA appends to the parity-0 queues
+                    launches += launch_camera(lc_, cp, ds_, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
+                                              B.counts.get(), q, d_ctr_.get(), st, act);
+                } else launches += launch_raygen(lc_, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts.get(), d_ctr_.get(), st, act);
                 mark(0);
                 int cur = 0; uint32_t k = 0;
                 for (;;) {
@@ -1007,9 +969,9 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty
-                    CK(cudaMemcpyAsync(B.h_count, B.counts + (k & 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+                    CK(cudaMemcpyAsync(B.h_count.get(), B.counts.get() + (k & 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
                     CK(cudaStreamSynchronize(st));
-                    if (B.h_count[0] == 0) break;
+                    if (*B.h_count == 0) break;
                     if (k > (1u << 20)) break;                    // runaway guard
                 }
                 bounces_total += k;
@@ -1017,12 +979,12 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             // the running mean folds the waves in dispatch order: this wave's resolve waits for the previous wave's (the other stream, possibly an earlier call)
             // and for whatever the caller enqueued on the image before this call
             if (overlap) {
-                if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1], 0));
-                CK(cudaStreamWaitEvent(st, image_free_ev_, 0));
+                if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1].get(), 0));
+                CK(cudaStreamWaitEvent(st, image_free_ev_.get(), 0));
             }
-            if (tracked) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_, B.sample_buf, d_image_, d_px_state_, st);
-            else launch_resolve(lc_, dc, B.d_disp, nd, P, B.sample_buf, d_image_, st);
-            CK(cudaEventRecord(resolved_ev_[ctx], st));
+            if (tracked) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_.get(), B.sample_buf, d_image_.get(), d_px_state_.get(), st);
+            else launch_resolve(lc_, dc, B.d_disp.get(), nd, P, B.sample_buf, d_image_.get(), st);
+            CK(cudaEventRecord(resolved_ev_[ctx].get(), st));
             wave_seq_++;
             launches++; waves++; mark(4);
             last_st = st;
@@ -1035,7 +997,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             if (active_count_ == 0) { todo = s0; break; }     // the frames not traced do not count
         }
     }
-    CK(cudaEventRecord(ev_[1], last_st));                     // ms_total: first kernel of the first wave .. resolve of the last (counters() synchronises before reading it)
+    CK(cudaEventRecord(ev_[1].get(), last_st));                     // ms_total: first kernel of the first wave .. resolve of the last (counters() synchronises before reading it)
     timed_ = true;
     CK(cudaGetLastError());
     dispatch_count_ += todo;
@@ -1046,7 +1008,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     if (profiling_ && prof_n > 1) {
         CK(cudaStreamSynchronize(stream_));
         float *acc[5] = { &last_.ms_raygen, &last_.ms_extend, &last_.ms_shade, &last_.ms_connect, &last_.ms_resolve };
-        for (size_t i = 1; i < prof_n; i++) { float ms = 0.0f; CK(cudaEventElapsedTime(&ms, prof_ev_[i - 1], prof_ev_[i])); if (prof_kind[i] >= 0) *acc[prof_kind[i]] += ms; }
+        for (size_t i = 1; i < prof_n; i++) { float ms = 0.0f; CK(cudaEventElapsedTime(&ms, prof_ev_[i - 1].get(), prof_ev_[i].get())); if (prof_kind[i] >= 0) *acc[prof_kind[i]] += ms; }
     }
     return samples_accumulated_ >= cfg_.MaxSamplesAccumulated || (adaptive && active_count_ == 0);
 }
@@ -1054,7 +1016,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
 void Engine::set_stream(cudaStream_t s) {
     CK(cudaSetDevice(device_));
     sync_all();
-    stream_ = s ? s : own_stream_;
+    stream_ = s ? s : own_stream_.get();
 }
 
 void Engine::synchronize() { CK(cudaSetDevice(device_)); sync_all(); CK(cudaGetLastError()); }
@@ -1062,12 +1024,12 @@ void Engine::synchronize() { CK(cudaSetDevice(device_)); sync_all(); CK(cudaGetL
 b200pt_counters Engine::counters() {
     CK(cudaSetDevice(device_));
     sync_all();
-    WaveCounters wc; CK(cudaMemcpy(&wc, d_ctr_, sizeof wc, cudaMemcpyDeviceToHost));
+    WaveCounters wc; CK(cudaMemcpy(&wc, d_ctr_.get(), sizeof wc, cudaMemcpyDeviceToHost));
     b200pt_counters c = last_;
     c.paths = wc.paths; c.extend_rays = wc.extend_rays; c.shade_invocations = wc.shade_invocations; c.surface_hits = wc.surface_hits;
     c.misses = wc.misses; c.shadow_rays = wc.shadow_rays; c.medium_events = wc.medium_events;
     float ms = 0.0f;
-    if (timed_) CK(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));   // (querying never-recorded events would leave an error for the next call to find)
+    if (timed_) CK(cudaEventElapsedTime(&ms, ev_[0].get(), ev_[1].get()));   // (querying never-recorded events would leave an error for the next call to find)
     c.ms_total = ms;
     return c;
 }
@@ -1076,7 +1038,7 @@ void Engine::get_hdr(float *dst, bool dev) {
     CK(cudaSetDevice(device_));
     if (!d_image_ || !dst) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no image" };
     join_waves();
-    CK(cudaMemcpyAsync(dst, d_image_, (size_t)W_ * local_rows_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(dst, d_image_.get(), (size_t)W_ * local_rows_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
     if (!dev) CK(cudaStreamSynchronize(stream_));        // a device destination stays asynchronous on the engine's stream: the NCCL gather that follows is stream-ordered,
                                                           // and the host can already enqueue the next wave (no per-step bubble on multi-GPU runs)
 }
@@ -1084,7 +1046,7 @@ void Engine::set_hdr(const float *src, bool dev) {
     CK(cudaSetDevice(device_));
     if (!d_image_ || !src) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no image" };
     join_waves();
-    CK(cudaMemcpyAsync(d_image_, src, (size_t)W_ * local_rows_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(d_image_.get(), src, (size_t)W_ * local_rows_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream_));
     CK(cudaStreamSynchronize(stream_));
 }
 
@@ -1107,7 +1069,7 @@ void Engine::save_checkpoint(const char *path) {
     if (adaptive) {
         prepare_adaptive();
         px.resize((size_t)W_ * local_rows_);
-        CK(cudaMemcpy(px.data(), d_px_state_, px.size() * sizeof(uint4), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(px.data(), d_px_state_.get(), px.size() * sizeof(uint4), cudaMemcpyDeviceToHost));
     }
     CkptHeader h{}; memcpy(h.magic, "B2PTCKPT", 8); h.version = adaptive ? 2 : 1; h.W = W_; h.H = H_; h.rank = rank_; h.world = world_; h.band = band_; h.local_rows = local_rows_;
     h.frame_count = frame_count_; h.samples_accumulated = samples_accumulated_; h.samples_per_frame = cfg_.SamplesPerFrame; h.chunk_count = cfg_.ScreenChunkCount;
@@ -1144,27 +1106,27 @@ void Engine::load_checkpoint(const char *path) {
     set_hdr(img.data(), false);
     if (records()) {                                   // the records, then the active list rebuilt from their flags
         reset(); prepare_adaptive();
-        CK(cudaMemcpy(d_px_state_, px.data(), px.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d_px_state_.get(), px.data(), px.size() * sizeof(uint4), cudaMemcpyHostToDevice));
         update_active(false, stream_);
     }
     dispatch_count_ = h.dispatch_count; frame_count_ = h.frame_count; samples_accumulated_ = h.samples_accumulated;
 }
 
 // ---------------------------------------------------------------- PostProcessor (PostProcessor.cpp:128-246)
-void Engine::free_post() { for (auto &m : d_mips_) if (m) cudaFree(m); d_mips_.clear(); mip_wh_.clear(); dfree(d_ldr_); post_w_ = post_h_ = 0; }
+void Engine::free_post() { d_mips_.clear(); mip_wh_.clear(); d_ldr_.reset(); post_w_ = post_h_ = 0; }
 void Engine::ensure_post() {
     if (post_w_ == W_ && post_h_ == H_ && !d_mips_.empty()) return;
     free_post();
     uint32_t wh[20]; const uint32_t levels = bloom_mip_sizes(W_, H_, wh);                     // SetInputImage :128-158
-    for (uint32_t i = 0; i < levels; i++) { float4 *p = nullptr; CK(cudaMalloc(&p, (size_t)wh[2 * i] * wh[2 * i + 1] * sizeof(float4))); d_mips_.push_back(p); mip_wh_.push_back(wh[2 * i]); mip_wh_.push_back(wh[2 * i + 1]); }
-    CK(cudaMalloc(&d_ldr_, (size_t)W_ * H_ * sizeof(uchar4)));
+    for (uint32_t i = 0; i < levels; i++) { DevPtr<float4> p; CK(alloc(p, (size_t)wh[2 * i] * wh[2 * i + 1] * sizeof(float4))); d_mips_.push_back(std::move(p)); mip_wh_.push_back(wh[2 * i]); mip_wh_.push_back(wh[2 * i + 1]); }
+    CK(alloc(d_ldr_, (size_t)W_ * H_ * sizeof(uchar4)));
     post_w_ = W_; post_h_ = H_;
 }
 void Engine::accumulate_rows(const float4 *d_frame, uint32_t frame_index, uint32_t y0, uint32_t y1) {
     CK(cudaSetDevice(device_));
     if (!d_image_ || !d_frame || y0 >= y1 || y1 > H_ || world_ != 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "accumulate_rows: no image / bad rows / partitioned image" };
     join_waves();
-    launch_accumulate(d_frame, d_image_, y0 * W_, (y1 - y0) * W_, frame_index, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);
+    launch_accumulate(d_frame, d_image_.get(), y0 * W_, (y1 - y0) * W_, frame_index, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);
     CK(cudaGetLastError());
 }
 // HDR rows read by post_process_rows(y0, y1): the final kernel's rows y0-1 .. y1-1 and the first down pass's taps 2y-2 .. 2y+1 over D[1]
@@ -1193,7 +1155,7 @@ void Engine::post_process() { post_process_rows(0, H_); }
 void Engine::post_process_rows(uint32_t y0, uint32_t y1) {
     CK(cudaSetDevice(device_));
     if (!d_image_ || !W_ || !H_) throw CudaError{ B200PT_ERR_NO_SCENE, "PostProcess without an input image" };
-    post_chain(d_image_, y0, y1);
+    post_chain(d_image_.get(), y0, y1);
     post_denoised_ = false;
 }
 void Engine::post_chain(const float4 *src, uint32_t y0, uint32_t y1) {
@@ -1228,17 +1190,17 @@ void Engine::post_chain(const float4 *src, uint32_t y0, uint32_t y1) {
         auto rows_of = [&](const int r[2], int out[2]) { out[0] = r[0]; out[1] = r[1] + 1; };
         int r[2];
         rows_of(D[1], r);
-        launch_bloom_down_first(src, W_, H_, d_mips_[1], mip_wh_[2], mip_wh_[3], p, stream_, whole ? nullptr : r);                               // :200-226, i == 0 and i == 1
-        for (uint32_t i = 2; i < mips; i++) { rows_of(D[i], r); launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_, whole ? nullptr : r); }
-        for (uint32_t i = mips - 1; i > 1; i--) { rows_of(U[i - 1], r); launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_, whole ? nullptr : r); }   // :229-235
+        launch_bloom_down_first(src, W_, H_, d_mips_[1].get(), mip_wh_[2], mip_wh_[3], p, stream_, whole ? nullptr : r);                               // :200-226, i == 0 and i == 1
+        for (uint32_t i = 2; i < mips; i++) { rows_of(D[i], r); launch_bloom_down(d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_, whole ? nullptr : r); }
+        for (uint32_t i = mips - 1; i > 1; i--) { rows_of(U[i - 1], r); launch_bloom_up(d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_, whole ? nullptr : r); }   // :229-235
         r[0] = (int)y0; r[1] = (int)y1;
-        launch_bloom_final(src, d_mips_[1], mip_wh_[2], mip_wh_[3], d_ldr_, (keep_bloom_ && whole) ? d_mips_[0] : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
+        launch_bloom_final(src, d_mips_[1].get(), mip_wh_[2], mip_wh_[3], d_ldr_.get(), (keep_bloom_ && whole) ? d_mips_[0].get() : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
         bloom_valid_ = keep_bloom_ && whole;
     } else {
-        launch_bloom_threshold(src, d_mips_[0], W_ * H_, p, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);            // :200-226, i == 0
-        for (uint32_t i = 1; i < mips; i++) launch_bloom_down(d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_);
-        for (uint32_t i = mips - 1; i > 0; i--) launch_bloom_up(d_mips_[i], mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1], mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_);   // :229-235
-        launch_tonemap(src, d_mips_[0], d_ldr_, W_, H_, p, stream_);                           // :238-245
+        launch_bloom_threshold(src, d_mips_[0].get(), W_ * H_, p, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);            // :200-226, i == 0
+        for (uint32_t i = 1; i < mips; i++) launch_bloom_down(d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_);
+        for (uint32_t i = mips - 1; i > 0; i--) launch_bloom_up(d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_);   // :229-235
+        launch_tonemap(src, d_mips_[0].get(), d_ldr_.get(), W_, H_, p, stream_);                           // :238-245
         bloom_valid_ = true;
     }
     CK(cudaGetLastError());
@@ -1246,13 +1208,13 @@ void Engine::post_chain(const float4 *src, uint32_t y0, uint32_t y1) {
 void Engine::get_ldr_rows(uint32_t y0, uint32_t y1, uint8_t *dst, bool dev) {
     CK(cudaSetDevice(device_));
     if (!d_ldr_ || !dst || y0 >= y1 || y1 > H_) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process has not run / bad row range" };
-    CK(cudaMemcpyAsync(dst, reinterpret_cast<const uint8_t *>(d_ldr_) + (size_t)y0 * W_ * 4, (size_t)(y1 - y0) * W_ * 4, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(dst, reinterpret_cast<const uint8_t *>(d_ldr_.get()) + (size_t)y0 * W_ * 4, (size_t)(y1 - y0) * W_ * 4, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
     if (!dev) CK(cudaStreamSynchronize(stream_));
 }
 void Engine::get_ldr(uint8_t *dst, bool dev) {
     CK(cudaSetDevice(device_));
     if (!d_ldr_ || !dst) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process has not run" };
-    CK(cudaMemcpyAsync(dst, d_ldr_, (size_t)W_ * H_ * 4, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(dst, d_ldr_.get(), (size_t)W_ * H_ * 4, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
 }
 void Engine::get_bloom(float *dst) {
@@ -1260,9 +1222,9 @@ void Engine::get_bloom(float *dst) {
     if (d_mips_.empty() || !dst) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "post_process has not run" };
     if (!bloom_valid_) {                                                     // the fused chain skips mip 0 until somebody asks for it: re-run it on the same input
         keep_bloom_ = true;
-        if (post_denoised_ && has_denoised()) post_chain(d_dn_ + 2 * dn_pixels_, 0, H_); else post_process();
+        if (post_denoised_ && has_denoised()) post_chain(d_dn_.get() + 2 * dn_pixels_, 0, H_); else post_process();
     }
-    CK(cudaMemcpyAsync(dst, d_mips_[0], (size_t)W_ * H_ * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(dst, d_mips_[0].get(), (size_t)W_ * H_ * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
 }
 
@@ -1270,7 +1232,7 @@ void Engine::volume_walks(uint32_t n, const float *org, const float *dir, const 
     CK(cudaSetDevice(device_));
     if (!n) return;
     sync_all();
-    HookArrays a(stream_);
+    DeviceBlocks a(stream_);
     float *d_T = a.out<float>(n), *d_s = a.out<float>(n); int32_t *d_v = a.out<int32_t>(n); uint32_t *d_r = a.out<uint32_t>(2 * (size_t)n);
     launch_volume_walks(ds_, n, a.in(org, 3 * (size_t)n), a.in(dir, 3 * (size_t)n), a.in(seeds, n), ray_depth, d_T, d_s, d_v, d_r, stream_);
     a.get(T, d_T, n); a.get(scatter, d_s, n); a.get(vol, d_v, n); a.get(rng2, d_r, 2 * (size_t)n);
@@ -1290,7 +1252,7 @@ void Engine::trace_query(int shape, int kind, bool fma, uint32_t n, const float 
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
     if (!n) return;
-    HookArrays a(stream_);
+    DeviceBlocks a(stream_);
     const bool any = kind != TQ_CLOSEST, tgt = kind == TQ_TARGET;
     TraceQuery q{};
     q.n = n;
@@ -1320,7 +1282,7 @@ void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, c
             throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: instance or primitive out of range" };
         gid[i] = h_instances_[inst[i]].tri_base + prim[i];
     }
-    HookArrays a(stream_);
+    DeviceBlocks a(stream_);
     ShadeQuery q{};
     q.n = n; q.force_general = force_general;
     q.gid = a.in(gid.data(), n); q.rng = a.in(rng, n);
@@ -1338,7 +1300,7 @@ void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, con
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
     if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "miss_query: no environment map" };
     if (!n) return;
-    HookArrays a(stream_);
+    DeviceBlocks a(stream_);
     MissQuery q{};
     q.n = n;
     q.dir = a.in(dir, 3 * (size_t)n); q.depth = a.in(depth, n); q.pay_pdf = a.in(pay_pdf, n);
@@ -1392,8 +1354,8 @@ void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *ou
     CK(cudaMemcpyAsync(pst[cur].medium_g, medium_g.data(), (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
     CK(cudaMemcpyAsync(B.sample_buf, sample.data(), b4, cudaMemcpyHostToDevice, stream_));
     CK(cudaMemsetAsync(B.rng_carry, 0, (size_t)n * 4, stream_));
-    CK(cudaMemsetAsync(B.counts, 0, CTRL_WORDS * sizeof(uint32_t), stream_));
-    CK(cudaMemcpyAsync(B.counts + (k & 1u), &n, 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemsetAsync(B.counts.get(), 0, CTRL_WORDS * sizeof(uint32_t), stream_));
+    CK(cudaMemcpyAsync(B.counts.get() + (k & 1u), &n, 4, cudaMemcpyHostToDevice, stream_));
     CK(cudaStreamSynchronize(stream_));                       // (the pageable sources above are copied by now)
 
     const DevConfig dc = make_dev_config();
@@ -1405,7 +1367,7 @@ void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *ou
     std::vector<float> nx_g(n);
     std::vector<uint32_t> carry(n), ctrl(CTRL_WORDS);
     const PathState &dst = pst[cur ^ 1];
-    CK(cudaMemcpyAsync(ctrl.data(), B.counts, CTRL_WORDS * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(ctrl.data(), B.counts.get(), CTRL_WORDS * 4, cudaMemcpyDeviceToHost, stream_));
     CK(cudaMemcpyAsync(hit.data(), B.so.hit, b4, cudaMemcpyDeviceToHost, stream_));
     CK(cudaMemcpyAsync(sample.data(), B.sample_buf, b4, cudaMemcpyDeviceToHost, stream_));
     CK(cudaMemcpyAsync(carry.data(), B.rng_carry, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
@@ -1460,20 +1422,18 @@ void Engine::bake_lut(int kind, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t 
         slices = (uint32_t)std::max<size_t>(1, (want + n - 1) / n);
     }
     slices = std::min<uint32_t>(slices, 4096u);
-    float *d_part = nullptr, *d_tab = nullptr;
-    CK(cudaMalloc(&d_part, n * slices * sizeof(float)));
-    if (cudaMalloc(&d_tab, n * sizeof(float)) != cudaSuccess) { cudaFree(d_part); throw CudaError{ B200PT_ERR_OUT_OF_MEMORY, "bake_lut: out of device memory" }; }
-    cudaEvent_t e0 = nullptr, e1 = nullptr; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0, stream_);
-    launch_bake_lut(kind, d_part, d_tab, sx, sy, sz, sample_count, seed, slices, stream_);
-    cudaEventRecord(e1, stream_);
-    cudaError_t e = cudaMemcpyAsync(out_host, d_tab, n * sizeof(float), cudaMemcpyDeviceToHost, stream_);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    float ms = 0.0f; if (e == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
+    DevPtr<float> d_part, d_tab;
+    CK(alloc(d_part, n * slices * sizeof(float)));
+    if (alloc(d_tab, n * sizeof(float)) != cudaSuccess) throw CudaError{ B200PT_ERR_OUT_OF_MEMORY, "bake_lut: out of device memory" };
+    const Event e0 = make_event(cudaEventDefault), e1 = make_event(cudaEventDefault);
+    CK(cudaEventRecord(e0.get(), stream_));
+    launch_bake_lut(kind, d_part.get(), d_tab.get(), sx, sy, sz, sample_count, seed, slices, stream_);
+    CK(cudaEventRecord(e1.get(), stream_));
+    CK(cudaMemcpyAsync(out_host, d_tab.get(), n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    float ms = 0.0f; CK(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
     if (elapsed_ms) *elapsed_ms = ms;
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(d_part); cudaFree(d_tab);
-    CK(e);
 }
 // ---------------------------------------------------------------- denoiser (denoise_kernels.cu, DESIGN.md section 12)
 static void check_denoise_params(const b200pt_denoise_params &p) {
@@ -1483,13 +1443,13 @@ static void check_denoise_params(const b200pt_denoise_params &p) {
         if (!std::isfinite(v) || v < 0.0f) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise sigmas must be finite and >= 0" };
 }
 static uint32_t pcg_host(uint32_t in) { const uint32_t st = in * 747796405u + 2891336453u; const uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; }
-void Engine::free_denoise() { dfree(d_dn_); dn_pixels_ = 0; dn_w_ = dn_h_ = 0; }   // (d_dn_img_ is sized by the caller's images: freed with the engine)
+void Engine::free_denoise() { d_dn_.reset(); dn_pixels_ = 0; dn_w_ = dn_h_ = 0; }   // (d_dn_img_ is sized by the caller's images: freed with the engine)
 void Engine::ensure_denoise() {
     const size_t n = (size_t)W_ * local_rows_;
     if (d_dn_ && n == dn_pixels_) return;
     sync_all();
     free_denoise();
-    CK(cudaMalloc(&d_dn_, std::max<size_t>(n, 1) * (6 * sizeof(float4) + sizeof(float))));
+    CK(alloc(d_dn_, std::max<size_t>(n, 1) * (6 * sizeof(float4) + sizeof(float))));
     dn_pixels_ = n;
 }
 void Engine::run_features(const b200pt_denoise_params &p) {
@@ -1507,36 +1467,32 @@ void Engine::run_features(const b200pt_denoise_params &p) {
     for (int k = 0; k < 3; k++) d[k] = (VI[k] * t[0] + VI[4 + k] * t[1] + VI[8 + k] * t[2]) / tl;
     const double dl = std::sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
     const float3 fwd = make_float3((float)(d[0] / dl), (float)(d[1] / dl), (float)(d[2] / dl));
-    CK((cudaError_t)launch_features(lc_, ds_, make_dev_config(), fwd, p.FeatureSamples, pcg_host(0x46454154u), d_dn_, d_dn_ + n, stream_));
-    launch_record_variance(d_px_state_, (uint32_t)n, reinterpret_cast<float *>(d_dn_ + 6 * n), stream_);
+    CK((cudaError_t)launch_features(lc_, ds_, make_dev_config(), fwd, p.FeatureSamples, pcg_host(0x46454154u), d_dn_.get(), d_dn_.get() + n, stream_));
+    launch_record_variance(d_px_state_.get(), (uint32_t)n, reinterpret_cast<float *>(d_dn_.get() + 6 * n), stream_);
     CK(cudaGetLastError());
 }
 void Engine::denoise(const b200pt_denoise_params &p, float *elapsed_ms) {
     CK(cudaSetDevice(device_));
     check_denoise_params(p);
     if (world_ != 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "denoise needs the full image (world 1): gather b200pt_get_denoise_inputs and use b200pt_denoise_image" };
-    cudaEvent_t e[2] = { nullptr, nullptr };
-    CK(cudaEventCreate(&e[0])); CK(cudaEventCreate(&e[1]));
-    try {
-        join_waves();                                         // the timed window starts behind the render's waves
-        CK(cudaEventRecord(e[0], stream_));
-        run_features(p);
-        const size_t n = dn_pixels_;
-        launch_denoise_filter(W_, H_, d_image_, d_dn_, d_dn_ + n, reinterpret_cast<const float *>(d_dn_ + 6 * n), p.Iterations, p.SigmaLuminance, p.SigmaNormal,
-                              p.SigmaDepth, d_dn_ + 3 * n, d_dn_ + 2 * n, stream_);
-        CK(cudaEventRecord(e[1], stream_));
-        CK(cudaStreamSynchronize(stream_));
-        CK(cudaGetLastError());
-        float ms = 0.0f; CK(cudaEventElapsedTime(&ms, e[0], e[1]));
-        if (elapsed_ms) *elapsed_ms = ms;
-        dn_w_ = W_; dn_h_ = H_;
-    } catch (...) { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); throw; }
-    cudaEventDestroy(e[0]); cudaEventDestroy(e[1]);
+    const Event e0 = make_event(cudaEventDefault), e1 = make_event(cudaEventDefault);
+    join_waves();                                             // the timed window starts behind the render's waves
+    CK(cudaEventRecord(e0.get(), stream_));
+    run_features(p);
+    const size_t n = dn_pixels_;
+    launch_denoise_filter(W_, H_, d_image_.get(), d_dn_.get(), d_dn_.get() + n, reinterpret_cast<const float *>(d_dn_.get() + 6 * n), p.Iterations, p.SigmaLuminance, p.SigmaNormal,
+                          p.SigmaDepth, d_dn_.get() + 3 * n, d_dn_.get() + 2 * n, stream_);
+    CK(cudaEventRecord(e1.get(), stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    float ms = 0.0f; CK(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+    if (elapsed_ms) *elapsed_ms = ms;
+    dn_w_ = W_; dn_h_ = H_;
 }
 void Engine::get_denoised(float *dst, bool dev) {
     CK(cudaSetDevice(device_));
     if (!dst || !has_denoised()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no denoised image of the current size (b200pt_denoise first)" };
-    CK(cudaMemcpyAsync(dst, d_dn_ + 2 * dn_pixels_, (size_t)W_ * H_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(dst, d_dn_.get() + 2 * dn_pixels_, (size_t)W_ * H_ * sizeof(float4), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
 }
 void Engine::denoise_inputs(const b200pt_denoise_params &p, float *albedo_cov, float *normal_depth, float *variance) {
@@ -1544,9 +1500,9 @@ void Engine::denoise_inputs(const b200pt_denoise_params &p, float *albedo_cov, f
     check_denoise_params(p);
     run_features(p);
     const size_t n = dn_pixels_;
-    if (albedo_cov) CK(cudaMemcpyAsync(albedo_cov, d_dn_, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
-    if (normal_depth) CK(cudaMemcpyAsync(normal_depth, d_dn_ + n, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
-    if (variance) CK(cudaMemcpyAsync(variance, d_dn_ + 6 * n, n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+    if (albedo_cov) CK(cudaMemcpyAsync(albedo_cov, d_dn_.get(), n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+    if (normal_depth) CK(cudaMemcpyAsync(normal_depth, d_dn_.get() + n, n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+    if (variance) CK(cudaMemcpyAsync(variance, d_dn_.get() + 6 * n, n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
     CK(cudaGetLastError());
 }
@@ -1557,10 +1513,10 @@ void Engine::denoise_image(uint32_t w, uint32_t h, const float *color, const flo
     if (!w || !h || w > 65535 || h > 65535) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bad image size" };
     const size_t n = (size_t)w * h, bytes = n * (dev ? 3 : 7) * sizeof(float4) + (dev ? 0 : n * sizeof(float));
     if (bytes > dn_img_bytes_) {                              // kept for the next call: repeated calls allocate nothing
-        sync_all(); dfree(d_dn_img_); dn_img_bytes_ = 0;
-        CK(cudaMalloc(&d_dn_img_, bytes)); dn_img_bytes_ = bytes;
+        sync_all(); dn_img_bytes_ = 0;
+        CK(alloc(d_dn_img_, bytes)); dn_img_bytes_ = bytes;
     }
-    float4 *const buf = d_dn_img_;                            // [scratch 3n | device copies of the inputs and the output when they are host memory]
+    float4 *const buf = d_dn_img_.get();                            // [scratch 3n | device copies of the inputs and the output when they are host memory]
     const float4 *c = reinterpret_cast<const float4 *>(color), *a = reinterpret_cast<const float4 *>(albedo_cov), *nd = reinterpret_cast<const float4 *>(normal_depth);
     const float *v = variance; float4 *o = reinterpret_cast<float4 *>(out);
     cudaError_t e = cudaSuccess;
@@ -1583,7 +1539,7 @@ void Engine::denoise_image(uint32_t w, uint32_t h, const float *color, const flo
 void Engine::post_process_denoised() {
     CK(cudaSetDevice(device_));
     if (!has_denoised()) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "no denoised image of the current size (b200pt_denoise first)" };
-    post_chain(d_dn_ + 2 * dn_pixels_, 0, H_);
+    post_chain(d_dn_.get() + 2 * dn_pixels_, 0, H_);
     post_denoised_ = true;
 }
 void Engine::scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const {
@@ -1598,16 +1554,16 @@ void Engine::ploc_build_query(const float *ref_boxes, uint32_t n, BvhNode *nodes
     *n_out = 0; *depth_out = 0; *n4_out = 0; *depth4_out = 0;
     for (size_t i = 0; i < (size_t)n; i++)
         for (int a = 0; a < 3; a++) if (!(ref_boxes[i * 6 + a] <= ref_boxes[i * 6 + 3 + a])) return;
-    HookArrays a(stream_);
+    DeviceBlocks a(stream_);
     const float *box = a.in(ref_boxes, (size_t)n * 6);
     BvhNode *nodes = a.out<BvhNode>(n - 1); uint32_t *perm = a.out<uint32_t>(n);
     uint32_t n2 = 0; int d2 = 0;
-    int r = ploc_build(box, n, nodes, perm, &n2, &d2, h_small_, stream_);
+    int r = ploc_build(box, n, nodes, perm, &n2, &d2, h_small_.get(), stream_);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("ploc_build failed: ") + cudaGetErrorString((cudaError_t)r) };
     if (n2 == 0) return;
     Bvh4Node *nodes4 = a.out<Bvh4Node>(n2);
     uint32_t n4 = 0; int d4 = 0;
-    r = bvh4_collapse_device(nodes, n2, 0, nodes4, &n4, &d4, h_small_, stream_);
+    r = bvh4_collapse_device(nodes, n2, 0, nodes4, &n4, &d4, h_small_.get(), stream_);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("bvh4_collapse_device failed: ") + cudaGetErrorString((cudaError_t)r) };
     a.get(nodes_out, nodes, n2); a.get(perm_out, perm, n);
     if (n4) a.get(nodes4_out, nodes4, n4);

@@ -3,6 +3,7 @@
 #pragma once
 #include "host_api.h"
 #include "kernels.h"
+#include "cuda_resources.h"
 #include <cuda_runtime.h>
 #include <functional>
 
@@ -77,7 +78,7 @@ public:
     void set_profiling(bool on) { profiling_ = on; }
     void get_hdr(float *dst, bool dst_is_device);
     void set_hdr(const float *src, bool src_is_device);
-    float4 *hdr_device() { return d_image_; }
+    float4 *hdr_device() { return d_image_.get(); }
     // checkpoint / resume of the accumulation (SURVEY 5 "checkpoint / resume", 8f row 4): image + dispatch bookkeeping
     void save_checkpoint(const char *path);
     void load_checkpoint(const char *path);
@@ -133,10 +134,11 @@ private:
     void check(cudaError_t e, const char *what) const;
 
     int device_;
-    cudaStream_t stream_ = nullptr, own_stream_ = nullptr;
+    Stream own_stream_, aux_stream_[2];             // declared first: destroyed after every member that may still be in use on them
+    cudaStream_t stream_ = nullptr;                 // own_stream_ or the caller's (set_stream)
     bool profiling_ = false;
-    std::vector<cudaEvent_t> prof_ev_;
-    cudaEvent_t ev_[2] = { nullptr, nullptr };
+    std::vector<Event> prof_ev_;
+    Event ev_[2];
     bool timed_ = false;                            // ev_ have been recorded (by a path_trace call that launched work)
 
     HostScene scene_;
@@ -149,20 +151,20 @@ private:
 
     // device scene
     DevScene ds_{};
-    b200pt_vertex *d_verts_ = nullptr; uint32_t *d_indices_ = nullptr; DevMesh *d_meshes_ = nullptr; DevInstance *d_instances_ = nullptr;
-    DevMaterial *d_materials_ = nullptr; DevTexture *d_textures_ = nullptr; DevEmissive *d_emissive_ = nullptr; EmTri *d_em_tris_ = nullptr; uint32_t *d_em_tri_base_ = nullptr;
-    std::vector<uint8_t *> d_texdata_;
+    DevPtr<b200pt_vertex> d_verts_; DevPtr<uint32_t> d_indices_; DevPtr<DevMesh> d_meshes_; DevPtr<DevInstance> d_instances_;
+    DevPtr<DevMaterial> d_materials_; DevPtr<DevTexture> d_textures_; DevPtr<DevEmissive> d_emissive_; DevPtr<EmTri> d_em_tris_; DevPtr<uint32_t> d_em_tri_base_;
+    std::vector<DevPtr<uint8_t>> d_texdata_;
     std::vector<DevInstance> h_instances_; std::vector<DevMesh> h_meshes_;
-    float4 *d_env_ = nullptr; uint2 *d_alias_ = nullptr; float2 *d_env_row_cos_ = nullptr; float *d_luts_[3] = { nullptr, nullptr, nullptr };
-    std::vector<b200pt_volume> volumes_; uint32_t phase_function_ = 0; DevVolume *d_volumes_ = nullptr;
-    struct GridData { PreparedGrid host; float *d_values = nullptr, *d_max_densities = nullptr; ~GridData(); };
+    DevPtr<float4> d_env_; DevPtr<uint2> d_alias_; DevPtr<float2> d_env_row_cos_; DevPtr<float> d_luts_[3];
+    std::vector<b200pt_volume> volumes_; uint32_t phase_function_ = 0; DevPtr<DevVolume> d_volumes_;
+    struct GridData { PreparedGrid host; DevPtr<float> d_values, d_max_densities; };
     std::vector<std::shared_ptr<GridData>> grids_;      // parallel to volumes_: density data of the heterogeneous ones (nullptr: homogeneous)
-    DevGrid *d_grids_ = nullptr; int density_data_counter_ = 0;   // PathTracer.cpp:1508-1513: slots are handed out round-robin
+    DevPtr<DevGrid> d_grids_; int density_data_counter_ = 0;   // PathTracer.cpp:1508-1513: slots are handed out round-robin
     b200pt_atmosphere atmosphere_{};
     LbvhResult bvh_{};
     LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
-    uint32_t *h_small_ = nullptr;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
-    void *d_scratch_ = nullptr; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices and pose
+    PinnedPtr<uint32_t> h_small_;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
+    DevPtr<uint8_t> d_scratch_; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices and pose
     void *scratch(size_t bytes);
     // the commit of update_instance_transforms, update_mesh_vertices and pose: the listed meshes' whole vertex arrays (host memory, or device
     // memory on the stream) and, when given, every instance transform; one refit / rebuild; ResetPathTracing.  A failure restores both.
@@ -171,38 +173,39 @@ private:
     // rest data of the deformable meshes of a glTF scene (pose_kernels.cu), uploaded by set_scene; nothing for other scenes
     void upload_pose_data();
     void free_pose_data();
-    std::vector<void *> d_pose_blocks_;             // every device allocation behind pose_dev_
+    DeviceBlocks pose_blocks_;                      // every device allocation behind pose_dev_
     PoseDev pose_dev_{};
     std::vector<PoseMesh> pose_meshes_;             // HostAnimation::deformable order
     uint32_t pose_grid_ = 0, pose_max_joints_ = 0, pose_vertices_ = 0, pose_palette_floats_ = 0, pose_morph_floats_ = 0;
     bool pose_gen_normals_ = false;
     LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
-    uint8_t *d_tri_class_ = nullptr; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c
+    DevPtr<uint8_t> d_tri_class_; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c
 
     // framebuffer + post
-    float4 *d_image_ = nullptr; size_t image_pixels_ = 0;
+    DevPtr<float4> d_image_; size_t image_pixels_ = 0;
     b200pt_tonemap tonemap_{ 1.0f, 2.2f };
     b200pt_bloom bloom_{ 2.0f, 1.0f, 10, 5.0f };
-    std::vector<float4 *> d_mips_; std::vector<uint32_t> mip_wh_; uchar4 *d_ldr_ = nullptr; uint32_t post_w_ = 0, post_h_ = 0;
+    std::vector<DevPtr<float4>> d_mips_; std::vector<uint32_t> mip_wh_; DevPtr<uchar4> d_ldr_; uint32_t post_w_ = 0, post_h_ = 0;
     bool keep_bloom_ = false, bloom_valid_ = false;   // fused post chain: mip 0 is written only once get_bloom() has been used
 
     // wave buffers: one context per wave in flight.  Two contexts on two internal streams let the latency-bound tail of wave w (late bounces: few, long rays)
     // overlap the full-machine head of wave w+1; k_resolve runs in dispatch order (events), so the image does not depend on it.
     struct WaveBuf {
+        DeviceBlocks arrays;                        // the cap-sized arrays below, from ps to q_miss
         PathState ps[2]{}; ShadeOut so{};
         float4 *sample_buf = nullptr; uint32_t *rng_carry = nullptr; uint32_t *q_hit = nullptr, *q_miss = nullptr;
-        uint32_t *counts = nullptr, *h_count = nullptr;
-        DevDispatch *d_disp = nullptr, *h_disp = nullptr; cudaEvent_t disp_ev = nullptr;   // this context's slice of the dispatch table (pinned host copy reusable once disp_ev has fired)
+        DevPtr<uint32_t> counts; PinnedPtr<uint32_t> h_count;
+        DevPtr<DevDispatch> d_disp; PinnedPtr<DevDispatch> h_disp; Event disp_ev;   // this context's slice of the dispatch table (pinned host copy reusable once disp_ev has fired)
         size_t cap = 0;
     };
     WaveBuf wb_[2];
-    cudaStream_t aux_stream_[2] = { nullptr, nullptr }; cudaEvent_t resolved_ev_[2] = { nullptr, nullptr }, image_free_ev_ = nullptr;
+    Event resolved_ev_[2], image_free_ev_;
     uint64_t wave_seq_ = 0;                         // waves launched so far: wave w runs in context w & 1 and resolves after wave w - 1
     size_t wave_cap_ = 0;                           // capacity (paths) of every allocated context
     void sync_all();                                // the caller's stream AND the internal wave streams are idle
     void join_waves();                              // work enqueued on the caller's stream from here on sees every launched wave resolved into the image
-    WaveCounters *d_ctr_ = nullptr;
+    DevPtr<WaveCounters> d_ctr_;
     b200pt_counters last_{};
     bool scene_has_media() const;                   // can a path random-walk inside a mesh without gaining Depth?
     // bounce k of a sub-wave in context B: the paths of pst[cur] (control word k & 1) are traced and shaded, the survivors written to
@@ -212,8 +215,8 @@ private:
 
     // adaptive sampling: allocated only while enabled.  The state is rebuilt lazily (prepare_adaptive) after every reset.
     b200pt_adaptive adaptive_{};
-    uint4 *d_px_state_ = nullptr;                   // one record per local pixel (kernels.h: meanL, M2, n_p, flags)
-    uint32_t *d_active_ = nullptr, *d_tile_count_ = nullptr, *d_active_count_ = nullptr, *h_active_count_ = nullptr;
+    DevPtr<uint4> d_px_state_;                      // one record per local pixel (kernels.h: meanL, M2, n_p, flags)
+    DevPtr<uint32_t> d_active_, d_tile_count_, d_active_count_; PinnedPtr<uint32_t> h_active_count_;
     size_t adaptive_pixels_ = 0;                    // local pixels the buffers were sized for
     uint32_t active_count_ = 0;                     // A: entries of d_active_ (host copy, read back at every interval boundary)
     bool adaptive_ready_ = false;                   // the state matches the accumulation (false after reset)
@@ -224,9 +227,9 @@ private:
     bool records() const { return adaptive_.Enable != 0u || track_variance_; }
 
     // denoiser: one allocation of W * local_rows pixels = [features 2n float4 | denoised n float4 | filter scratch 3n float4 | variance n float]
-    float4 *d_dn_ = nullptr; size_t dn_pixels_ = 0;
+    DevPtr<float4> d_dn_; size_t dn_pixels_ = 0;
     uint32_t dn_w_ = 0, dn_h_ = 0;                  // size of the image the denoised buffer holds (0: none)
-    float4 *d_dn_img_ = nullptr; size_t dn_img_bytes_ = 0;   // denoise_image: filter scratch (+ device copies of host arrays)
+    DevPtr<float4> d_dn_img_; size_t dn_img_bytes_ = 0;   // denoise_image: filter scratch (+ device copies of host arrays)
     bool post_denoised_ = false;                    // the last post pass read the denoised image (get_bloom re-runs it on the same input)
     void ensure_denoise();
     void free_denoise();

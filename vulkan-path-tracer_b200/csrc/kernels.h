@@ -1,6 +1,7 @@
 // kernels.h -- host-callable launchers of the sm_90a kernels (wavefront_kernels.cu, lbvh.cu, post_kernels.cu, denoise_kernels.cu, trace_query.cu)
 #pragma once
 #include "device_types.h"
+#include "cuda_resources.h"
 #include <cuda_runtime.h>
 #include <vector>
 
@@ -136,7 +137,7 @@ struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri 
 // Returns cudaError_t as int.
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
                const DevInstance *h_instances, const DevMesh *h_meshes, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes = false,
-               float **dev_ref_box = nullptr);   // dev_ref_box: receives the Morton-ordered per-slot reference boxes (device, n_tris x 6; the caller frees)
+               DevPtr<float> *dev_ref_box = nullptr);   // dev_ref_box: receives the Morton-ordered per-slot reference boxes (device, n_tris x 6)
 void lbvh_free(LbvhResult *r);
 // BVH2 -> BVH4 on the host (pure CPU code, unit-tested without a GPU through b200pt_bvh4_collapse).  `out` must hold n_nodes2 entries.
 // Returns the number of BVH4 nodes written (0 if the root is a leaf), *depth4 = depth of the BVH4 (root = 1).
@@ -161,8 +162,8 @@ int ploc_build(const float *d_ref_box, uint32_t n, BvhNode *d_out, uint32_t *d_p
 int bvh4_collapse_device(const BvhNode *d_nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *d_out, uint32_t *n4, int *depth4, uint32_t *h_small, cudaStream_t st);
 // The GPU rebuild of an LBVH (update_instance_transforms(rebuild == 2)): ploc_build over the Morton-ordered reference boxes lbvh_build kept on the
 // device, then the BvhTri slots permuted and tri_slot re-derived on the device.  A tree deeper than BVH_STACK_MAX - 2 and than the LBVH is
-// dropped (the LBVH stays).  Frees d_ref_box.  Returns cudaError_t as int.
-int lbvh_ploc_rebuild(LbvhResult *r, float *d_ref_box, uint32_t *h_small, cudaStream_t st);
+// dropped (the LBVH stays).  Returns cudaError_t as int.
+int lbvh_ploc_rebuild(LbvhResult *r, DevPtr<float> ref_box, uint32_t *h_small, cudaStream_t st);
 // lbvh_build_wide with the collapse on the device (scratch of n_nodes BVH4 nodes; r->nodes4 is allocated at the exact size).
 int lbvh_build_wide_device(LbvhResult *r, uint32_t *h_small, cudaStream_t st);
 // mode 1: inner nodes only (download, rebuild, upload in place); mode 2: full build from r->h_ref_box, reference slots and tri_slot permuted

@@ -1148,8 +1148,8 @@ void lbvh_free(LbvhResult *r) {
 
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
                const DevInstance *, const DevMesh *, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes,
-               float **dev_ref_box) {
-    if (dev_ref_box) *dev_ref_box = nullptr;
+               DevPtr<float> *dev_ref_box) {
+    if (dev_ref_box) dev_ref_box->reset();
     out->shade = nullptr; out->tri_slot = nullptr; out->h_ref_box = nullptr; out->n_prims = n_tris;
     out->nodes = nullptr; out->tris = nullptr; out->n_nodes = 0; out->n_tris = n_tris; out->root = 0; out->max_depth = 1; out->bytes = 0;
     out->nodes4 = nullptr; out->n_nodes4 = 0; out->depth4 = 0;
@@ -1157,63 +1157,61 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
     const uint32_t nt = n_tris, ntblocks = (nt + 255) / 256;
 
     // ---- per-triangle stage: world-space triangles, shading records (final, gid order), boxes, scene bounds, split counts
-    ShadeTri *shade = nullptr; BvhTri *tmp = nullptr; float *aabb = nullptr, *bounds = nullptr; uint32_t *ksplit = nullptr, *ref_off = nullptr;
-    LBVH_CHECK(cudaMalloc(&shade, (size_t)nt * sizeof(ShadeTri)));
-    uint32_t *tri_slot = nullptr;
-    LBVH_CHECK(cudaMalloc(&tri_slot, (size_t)nt * sizeof(uint32_t)));
-    LBVH_CHECK(cudaMalloc(&tmp, (size_t)nt * sizeof(BvhTri)));
-    LBVH_CHECK(cudaMalloc(&aabb, (size_t)nt * 6 * sizeof(float)));
-    LBVH_CHECK(cudaMalloc(&bounds, 6 * sizeof(float)));
-    LBVH_CHECK(cudaMalloc(&ksplit, (size_t)nt * 4)); LBVH_CHECK(cudaMalloc(&ref_off, (size_t)nt * 4));
+    DevPtr<ShadeTri> shade; DevPtr<uint32_t> tri_slot, ksplit, ref_off; DevPtr<BvhTri> tmp; DevPtr<float> aabb, bounds;
+    LBVH_CHECK(alloc(shade, (size_t)nt * sizeof(ShadeTri)));
+    LBVH_CHECK(alloc(tri_slot, (size_t)nt * sizeof(uint32_t)));
+    LBVH_CHECK(alloc(tmp, (size_t)nt * sizeof(BvhTri)));
+    LBVH_CHECK(alloc(aabb, (size_t)nt * 6 * sizeof(float)));
+    LBVH_CHECK(alloc(bounds, 6 * sizeof(float)));
+    LBVH_CHECK(alloc(ksplit, (size_t)nt * 4)); LBVH_CHECK(alloc(ref_off, (size_t)nt * 4));
     const float binit[6] = { 3.0e38f, 3.0e38f, 3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f };
-    LBVH_CHECK(cudaMemcpyAsync(bounds, binit, sizeof(binit), cudaMemcpyHostToDevice, st));
-    k_world_tris<<<ntblocks, 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, n_instances, nt, tmp, shade, aabb, bounds);
-    k_split_count<<<ntblocks, 256, 0, st>>>(tmp, aabb, bounds, nt, ksplit);
+    LBVH_CHECK(cudaMemcpyAsync(bounds.get(), binit, sizeof(binit), cudaMemcpyHostToDevice, st));
+    k_world_tris<<<ntblocks, 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, n_instances, nt, tmp.get(), shade.get(), aabb.get(), bounds.get());
+    k_split_count<<<ntblocks, 256, 0, st>>>(tmp.get(), aabb.get(), bounds.get(), nt, ksplit.get());
     std::vector<uint32_t> hk(nt), hoff(nt);
-    LBVH_CHECK(cudaMemcpyAsync(hk.data(), ksplit, (size_t)nt * 4, cudaMemcpyDeviceToHost, st));
+    LBVH_CHECK(cudaMemcpyAsync(hk.data(), ksplit.get(), (size_t)nt * 4, cudaMemcpyDeviceToHost, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     uint64_t total = 0; for (uint32_t i = 0; i < nt; i++) { hoff[i] = (uint32_t)total; total += hk[i]; }
     if (total >= (1ull << 28)) return (int)cudaErrorMemoryAllocation;       // leaf references keep the slot in 28 bits
-    LBVH_CHECK(cudaMemcpyAsync(ref_off, hoff.data(), (size_t)nt * 4, cudaMemcpyHostToDevice, st));
+    LBVH_CHECK(cudaMemcpyAsync(ref_off.get(), hoff.data(), (size_t)nt * 4, cudaMemcpyHostToDevice, st));
 
     // ---- per-reference stage
     const uint32_t n = (uint32_t)total, n_int = n > 1 ? n - 1 : 0, n_nodes_alloc = n_int ? n_int : 1;
     const size_t node_bytes = (size_t)n_nodes_alloc * sizeof(BvhNode), tri_bytes = (size_t)n * sizeof(BvhTri);
-    unsigned char *blob = nullptr;
-    LBVH_CHECK(cudaMalloc(&blob, node_bytes + tri_bytes));
-    LBVH_CHECK(cudaMemsetAsync(blob, 0, node_bytes, st));
-    BvhNode *nodes = reinterpret_cast<BvhNode *>(blob);
-    BvhTri *tris = reinterpret_cast<BvhTri *>(blob + node_bytes);
-    float *ref_box = nullptr, *leaf_box = nullptr, *node_box = nullptr; uint32_t *ref_tri = nullptr;
-    unsigned long long *keys = nullptr, *keys2 = nullptr; uint32_t *vals = nullptr, *vals2 = nullptr, *hist = nullptr;
-    int *left = nullptr, *right = nullptr, *parent_int = nullptr, *parent_leaf = nullptr; unsigned int *flags = nullptr; int2 *range = nullptr;
+    DevPtr<unsigned char> blob;
+    LBVH_CHECK(alloc(blob, node_bytes + tri_bytes));
+    LBVH_CHECK(cudaMemsetAsync(blob.get(), 0, node_bytes, st));
+    BvhNode *nodes = reinterpret_cast<BvhNode *>(blob.get());
+    BvhTri *tris = reinterpret_cast<BvhTri *>(blob.get() + node_bytes);
+    DevPtr<float> ref_box, leaf_box, node_box; DevPtr<uint32_t> ref_tri, vals, vals2, hist; DevPtr<unsigned long long> keys, keys2;
+    DevPtr<int> left, right, parent_int, parent_leaf; DevPtr<unsigned int> flags; DevPtr<int2> range;
     const uint32_t nblocks = (n + 255) / 256;
-    LBVH_CHECK(cudaMalloc(&ref_box, (size_t)n * 6 * sizeof(float))); LBVH_CHECK(cudaMalloc(&ref_tri, (size_t)n * 4));
-    LBVH_CHECK(cudaMalloc(&leaf_box, (size_t)n * 6 * sizeof(float)));
-    LBVH_CHECK(cudaMalloc(&node_box, (size_t)n_nodes_alloc * 6 * sizeof(float)));
-    LBVH_CHECK(cudaMalloc(&keys, (size_t)n * 8)); LBVH_CHECK(cudaMalloc(&vals, (size_t)n * 4));
-    LBVH_CHECK(cudaMalloc(&keys2, (size_t)n * 8)); LBVH_CHECK(cudaMalloc(&vals2, (size_t)n * 4));
-    LBVH_CHECK(cudaMalloc(&hist, (size_t)16 * nblocks * 4));
-    LBVH_CHECK(cudaMalloc(&range, (size_t)n_nodes_alloc * sizeof(int2)));
-    LBVH_CHECK(cudaMalloc(&left, (size_t)n_nodes_alloc * 4)); LBVH_CHECK(cudaMalloc(&right, (size_t)n_nodes_alloc * 4));
-    LBVH_CHECK(cudaMalloc(&parent_int, (size_t)n_nodes_alloc * 4)); LBVH_CHECK(cudaMalloc(&parent_leaf, (size_t)n * 4));
-    LBVH_CHECK(cudaMalloc(&flags, (size_t)n_nodes_alloc * 4));
-    LBVH_CHECK(cudaMemsetAsync(flags, 0, (size_t)n_nodes_alloc * 4, st));
-    LBVH_CHECK(cudaMemsetAsync(parent_leaf, 0xFF, (size_t)n * 4, st));
+    LBVH_CHECK(alloc(ref_box, (size_t)n * 6 * sizeof(float))); LBVH_CHECK(alloc(ref_tri, (size_t)n * 4));
+    LBVH_CHECK(alloc(leaf_box, (size_t)n * 6 * sizeof(float)));
+    LBVH_CHECK(alloc(node_box, (size_t)n_nodes_alloc * 6 * sizeof(float)));
+    LBVH_CHECK(alloc(keys, (size_t)n * 8)); LBVH_CHECK(alloc(vals, (size_t)n * 4));
+    LBVH_CHECK(alloc(keys2, (size_t)n * 8)); LBVH_CHECK(alloc(vals2, (size_t)n * 4));
+    LBVH_CHECK(alloc(hist, (size_t)16 * nblocks * 4));
+    LBVH_CHECK(alloc(range, (size_t)n_nodes_alloc * sizeof(int2)));
+    LBVH_CHECK(alloc(left, (size_t)n_nodes_alloc * 4)); LBVH_CHECK(alloc(right, (size_t)n_nodes_alloc * 4));
+    LBVH_CHECK(alloc(parent_int, (size_t)n_nodes_alloc * 4)); LBVH_CHECK(alloc(parent_leaf, (size_t)n * 4));
+    LBVH_CHECK(alloc(flags, (size_t)n_nodes_alloc * 4));
+    LBVH_CHECK(cudaMemsetAsync(flags.get(), 0, (size_t)n_nodes_alloc * 4, st));
+    LBVH_CHECK(cudaMemsetAsync(parent_leaf.get(), 0xFF, (size_t)n * 4, st));
 
-    k_make_refs<<<ntblocks, 256, 0, st>>>(tmp, aabb, ksplit, ref_off, nt, ref_box, ref_tri);
-    k_morton<<<nblocks, 256, 0, st>>>(ref_box, bounds, n, keys, vals);
+    k_make_refs<<<ntblocks, 256, 0, st>>>(tmp.get(), aabb.get(), ksplit.get(), ref_off.get(), nt, ref_box.get(), ref_tri.get());
+    k_morton<<<nblocks, 256, 0, st>>>(ref_box.get(), bounds.get(), n, keys.get(), vals.get());
     for (int pass = 0; pass < 16; pass++) {                              // 62-bit keys, 4-bit digits
-        k_radix_hist<<<nblocks, 256, 0, st>>>(keys, n, pass * 4, hist, nblocks);
-        k_radix_scan<<<1, 1024, 0, st>>>(hist, 16 * nblocks);
-        k_radix_scatter<<<nblocks, 256, 0, st>>>(keys, vals, n, pass * 4, hist, nblocks, keys2, vals2);
+        k_radix_hist<<<nblocks, 256, 0, st>>>(keys.get(), n, pass * 4, hist.get(), nblocks);
+        k_radix_scan<<<1, 1024, 0, st>>>(hist.get(), 16 * nblocks);
+        k_radix_scatter<<<nblocks, 256, 0, st>>>(keys.get(), vals.get(), n, pass * 4, hist.get(), nblocks, keys2.get(), vals2.get());
         std::swap(keys, keys2); std::swap(vals, vals2);
     }
-    k_reorder<<<nblocks, 256, 0, st>>>(tmp, ref_tri, ref_box, vals, n, tris, leaf_box, tri_slot);
+    k_reorder<<<nblocks, 256, 0, st>>>(tmp.get(), ref_tri.get(), ref_box.get(), vals.get(), n, tris, leaf_box.get(), tri_slot.get());
     if (n_int) {
-        k_karras<<<(n_int + 255) / 256, 256, 0, st>>>(keys, (int)n, left, right, parent_int, parent_leaf, range);
-        k_refit<<<nblocks, 256, 0, st>>>((int)n, left, right, parent_int, parent_leaf, leaf_box, node_box, flags);
-        k_emit<<<(n_int + 255) / 256, 256, 0, st>>>((int)n_int, left, right, range, leaf_box, node_box, bounds, nodes);
+        k_karras<<<(n_int + 255) / 256, 256, 0, st>>>(keys.get(), (int)n, left.get(), right.get(), parent_int.get(), parent_leaf.get(), range.get());
+        k_refit<<<nblocks, 256, 0, st>>>((int)n, left.get(), right.get(), parent_int.get(), parent_leaf.get(), leaf_box.get(), node_box.get(), flags.get());
+        k_emit<<<(n_int + 255) / 256, 256, 0, st>>>((int)n_int, left.get(), right.get(), range.get(), leaf_box.get(), node_box.get(), bounds.get(), nodes);
     }
     LBVH_CHECK(cudaStreamSynchronize(st));
     LBVH_CHECK(cudaGetLastError());
@@ -1222,9 +1220,9 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
     int max_depth = 1; int root_ref = n_int ? 0 : ~0;
     if (n_int) {
         std::vector<int> hl(n_int), hr(n_int); std::vector<int2> hrange(n_int);
-        LBVH_CHECK(cudaMemcpy(hl.data(), left, (size_t)n_int * 4, cudaMemcpyDeviceToHost));
-        LBVH_CHECK(cudaMemcpy(hr.data(), right, (size_t)n_int * 4, cudaMemcpyDeviceToHost));
-        LBVH_CHECK(cudaMemcpy(hrange.data(), range, (size_t)n_int * sizeof(int2), cudaMemcpyDeviceToHost));
+        LBVH_CHECK(cudaMemcpy(hl.data(), left.get(), (size_t)n_int * 4, cudaMemcpyDeviceToHost));
+        LBVH_CHECK(cudaMemcpy(hr.data(), right.get(), (size_t)n_int * 4, cudaMemcpyDeviceToHost));
+        LBVH_CHECK(cudaMemcpy(hrange.data(), range.get(), (size_t)n_int * sizeof(int2), cudaMemcpyDeviceToHost));
         auto is_leaf = [&](int c) { return c < 0 || hrange[c].y - hrange[c].x + 1 <= LBVH_LEAF_MAX; };
         if (is_leaf(0)) root_ref = ~((0 << 2) | (int)(n - 1));              // whole scene fits one leaf
         else {
@@ -1239,17 +1237,12 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
     }
     if (keep_ref_boxes && n_int) {                                          // opt-in SAH build (lbvh_refine_sah mode 2) works from these
         out->h_ref_box = static_cast<float *>(malloc((size_t)n * 6 * sizeof(float)));
-        if (out->h_ref_box) LBVH_CHECK(cudaMemcpy(out->h_ref_box, leaf_box, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
+        if (out->h_ref_box) LBVH_CHECK(cudaMemcpy(out->h_ref_box, leaf_box.get(), (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
     }
-    cudaFree(tmp); cudaFree(aabb); cudaFree(bounds); cudaFree(ksplit); cudaFree(ref_off);
-    if (dev_ref_box && n_int) *dev_ref_box = leaf_box;                      // the GPU builder (lbvh_ploc_rebuild) works from these, on the device
-    else cudaFree(leaf_box);
-    cudaFree(ref_box); cudaFree(ref_tri); cudaFree(node_box);
-    cudaFree(keys); cudaFree(vals); cudaFree(keys2); cudaFree(vals2); cudaFree(hist);
-    cudaFree(left); cudaFree(right); cudaFree(parent_int); cudaFree(parent_leaf); cudaFree(flags); cudaFree(range);
+    if (dev_ref_box && n_int) *dev_ref_box = std::move(leaf_box);           // the GPU builder (lbvh_ploc_rebuild) works from these, on the device
 
-    out->shade = shade; out->tri_slot = tri_slot;
-    out->nodes = nodes; out->tris = tris; out->n_nodes = n_nodes_alloc; out->n_tris = n;   // n_tris = BvhTri slots (references)
+    out->shade = shade.release(); out->tri_slot = tri_slot.release();
+    out->nodes = reinterpret_cast<BvhNode *>(blob.release()); out->tris = tris; out->n_nodes = n_nodes_alloc; out->n_tris = n;   // n_tris = BvhTri slots (references)
     out->root = root_ref;
     out->max_depth = max_depth;
     out->bytes = node_bytes + tri_bytes;

@@ -112,54 +112,42 @@ int ploc_build(const float *d_ref_box, uint32_t n, BvhNode *d_out, uint32_t *d_p
     *n_out = 0; *depth = 0;
     if (n <= (uint32_t)LBVH_LEAF_MAX || n >= (1u << 28)) return 0;
     const uint32_t n_all = 2 * n - 1, nb = (n + 255) / 256;
-    float *box = nullptr; PlocMeta *meta = nullptr; uint32_t *child = nullptr, *cl = nullptr, *nn = nullptr, *bcnt = nullptr; uint2 *place = nullptr;
-    int err = 0;
-    auto run = [&]() -> int {
-        PLOC_CHECK(cudaMalloc(&box, (size_t)n_all * 6 * sizeof(float)));
-        PLOC_CHECK(cudaMalloc(&meta, (size_t)n_all * sizeof(PlocMeta)));
-        PLOC_CHECK(cudaMalloc(&child, (size_t)(n - 1) * 2 * 4));
-        PLOC_CHECK(cudaMalloc(&cl, (size_t)n * 2 * 4));
-        PLOC_CHECK(cudaMalloc(&nn, (size_t)n * 4));
-        PLOC_CHECK(cudaMalloc(&bcnt, ((size_t)2 * nb + 1) * 4));
-        PLOC_CHECK(cudaMalloc(&place, (size_t)(n - 1) * sizeof(uint2)));
-        k_ploc_init<<<nb, 256, 0, st>>>(d_ref_box, n, box, meta, cl);
-        std::vector<uint32_t> step_m{ n };                                    // clusters at the start of each step
-        uint32_t *cur = cl, *nxt = cl + n, m = n;
-        while (m > 1) {
-            const uint32_t mb = (m + 255) / 256;
-            k_ploc_nearest<<<mb, 256, 0, st>>>(cur, m, box, nn);
-            k_ploc_count<<<mb, 256, 0, st>>>(nn, m, bcnt, mb);
-            k_scan_excl<<<1, 256, 0, st>>>(bcnt, 2 * mb, bcnt + 2 * mb);
-            k_ploc_merge<<<mb, 256, 0, st>>>(cur, nn, m, bcnt, mb, n + (n - m), n, box, meta, child, nxt);
-            PLOC_CHECK(cudaMemcpyAsync(h_small, bcnt + mb, 4, cudaMemcpyDeviceToHost, st));
-            PLOC_CHECK(cudaStreamSynchronize(st));
-            if (h_small[0] >= m) return (int)cudaErrorUnknown;                 // every step merges at least one pair (ploc_union_area)
-            m = h_small[0]; step_m.push_back(m);
-            std::swap(cur, nxt);
-        }
-        const uint32_t root = n_all - 1;
-        PLOC_CHECK(cudaMemcpyAsync(h_small, meta + root, sizeof(PlocMeta), cudaMemcpyDeviceToHost, st));
-        PLOC_CHECK(cudaMemsetAsync(place, 0xFF, (size_t)(n - 1) * sizeof(uint2), st));
-        const uint2 root_place = make_uint2(0u, 0u);
-        PLOC_CHECK(cudaMemcpyAsync(place + (root - n), &root_place, sizeof root_place, cudaMemcpyHostToDevice, st));
-        for (size_t s = step_m.size() - 1; s-- > 0;) {                       // step s created nodes [n + (n - m_s), n + (n - m_{s+1}))
-            const uint32_t first = n + (n - step_m[s]), count = step_m[s] - step_m[s + 1];
-            k_ploc_emit<<<(count + 255) / 256, 256, 0, st>>>(first, count, n, root, box, meta, child, place, d_out, d_perm);
-        }
-        PLOC_CHECK(cudaGetLastError());
+    DevPtr<float> box; DevPtr<PlocMeta> meta; DevPtr<uint32_t> child, cl, nn, bcnt; DevPtr<uint2> place;
+    PLOC_CHECK(alloc(box, (size_t)n_all * 6 * sizeof(float)));
+    PLOC_CHECK(alloc(meta, (size_t)n_all * sizeof(PlocMeta)));
+    PLOC_CHECK(alloc(child, (size_t)(n - 1) * 2 * 4));
+    PLOC_CHECK(alloc(cl, (size_t)n * 2 * 4));
+    PLOC_CHECK(alloc(nn, (size_t)n * 4));
+    PLOC_CHECK(alloc(bcnt, ((size_t)2 * nb + 1) * 4));
+    PLOC_CHECK(alloc(place, (size_t)(n - 1) * sizeof(uint2)));
+    k_ploc_init<<<nb, 256, 0, st>>>(d_ref_box, n, box.get(), meta.get(), cl.get());
+    std::vector<uint32_t> step_m{ n };                                        // clusters at the start of each step
+    uint32_t *cur = cl.get(), *nxt = cl.get() + n, m = n;
+    while (m > 1) {
+        const uint32_t mb = (m + 255) / 256;
+        k_ploc_nearest<<<mb, 256, 0, st>>>(cur, m, box.get(), nn.get());
+        k_ploc_count<<<mb, 256, 0, st>>>(nn.get(), m, bcnt.get(), mb);
+        k_scan_excl<<<1, 256, 0, st>>>(bcnt.get(), 2 * mb, bcnt.get() + 2 * mb);
+        k_ploc_merge<<<mb, 256, 0, st>>>(cur, nn.get(), m, bcnt.get(), mb, n + (n - m), n, box.get(), meta.get(), child.get(), nxt);
+        PLOC_CHECK(cudaMemcpyAsync(h_small, bcnt.get() + mb, 4, cudaMemcpyDeviceToHost, st));
         PLOC_CHECK(cudaStreamSynchronize(st));
-        *n_out = h_small[1]; *depth = (int)h_small[2];                        // PlocMeta {cnt, sub, dep, leaf} of the root
-        return 0;
-    };
-    err = run();
-    if (box) cudaFree(box);
-    if (meta) cudaFree(meta);
-    if (child) cudaFree(child);
-    if (cl) cudaFree(cl);
-    if (nn) cudaFree(nn);
-    if (bcnt) cudaFree(bcnt);
-    if (place) cudaFree(place);
-    return err;
+        if (h_small[0] >= m) return (int)cudaErrorUnknown;                     // every step merges at least one pair (ploc_union_area)
+        m = h_small[0]; step_m.push_back(m);
+        std::swap(cur, nxt);
+    }
+    const uint32_t root = n_all - 1;
+    PLOC_CHECK(cudaMemcpyAsync(h_small, meta.get() + root, sizeof(PlocMeta), cudaMemcpyDeviceToHost, st));
+    PLOC_CHECK(cudaMemsetAsync(place.get(), 0xFF, (size_t)(n - 1) * sizeof(uint2), st));
+    const uint2 root_place = make_uint2(0u, 0u);
+    PLOC_CHECK(cudaMemcpyAsync(place.get() + (root - n), &root_place, sizeof root_place, cudaMemcpyHostToDevice, st));
+    for (size_t s = step_m.size() - 1; s-- > 0;) {                           // step s created nodes [n + (n - m_s), n + (n - m_{s+1}))
+        const uint32_t first = n + (n - step_m[s]), count = step_m[s] - step_m[s + 1];
+        k_ploc_emit<<<(count + 255) / 256, 256, 0, st>>>(first, count, n, root, box.get(), meta.get(), child.get(), place.get(), d_out, d_perm);
+    }
+    PLOC_CHECK(cudaGetLastError());
+    PLOC_CHECK(cudaStreamSynchronize(st));
+    *n_out = h_small[1]; *depth = (int)h_small[2];                            // PlocMeta {cnt, sub, dep, leaf} of the root
+    return 0;
 }
 
 // ---- slot permutation -----------------------------------------------------------------------------------------------------------------
@@ -171,38 +159,30 @@ __global__ void k_permute_tris(const BvhTri *__restrict__ src, const uint32_t *_
     atomicMax(&tri_slot[__float_as_uint(t.a.w)], i);                       // the highest of a triangle's slots: deterministic
 }
 
-int lbvh_ploc_rebuild(LbvhResult *r, float *d_ref_box, uint32_t *h_small, cudaStream_t st) {
+int lbvh_ploc_rebuild(LbvhResult *r, DevPtr<float> ref_box, uint32_t *h_small, cudaStream_t st) {
     const uint32_t n = r->n_tris;
-    BvhNode *nodes = nullptr; uint32_t *perm = nullptr; BvhTri *tris = nullptr;
-    auto run = [&]() -> int {
-        if (!r->nodes || r->root < 0 || n <= (uint32_t)LBVH_LEAF_MAX || n - 1 > r->n_nodes) return 0;
-        PLOC_CHECK(cudaMalloc(&nodes, (size_t)(n - 1) * sizeof(BvhNode)));
-        PLOC_CHECK(cudaMalloc(&perm, (size_t)n * 4));
-        uint32_t n_out = 0; int depth = 0;
-        const int e = ploc_build(d_ref_box, n, nodes, perm, &n_out, &depth, h_small, st);
-        if (e != 0) return e;
-        // a tree of detail nested around a point can be far deeper than the LBVH: keep the shallower one rather than make every traversal
-        // kernel carry a deeper stack (lbvh_refine_sah's rule)
-        const bool depth_ok = depth + 2 <= BVH_STACK_MAX || depth <= r->max_depth;
-        if (getenv("B200PT_DEBUG"))
-            fprintf(stderr, "[b200pt] GPU PLOC build: %u nodes, depth %d (LBVH %d)%s\n", n_out, depth, r->max_depth, depth_ok ? "" : ": too deep, LBVH kept");
-        if (n_out == 0 || !depth_ok) return 0;
-        PLOC_CHECK(cudaMalloc(&tris, (size_t)n * sizeof(BvhTri)));
-        PLOC_CHECK(cudaMemcpyAsync(tris, r->tris, (size_t)n * sizeof(BvhTri), cudaMemcpyDeviceToDevice, st));
-        PLOC_CHECK(cudaMemsetAsync(r->tri_slot, 0, (size_t)r->n_prims * 4, st));
-        k_permute_tris<<<(n + 255) / 256, 256, 0, st>>>(tris, perm, n, r->tris, r->tri_slot);
-        PLOC_CHECK(cudaMemcpyAsync(r->nodes, nodes, (size_t)n_out * sizeof(BvhNode), cudaMemcpyDeviceToDevice, st));
-        PLOC_CHECK(cudaGetLastError());
-        PLOC_CHECK(cudaStreamSynchronize(st));
-        r->root = 0; r->max_depth = depth;
-        return 0;
-    };
-    const int err = run();
-    cudaFree(d_ref_box);
-    if (nodes) cudaFree(nodes);
-    if (perm) cudaFree(perm);
-    if (tris) cudaFree(tris);
-    return err;
+    if (!r->nodes || r->root < 0 || n <= (uint32_t)LBVH_LEAF_MAX || n - 1 > r->n_nodes) return 0;
+    DevPtr<BvhNode> nodes; DevPtr<uint32_t> perm; DevPtr<BvhTri> tris;
+    PLOC_CHECK(alloc(nodes, (size_t)(n - 1) * sizeof(BvhNode)));
+    PLOC_CHECK(alloc(perm, (size_t)n * 4));
+    uint32_t n_out = 0; int depth = 0;
+    const int e = ploc_build(ref_box.get(), n, nodes.get(), perm.get(), &n_out, &depth, h_small, st);
+    if (e != 0) return e;
+    // a tree of detail nested around a point can be far deeper than the LBVH: keep the shallower one rather than make every traversal
+    // kernel carry a deeper stack (lbvh_refine_sah's rule)
+    const bool depth_ok = depth + 2 <= BVH_STACK_MAX || depth <= r->max_depth;
+    if (getenv("B200PT_DEBUG"))
+        fprintf(stderr, "[b200pt] GPU PLOC build: %u nodes, depth %d (LBVH %d)%s\n", n_out, depth, r->max_depth, depth_ok ? "" : ": too deep, LBVH kept");
+    if (n_out == 0 || !depth_ok) return 0;
+    PLOC_CHECK(alloc(tris, (size_t)n * sizeof(BvhTri)));
+    PLOC_CHECK(cudaMemcpyAsync(tris.get(), r->tris, (size_t)n * sizeof(BvhTri), cudaMemcpyDeviceToDevice, st));
+    PLOC_CHECK(cudaMemsetAsync(r->tri_slot, 0, (size_t)r->n_prims * 4, st));
+    k_permute_tris<<<(n + 255) / 256, 256, 0, st>>>(tris.get(), perm.get(), n, r->tris, r->tri_slot);
+    PLOC_CHECK(cudaMemcpyAsync(r->nodes, nodes.get(), (size_t)n_out * sizeof(BvhNode), cudaMemcpyDeviceToDevice, st));
+    PLOC_CHECK(cudaGetLastError());
+    PLOC_CHECK(cudaStreamSynchronize(st));
+    r->root = 0; r->max_depth = depth;
+    return 0;
 }
 
 // ---- BVH2 -> BVH4, level by level ------------------------------------------------------------------------------------------------------
@@ -270,52 +250,40 @@ __global__ void __launch_bounds__(256) k_c4_emit(const BvhNode *__restrict__ nod
 int bvh4_collapse_device(const BvhNode *d_nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *d_out, uint32_t *n4, int *depth4, uint32_t *h_total, cudaStream_t st) {
     *n4 = 0; *depth4 = 0;
     if (root2 < 0 || n_nodes2 == 0) return 0;
-    int32_t *q2 = nullptr; uint32_t *bcnt = nullptr;
     const uint32_t nb_max = (n_nodes2 + 255) / 256;
-    auto run = [&]() -> int {
-        PLOC_CHECK(cudaMalloc(&q2, (size_t)n_nodes2 * 4));
-        PLOC_CHECK(cudaMalloc(&bcnt, ((size_t)nb_max + 1) * 4));
-        PLOC_CHECK(cudaMemcpyAsync(q2, &root2, 4, cudaMemcpyHostToDevice, st));
-        uint32_t b = 0, e = 1; int levels = 0;
-        while (b < e) {
-            const uint32_t nb = (e - b + 255) / 256;
-            k_c4_count<<<nb, 256, 0, st>>>(d_nodes2, q2, b, e, bcnt);
-            k_scan_excl<<<1, 256, 0, st>>>(bcnt, nb, bcnt + nb);
-            k_c4_emit<<<nb, 256, 0, st>>>(d_nodes2, q2, b, e, bcnt, d_out);
-            PLOC_CHECK(cudaMemcpyAsync(h_total, bcnt + nb, 4, cudaMemcpyDeviceToHost, st));
-            PLOC_CHECK(cudaStreamSynchronize(st));
-            levels++;
-            if ((uint64_t)e + h_total[0] > n_nodes2) return (int)cudaErrorInvalidValue;   // every BVH4 node consumes at least one BVH2 node
-            b = e; e += h_total[0];
-        }
-        PLOC_CHECK(cudaGetLastError());
-        *n4 = e; *depth4 = levels;
-        return 0;
-    };
-    const int err = run();
-    if (q2) cudaFree(q2);
-    if (bcnt) cudaFree(bcnt);
-    return err;
+    DevPtr<int32_t> q2; DevPtr<uint32_t> bcnt;
+    PLOC_CHECK(alloc(q2, (size_t)n_nodes2 * 4));
+    PLOC_CHECK(alloc(bcnt, ((size_t)nb_max + 1) * 4));
+    PLOC_CHECK(cudaMemcpyAsync(q2.get(), &root2, 4, cudaMemcpyHostToDevice, st));
+    uint32_t b = 0, e = 1; int levels = 0;
+    while (b < e) {
+        const uint32_t nb = (e - b + 255) / 256;
+        k_c4_count<<<nb, 256, 0, st>>>(d_nodes2, q2.get(), b, e, bcnt.get());
+        k_scan_excl<<<1, 256, 0, st>>>(bcnt.get(), nb, bcnt.get() + nb);
+        k_c4_emit<<<nb, 256, 0, st>>>(d_nodes2, q2.get(), b, e, bcnt.get(), d_out);
+        PLOC_CHECK(cudaMemcpyAsync(h_total, bcnt.get() + nb, 4, cudaMemcpyDeviceToHost, st));
+        PLOC_CHECK(cudaStreamSynchronize(st));
+        levels++;
+        if ((uint64_t)e + h_total[0] > n_nodes2) return (int)cudaErrorInvalidValue;   // every BVH4 node consumes at least one BVH2 node
+        b = e; e += h_total[0];
+    }
+    PLOC_CHECK(cudaGetLastError());
+    *n4 = e; *depth4 = levels;
+    return 0;
 }
 
 int lbvh_build_wide_device(LbvhResult *r, uint32_t *h_small, cudaStream_t st) {
     r->nodes4 = nullptr; r->n_nodes4 = 0; r->depth4 = 0;
     if (!r->nodes || r->root < 0 || r->n_nodes == 0) return 0;
-    Bvh4Node *scratch = nullptr, *out = nullptr;                           // collapsed into room for n_nodes, kept at the exact size
+    DevPtr<Bvh4Node> scratch, out;                                         // collapsed into room for n_nodes, kept at the exact size
     uint32_t n4 = 0; int d4 = 0;
-    auto run = [&]() -> int {
-        PLOC_CHECK(cudaMalloc(&scratch, (size_t)r->n_nodes * sizeof(Bvh4Node)));
-        const int e = bvh4_collapse_device(r->nodes, r->n_nodes, r->root, scratch, &n4, &d4, h_small, st);
-        if (e != 0 || n4 == 0) return e;
-        PLOC_CHECK(cudaMalloc(&out, (size_t)n4 * sizeof(Bvh4Node)));
-        PLOC_CHECK(cudaMemcpyAsync(out, scratch, (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyDeviceToDevice, st));
-        PLOC_CHECK(cudaStreamSynchronize(st));
-        return 0;
-    };
-    const int err = run();
-    if (scratch) cudaFree(scratch);
-    if (err != 0 || n4 == 0) { if (out) cudaFree(out); return err; }
-    r->nodes4 = out; r->n_nodes4 = n4; r->depth4 = d4;
+    PLOC_CHECK(alloc(scratch, (size_t)r->n_nodes * sizeof(Bvh4Node)));
+    const int e = bvh4_collapse_device(r->nodes, r->n_nodes, r->root, scratch.get(), &n4, &d4, h_small, st);
+    if (e != 0 || n4 == 0) return e;
+    PLOC_CHECK(alloc(out, (size_t)n4 * sizeof(Bvh4Node)));
+    PLOC_CHECK(cudaMemcpyAsync(out.get(), scratch.get(), (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyDeviceToDevice, st));
+    PLOC_CHECK(cudaStreamSynchronize(st));
+    r->nodes4 = out.release(); r->n_nodes4 = n4; r->depth4 = d4;
     return 0;
 }
 
