@@ -4,9 +4,12 @@
 // launches do nothing, and a device-to-host copy fills its destination with a chosen word (what the builders read back).  For every k:
 //   * Engine (b200pt_create): the k-th creation of a stream, event or block fails; nothing is live after the error, nor after
 //     b200pt_destroy of an engine whose creation succeeded;
-//   * lbvh_build, ploc_build, lbvh_ploc_rebuild, bvh4_collapse_device, lbvh_build_wide_device: the k-th cudaMalloc fails; a failing
-//     call leaves nothing live, a successful call exactly its outputs;
+//   * lbvh_build, ploc_build, lbvh_ploc_rebuild, bvh4_collapse_device, lbvh_build_wide, lbvh_build_wide_device: the k-th cudaMalloc
+//     fails; a failing call leaves nothing live, a successful call exactly its outputs;
+//   * the first lbvh_refit of a tree, with and without a BVH4: the k-th cudaMalloc of the refit state fails; a failing call leaves the
+//     tree and no refit state, the next call succeeds, and a successful call leaves exactly the tree and its refit state;
 //   * lbvh_build of a scene whose split counts add up to 2^28 references returns an error and leaves nothing live.
+// The trees handed to the functions under test are blocks of the shim too, so the LbvhResult that owns them releases them.
 // Built and run by tests/test_resource_ownership.py: nvcc --cudart shared ... tests/native/alloc_faults.cpp <every object of build/> -lz
 #include <cstdio>
 #include <cstdlib>
@@ -23,6 +26,8 @@ static std::set<void *> g_live;
 static uint32_t g_readback = 0;
 
 static void arm(long k, uint32_t readback) { g_fail_at = k; g_created = 0; g_readback = readback; }
+// Runs f with no creation failing and none counted: the inputs a case creates for the function under test.
+template <class F> static void unarmed(F f) { const long k = g_fail_at, c = g_created; g_fail_at = 0; f(); g_fail_at = k; g_created = c; }
 static cudaError_t create(void **p, size_t bytes) {
     *p = nullptr;
     if (++g_created == g_fail_at) return cudaErrorMemoryAllocation;
@@ -108,10 +113,9 @@ int main() {
     std::vector<b200pt_vertex> verts(3 * nt); std::vector<uint32_t> idx(3 * nt); DevMesh mesh{ 0, 0, nt, 0 }; DevInstance inst{};
     for (uint32_t i = 0; i < 3 * nt; i++) idx[i] = i;
     auto build = [&](uint32_t n_tris, std::vector<void *> *outs) {
-        LbvhResult res{}; DevPtr<float> ref_box;
-        const int r = lbvh_build(verts.data(), idx.data(), &mesh, &inst, &inst, &mesh, 1, n_tris, &res, nullptr, true, &ref_box);
-        if (r == 0) { *outs = { res.shade, res.tri_slot, res.nodes, ref_box.release() }; free(res.h_ref_box); }
-        else lbvh_free(&res);
+        LbvhResult res{}; std::vector<float> host_ref_box; DevPtr<float> ref_box;
+        const int r = lbvh_build(verts.data(), idx.data(), &mesh, &inst, 1, n_tris, &res, nullptr, &host_ref_box, &ref_box);
+        if (r == 0) *outs = { res.shade.release(), res.tri_slot.release(), res.nodes.release(), ref_box.release() };
         return r;
     };
     each_k("lbvh_build", 1u, true, [&](std::vector<void *> *o) { return build(nt, o); });
@@ -122,17 +126,23 @@ int main() {
     });
 
     // the device tree builder and collapse on host arrays: one clustering step (cluster count read back as 1), one BVH4 level (0)
-    std::vector<float> boxes((size_t)nt * 6, 0.0f); std::vector<BvhNode> nodes(nt - 1), nodes2(nt - 1); std::vector<uint32_t> perm(nt), slot(nt);
-    std::vector<BvhTri> tris(nt); std::vector<Bvh4Node> nodes4(nt - 1);
+    std::vector<float> boxes((size_t)nt * 6, 0.0f); std::vector<BvhNode> nodes(nt - 1), nodes2(nt - 1); std::vector<uint32_t> perm(nt);
+    std::vector<Bvh4Node> nodes4(nt - 1);
+    // a tree of n_nodes zeroed nodes followed by n_tris slots, created through the shim and owned by the result
+    auto tree = [](LbvhResult *res, uint32_t n_nodes, uint32_t n_tris) {
+        unarmed([&] {
+            alloc(res->nodes, (size_t)n_nodes * sizeof(BvhNode) + (size_t)n_tris * sizeof(BvhTri));
+            alloc(res->tri_slot, (size_t)n_tris * 4);
+        });
+        res->tris = reinterpret_cast<BvhTri *>(res->nodes.get() + n_nodes); res->n_nodes = n_nodes; res->n_tris = res->n_prims = n_tris;
+    };
     each_k("ploc_build", 1u, true, [&](std::vector<void *> *) {
         uint32_t n_out = 0; int depth = 0; uint32_t h_small[4];
         return ploc_build(boxes.data(), nt, nodes.data(), perm.data(), &n_out, &depth, h_small, nullptr);
     });
     each_k("lbvh_ploc_rebuild", 1u, true, [&](std::vector<void *> *) {
-        LbvhResult res{}; res.nodes = nodes.data(); res.tris = tris.data(); res.tri_slot = slot.data(); res.n_nodes = nt - 1; res.n_tris = res.n_prims = nt;
-        res.max_depth = 10;
-        const long k = g_fail_at; arm(0, 1u);                     // the reference boxes come from the caller, beside the count
-        DevPtr<float> ref_box; alloc(ref_box, (size_t)nt * 6 * sizeof(float)); arm(k, 1u);
+        LbvhResult res{}; tree(&res, nt - 1, nt); res.max_depth = 10;
+        DevPtr<float> ref_box; unarmed([&] { alloc(ref_box, (size_t)nt * 6 * sizeof(float)); });   // from the caller, beside the tree
         uint32_t h_small[4];
         return lbvh_ploc_rebuild(&res, std::move(ref_box), h_small, nullptr);
     });
@@ -141,12 +151,47 @@ int main() {
         return bvh4_collapse_device(nodes2.data(), nt - 1, 0, nodes4.data(), &n4, &d4, h_total, nullptr);
     });
     each_k("lbvh_build_wide_device", 0u, true, [&](std::vector<void *> *o) {
-        LbvhResult res{}; res.nodes = nodes2.data(); res.n_nodes = nt - 1;
+        LbvhResult res{}; tree(&res, nt - 1, 0);
         uint32_t h_small[4];
         const int r = lbvh_build_wide_device(&res, h_small, nullptr);
-        *o = { res.nodes4 };
+        *o = { res.nodes4.release() };
         return r;
     });
+    // the host collapse: both children of the root read back as one-slot leaves (0xFFFFFFFF), one BVH4 node
+    each_k("lbvh_build_wide", 0xFFFFFFFFu, true, [&](std::vector<void *> *o) {
+        LbvhResult res{}; tree(&res, 1, 0);
+        const int r = lbvh_build_wide(&res, nullptr);
+        if (r == 0 && res.n_nodes4 != 1) { printf("FAIL: lbvh_build_wide made %u nodes\n", res.n_nodes4); failures++; }
+        *o = { res.nodes4.release() };
+        return r;
+    });
+
+    // the first refit of a tree derives its refit state: one root over two one-slot leaves (read back as 0xFFFFFFFF), four slots of one
+    // triangle, and with `wide` a one-node BVH4
+    auto refit = [&](bool wide) {
+        LbvhResult res{}; tree(&res, 1, 4);
+        if (wide) { unarmed([&] { alloc(res.nodes4, sizeof(Bvh4Node)); }); res.n_nodes4 = 1; }
+        const long k = g_fail_at;
+        const std::set<void *> tree_blocks = g_live;
+        auto call = [&] { return lbvh_refit(&res, verts.data(), idx.data(), &mesh, &inst, 1, nullptr); };
+        const LbvhRefit &s = res.refit;
+        const int r = call();
+        if (r != 0) {
+            expect(g_live == tree_blocks && !s.ready && !s.slot_jk && !s.slot_box && !s.node_box && !s.bounds && !s.order && !s.src4 && s.level_off.empty(),
+                   "failed refit: the tree and no refit state", k);
+            int again = -1; unarmed([&] { again = call(); });
+            expect(again == 0 && s.ready, "refit after a failed prepare", k);
+        } else {
+            std::set<void *> want = tree_blocks;
+            for (void *p : std::initializer_list<void *>{ s.slot_jk.get(), s.slot_box.get(), s.node_box.get(), s.bounds.get(), s.order.get(), s.src4.get() })
+                if (p) want.insert(p);
+            expect(s.ready && s.slot_jk && s.slot_box && s.node_box && s.bounds && s.order && (s.src4 != nullptr) == wide && g_live == want,
+                   "refit: the tree and its refit state", k);
+        }
+        return r;                                                  // res releases the tree and its refit state
+    };
+    each_k("lbvh_refit", 0xFFFFFFFFu, true, [&](std::vector<void *> *) { return refit(false); });
+    each_k("lbvh_refit (BVH4)", 0xFFFFFFFFu, true, [&](std::vector<void *> *) { return refit(true); });
     if (failures) { printf("%d failures\n", failures); return 1; }
     puts("ok");
     return 0;

@@ -1,8 +1,9 @@
 // Host-only check of lbvh_refine_sah's plumbing (csrc/lbvh.cu): the CUDA copies are replaced by memcpy shims defined in THIS file
-// (the executable's own symbols win over libcudart's), so the function runs on host arrays without a GPU.  For every mode 1..5:
+// (the executable's own symbols win over libcudart's), and cudaFree by a no-op because the result's owners wrap host vectors, so the
+// function runs on host arrays without a GPU.  For every mode 1..5:
 //   * every ray finds the same closest triangle id and distance in the refined structure as by brute force over all triangles,
 //   * tri_slot[gid] points at a slot that holds triangle gid, root == 0, max_depth == the depth of the emitted tree.
-// Build and run by hand (or through tests/test_host_api.py::test_refine_plumbing_with_cuda_shims, which does exactly this):
+// Build and run by hand (or through tests/test_host_api.py::test_refine_sah_plumbing_with_caller_reference_boxes, which does exactly this):
 //   nvcc -std=c++17 -O1 -gencode arch=compute_90a,code=sm_90a -Ivulkan-path-tracer_b200/csrc -Iinclude tests/native/refine_plumbing.cpp vulkan-path-tracer_b200/build/lbvh.o -o /tmp/refine_plumbing
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +20,7 @@ extern "C" {
 cudaError_t cudaMemcpyAsync(void *dst, const void *src, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy(dst, src, n); return cudaSuccess; }
 cudaError_t cudaMemcpy(void *dst, const void *src, size_t n, cudaMemcpyKind) { memcpy(dst, src, n); return cudaSuccess; }
 cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
+cudaError_t cudaFree(void *) { return cudaSuccess; }
 }
 
 struct Hit { float t; uint32_t gid; };
@@ -123,10 +125,11 @@ int main() {
         }
         for (int mode = 0; mode <= 5; mode++) {
             LbvhResult res{}; std::vector<BvhNode> nodes = shuf; std::vector<BvhTri> tris = tris0; std::vector<uint32_t> slot = slot0; std::vector<float> rb = boxes0;
-            res.nodes = nodes.data(); res.tris = tris.data(); res.tri_slot = slot.data(); res.n_nodes = n - 1; res.n_tris = n; res.root = root0; res.max_depth = d0;
-            res.h_ref_box = (mode == 2 || mode == 3) ? rb.data() : nullptr; res.n_prims = n_prims;
+            res.nodes.reset(nodes.data()); res.tris = tris.data(); res.tri_slot.reset(slot.data()); res.n_nodes = n - 1; res.n_tris = n; res.root = root0; res.max_depth = d0;
+            res.n_prims = n_prims;
+            const float *ref_box = (mode == 2 || mode == 3) ? rb.data() : nullptr;
             double sah[2] = { 0, 0 };
-            if (mode && lbvh_refine_sah(&res, nullptr, sah, mode) != 0) { printf("mode %d failed\n", mode); return 1; }
+            if (mode && lbvh_refine_sah(&res, ref_box, nullptr, sah, mode) != 0) { printf("mode %d failed\n", mode); return 1; }
             const bool kept = mode && res.root == root0 && sah[1] == sah[0];   // the pass found nothing cheaper and left the structure alone
             if (mode && !kept && (res.root != 0 || !(sah[1] < sah[0]))) { printf("scene %d mode %d: root %d cost %g -> %g\n", scene, mode, res.root, sah[0], sah[1]); return 1; }
             if (res.max_depth != depth_of(nodes, res.root)) { printf("scene %d mode %d: max_depth %d != %d\n", scene, mode, res.max_depth, depth_of(nodes, res.root)); return 1; }

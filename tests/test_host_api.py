@@ -480,9 +480,10 @@ def test_bvh2_sah_rebuild_is_independent_of_the_thread_count(monkeypatch):
     assert outs[1] == outs[0] and outs[2] == outs[0]
 
 
-def test_refine_plumbing_with_cuda_shims(tmp_path):
-    """lbvh_refine_sah (the device-touching half of the opt-in tree passes) run on host arrays: tests/native/refine_plumbing.cpp replaces the
-    three CUDA copy calls by memcpy shims, then checks for modes 0..5 that every ray finds the same closest triangle as brute force, that
+def test_refine_sah_plumbing_with_caller_reference_boxes(tmp_path):
+    """lbvh_refine_sah (the device-touching half of the opt-in tree passes) run on host arrays, with the reference boxes passed by the caller
+    (null outside modes 2 / 3): tests/native/refine_plumbing.cpp replaces the three CUDA copy calls by memcpy shims and cudaFree by a no-op
+    (the tree's owners wrap host vectors), then checks for modes 0..5 that every ray finds the same closest triangle as brute force, that
     tri_slot survives the slot permutation of modes 2 / 3, root / max_depth bookkeeping and that a costlier tree is never uploaded."""
     import shutil, subprocess
     obj = os.path.join(util.ROOT, "vulkan-path-tracer_b200", "build", "lbvh.o")

@@ -62,7 +62,6 @@ Engine::~Engine() {
     cudaSetDevice(device_);
     for (auto &st : aux_stream_) if (st) cudaStreamSynchronize(st.get());
     if (stream_) cudaStreamSynchronize(stream_);
-    lbvh_free(&bvh_); lbvh_refit_free(&refit_);
 }
 
 // Device scratch of the engine, grown on demand and kept: the per-frame updates allocate (and free, which synchronises the device) nothing.
@@ -88,7 +87,7 @@ void Engine::free_scene() {
     d_verts_.reset(); d_indices_.reset(); d_meshes_.reset(); d_instances_.reset(); d_materials_.reset(); d_textures_.reset(); d_emissive_.reset();
     d_em_tris_.reset(); d_em_tri_base_.reset(); d_tri_class_.reset();
     d_texdata_.clear();
-    lbvh_free(&bvh_); lbvh_refit_free(&refit_);
+    bvh_ = {};
     free_pose_data();
     has_scene_ = false;
 }
@@ -171,8 +170,8 @@ void Engine::fill_instances() {
     n_tris_ = tri_base;
 }
 
-// The acceleration structure of the instances in d_instances_, built into *out (which the caller owns, also on failure): the BVH fields of *ds
-// and the launch configuration *lc are set from it.  set_scene and update_instance_transforms(rebuild) both use it.
+// The acceleration structure of the instances in d_instances_, built into *out: the BVH fields of *ds and the launch configuration *lc are set
+// from it (moving *out keeps them valid).  set_scene and update_instance_transforms(rebuild) both use it.
 // gpu_builder: the tree is built on the device (PLOC over the LBVH's references, ploc.cu) instead of by the host tree-quality passes.
 void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_builder) {
     // acceleration structure: GPU LBVH over the flattened instances
@@ -182,9 +181,9 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_bu
     int sah_mode = 3;
     if (const char *e = getenv("B200PT_BVH_SAH")) sah_mode = (e[0] >= '0' && e[0] <= '5' && e[1] == 0) ? e[0] - '0' : 3;
     if (gpu_builder) sah_mode = 0;
-    DevPtr<float> ref_box;
-    int r = lbvh_build(d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), (uint32_t)h_instances_.size(), n_tris_, out, stream_,
-                       sah_mode == 2 || sah_mode == 3, gpu_builder ? &ref_box : nullptr);
+    std::vector<float> host_ref_box; DevPtr<float> ref_box;                 // inputs of the tree passes below, released when the build ends
+    int r = lbvh_build(d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), n_tris_, out, stream_,
+                       sah_mode == 2 || sah_mode == 3 ? &host_ref_box : nullptr, gpu_builder ? &ref_box : nullptr);
     if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build failed: ") + cudaGetErrorString((cudaError_t)r) };
     if (gpu_builder) {
         r = lbvh_ploc_rebuild(out, std::move(ref_box), h_small_.get(), stream_);
@@ -192,17 +191,17 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_bu
     }
     if (sah_mode) {
         double sah[2];
-        r = lbvh_refine_sah(out, stream_, sah, sah_mode);
+        r = lbvh_refine_sah(out, host_ref_box.empty() ? nullptr : host_ref_box.data(), stream_, sah, sah_mode);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refine_sah failed: ") + cudaGetErrorString((cudaError_t)r) };
         if (getenv("B200PT_DEBUG")) fprintf(stderr, "[b200pt] SAH pass (mode %d): cost %.3f -> %.3f, depth %d\n", sah_mode, sah[0], sah[1], out->max_depth);
     }
-    ds->nodes = out->nodes; ds->tris = out->tris; ds->shade_tris = out->shade; ds->tri_slot = out->tri_slot;
+    ds->nodes = out->nodes.get(); ds->tris = out->tris; ds->shade_tris = out->shade.get(); ds->tri_slot = out->tri_slot.get();
     ds->n_tris = out->n_tris; ds->n_nodes = out->n_nodes; ds->root = out->root; ds->bvh_bytes = out->bytes <= 0xFFFFFFFFull ? (uint32_t)out->bytes : 0;
     ds->nodes4 = nullptr; ds->n_nodes4 = 0;
     if (out->bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
         r = gpu_builder ? lbvh_build_wide_device(out, h_small_.get(), stream_) : lbvh_build_wide(out, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build_wide failed: ") + cudaGetErrorString((cudaError_t)r) };
-        ds->nodes4 = out->nodes4; ds->n_nodes4 = out->n_nodes4;
+        ds->nodes4 = out->nodes4.get(); ds->n_nodes4 = out->n_nodes4;
     }
     // A handful of triangle slots (the 12-triangle Cornell box): shared-memory traversals test them in order, no hierarchy (bvh_traverse.cuh).
     {
@@ -320,7 +319,7 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         for (size_t a = 0; a < h_instances_.size(); a++) if (listed[h_instances_[a].mesh]) changed.push_back((uint32_t)a);
         uint32_t *const d_list = src.empty() ? nullptr : static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
         auto refit = [&]() {
-            int r = lbvh_refit(&bvh_, &refit_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), stream_);
+            int r = lbvh_refit(&bvh_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), stream_);
             if (r == 0 && !src.empty())
                 r = lbvh_refresh_shade(&bvh_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), changed.data(),
                                        (uint32_t)changed.size(), d_list, stream_);
@@ -334,9 +333,8 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
     } else {
         LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
         try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
-        catch (...) { lbvh_free(&fresh); try { restore(); } catch (...) { has_scene_ = false; } throw; }
-        lbvh_free(&bvh_); lbvh_refit_free(&refit_);
-        bvh_ = fresh; ds_ = ds; lc_ = lc;
+        catch (...) { try { restore(); } catch (...) { has_scene_ = false; } throw; }
+        bvh_ = std::move(fresh); ds_ = ds; lc_ = lc;
     }
     reset();
 }

@@ -162,7 +162,6 @@ private:
     DevPtr<DevGrid> d_grids_; int density_data_counter_ = 0;   // PathTracer.cpp:1508-1513: slots are handed out round-robin
     b200pt_atmosphere atmosphere_{};
     LbvhResult bvh_{};
-    LbvhRefit refit_{};                             // refit state of bvh_'s tree (from the first update on)
     PinnedPtr<uint32_t> h_small_;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
     DevPtr<uint8_t> d_scratch_; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices and pose
     void *scratch(size_t bytes);

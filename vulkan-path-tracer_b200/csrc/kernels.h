@@ -130,15 +130,21 @@ struct MissQuery {                            // device arrays of n misses; out:
 int launch_miss_query(const DevScene &sc, const DevConfig &cfg, const MissQuery &q, cudaStream_t st);     // cudaError_t as int
 
 // ---- LBVH build (lbvh.cu): world-space flattening of the two-level TLAS/BLAS ----
-struct LbvhResult { ShadeTri *shade; uint32_t *tri_slot; BvhNode *nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;
-                    Bvh4Node *nodes4; uint32_t n_nodes4; int depth4;
-                    float *h_ref_box; uint32_t n_prims; };                  // host copy of the per-slot reference boxes (only when asked for), triangle count
-// Builds into ONE contiguous allocation [nodes | tris] (so small scenes can be staged to smem with one bulk copy).
-// Returns cudaError_t as int.
+// What lbvh_refit needs of a tree (per-slot slab assignment, BVH2 levels, BVH4 source map), derived at the first refit of that tree.
+struct LbvhRefit { DevPtr<uint32_t> slot_jk; DevPtr<float> slot_box, node_box, bounds; DevPtr<int32_t> order, src4;
+                   std::vector<uint32_t> level_off; uint32_t n4 = 0; bool ready = false; };
+// One acceleration structure with its device blocks and its refit state: replacing or clearing a tree releases both.  nodes owns the one
+// [nodes | tris] block; tris points into it, so it stays valid when the result is moved.  Move-only.
+struct LbvhResult { DevPtr<ShadeTri> shade; DevPtr<uint32_t> tri_slot; DevPtr<BvhNode> nodes; BvhTri *tris; uint32_t n_nodes, n_tris; int32_t root; int max_depth; size_t bytes;
+                    DevPtr<Bvh4Node> nodes4; uint32_t n_nodes4; int depth4;
+                    uint32_t n_prims;                                        // triangle count
+                    LbvhRefit refit; };
+// Builds into ONE contiguous allocation [nodes | tris] (so small scenes can be staged to smem with one bulk copy).  The Morton-ordered
+// per-slot reference boxes (n_tris x 6 floats) are handed out when asked for: host_ref_box receives a host copy (lbvh_refine_sah modes 2, 3),
+// dev_ref_box the device array (lbvh_ploc_rebuild).  Returns cudaError_t as int.
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
-               const DevInstance *h_instances, const DevMesh *h_meshes, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes = false,
-               DevPtr<float> *dev_ref_box = nullptr);   // dev_ref_box: receives the Morton-ordered per-slot reference boxes (device, n_tris x 6)
-void lbvh_free(LbvhResult *r);
+               uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, std::vector<float> *host_ref_box = nullptr,
+               DevPtr<float> *dev_ref_box = nullptr);
 // BVH2 -> BVH4 on the host (pure CPU code, unit-tested without a GPU through b200pt_bvh4_collapse).  `out` must hold n_nodes2 entries.
 // Returns the number of BVH4 nodes written (0 if the root is a leaf), *depth4 = depth of the BVH4 (root = 1).
 uint32_t bvh4_collapse_host(const BvhNode *nodes2, uint32_t n_nodes2, int32_t root2, Bvh4Node *out, int *depth4);
@@ -166,22 +172,20 @@ int bvh4_collapse_device(const BvhNode *d_nodes2, uint32_t n_nodes2, int32_t roo
 int lbvh_ploc_rebuild(LbvhResult *r, DevPtr<float> ref_box, uint32_t *h_small, cudaStream_t st);
 // lbvh_build_wide with the collapse on the device (scratch of n_nodes BVH4 nodes; r->nodes4 is allocated at the exact size).
 int lbvh_build_wide_device(LbvhResult *r, uint32_t *h_small, cudaStream_t st);
-// mode 1: inner nodes only (download, rebuild, upload in place); mode 2: full build from r->h_ref_box, reference slots and tri_slot permuted
-// (falls back to mode 1 when the boxes were not kept); mode 3: mode 2 + insertion-based refinement; 4: mode 1 + refinement; 5: refinement only.  Returns cudaError_t as int.
+// mode 1: inner nodes only (download, rebuild, upload in place); mode 2: full build from ref_box (the host reference boxes of lbvh_build),
+// reference slots and tri_slot permuted (falls back to mode 1 when ref_box is null); mode 3: mode 2 + insertion-based refinement; 4: mode 1 +
+// refinement; 5: refinement only.  Returns cudaError_t as int.
 // A pass result deeper than BVH_STACK_MAX - 2 is dropped unless the input tree is deeper still (query_launch_cfg sizes the stacks from the depth).
 constexpr int BVH_STACK_MAX = 64;
-int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode = 1);
+int lbvh_refine_sah(LbvhResult *r, const float *ref_box, cudaStream_t st, double sah[2], int mode = 1);
 // Downloads r->nodes, collapses, uploads r->nodes4 (own allocation).  Returns cudaError_t as int; leaves nodes4 = nullptr if the root is a leaf.
 int lbvh_build_wide(LbvhResult *r, cudaStream_t st);
 // Refit in place after the instance transforms changed (d_instances holds the new o2w): the topology, slot order and tri_slot of r stay,
 // every slot record and box, every reachable BVH2 child box (padded from the new scene bounds) and every BVH4 child box are recomputed.
-// The state (per-slot slab assignment, BVH2 levels, BVH4 source map) is derived at the first call and kept in s; it belongs to r's tree
-// and is freed (lbvh_refit_free) whenever that tree is replaced.  Returns cudaError_t as int.
-struct LbvhRefit { uint32_t *slot_jk = nullptr; float *slot_box = nullptr, *node_box = nullptr, *bounds = nullptr; int32_t *order = nullptr, *src4 = nullptr;
-                   std::vector<uint32_t> level_off; uint32_t n4 = 0; bool ready = false; };
-int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+// The refit state is derived at the first call and kept in r->refit; a failure to derive it leaves r->refit empty, and the next call
+// tries again.  Returns cudaError_t as int.
+int lbvh_refit(LbvhResult *r, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
                uint32_t n_instances, cudaStream_t st);
-void lbvh_refit_free(LbvhRefit *s);
 // After the vertices of some meshes changed (d_verts holds them) and lbvh_refit ran: r->shade of every triangle of instances insts[0, m) is
 // rewritten as lbvh_build writes it.  Both rebuilds recompute r->shade themselves.  d_list: device scratch of at least 2 m + 1 words.
 // Returns cudaError_t as int.

@@ -918,14 +918,14 @@ int lbvh_build_wide(LbvhResult *r, cudaStream_t st) {
     r->nodes4 = nullptr; r->n_nodes4 = 0; r->depth4 = 0;
     if (!r->nodes || r->root < 0 || r->n_nodes == 0) return 0;
     std::vector<BvhNode> h2(r->n_nodes);
-    LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes, (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
+    LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes.get(), (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     std::vector<Bvh4Node> h4(r->n_nodes);
     int d4 = 0;
     const uint32_t n4 = bvh4_collapse_host(h2.data(), r->n_nodes, r->root, h4.data(), &d4);
     if (n4 == 0) return 0;
-    LBVH_CHECK(cudaMalloc(&r->nodes4, (size_t)n4 * sizeof(Bvh4Node)));
-    LBVH_CHECK(cudaMemcpyAsync(r->nodes4, h4.data(), (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyHostToDevice, st));
+    LBVH_CHECK(alloc(r->nodes4, (size_t)n4 * sizeof(Bvh4Node)));
+    LBVH_CHECK(cudaMemcpyAsync(r->nodes4.get(), h4.data(), (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyHostToDevice, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     r->n_nodes4 = n4; r->depth4 = d4;
     return 0;
@@ -933,15 +933,15 @@ int lbvh_build_wide(LbvhResult *r, cudaStream_t st) {
 
 // Opt-in (B200PT_BVH_SAH=1..5; 3 = 2 followed by bvh2_reinsert_host, 3 passes over the largest quarter of the nodes; 4 = 1 followed by the
 // same; 5 = re-insertion alone on the Morton-order tree -- 1, 4 and 5 leave the triangle slots where they are).  Mode 1 rebuilds the inner nodes in place with bvh2_sah_rebuild_host: the live node count is unchanged
-// (leaves - 1), so the rebuilt array fits the existing allocation.  Mode 2 builds from the kept per-slot reference boxes with
+// (leaves - 1), so the rebuilt array fits the existing allocation.  Mode 2 builds from the per-slot reference boxes ref_box with
 // bvh2_sah_build_host (at most slots - 1 nodes: fits as well), then permutes the 48-B triangle slots to the new leaf order and re-derives
 // tri_slot (global triangle id -> one of its slots) from the ids stored in the slots.  Root becomes 0, max_depth the new depth.
 // A no-op for one-leaf scenes.
-int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
+int lbvh_refine_sah(LbvhResult *r, const float *ref_box, cudaStream_t st, double sah[2], int mode) {
     if (sah) sah[0] = sah[1] = 0.0;
     if (!r->nodes || r->root < 0 || r->n_nodes == 0) return 0;
     std::vector<BvhNode> h2(r->n_nodes), out(r->n_nodes);
-    LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes, (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
+    LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes.get(), (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     int depth = 0;
     // two sweeps over the largest tenth of the nodes: SAH cost 37.1 -> 34.10 in 0.17 s on BreakfastRoom (8 host threads) against 33.95 in 0.65 s for three sweeps over a quarter
@@ -956,11 +956,11 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
     // shallower input rather than make every traversal kernel carry a deeper stack
     auto depth_ok = [&](int d) { return d + 2 <= BVH_STACK_MAX || d <= r->max_depth; };
     const bool full = mode == 2 || mode == 3, refine = mode >= 3;
-    if (full && r->h_ref_box && r->n_tris > (uint32_t)LBVH_LEAF_MAX && r->n_tris - 1 <= r->n_nodes) {
+    if (full && ref_box && r->n_tris > (uint32_t)LBVH_LEAF_MAX && r->n_tris - 1 <= r->n_nodes) {
         std::vector<uint32_t> perm(r->n_tris);
         double c_new = 0.0, c_old[2] = { 0.0, 0.0 };
         { std::vector<BvhNode> scratch(r->n_nodes); int d; bvh2_sah_rebuild_host(h2.data(), r->n_nodes, r->root, scratch.data(), &d, c_old); }   // cost of the LBVH, for the log
-        const uint32_t n = bvh2_sah_build_host(r->h_ref_box, r->n_tris, 1.0f, out.data(), perm.data(), &depth, &c_new);
+        const uint32_t n = bvh2_sah_build_host(ref_box, r->n_tris, 1.0f, out.data(), perm.data(), &depth, &c_new);
         if (n != 0 && refine) reinsert(n, &c_new);
         if (n != 0 && c_new < c_old[0] && depth_ok(depth)) {                    // never trade the tree for a costlier one
             std::vector<BvhTri> t_old(r->n_tris), t_new(r->n_tris);
@@ -973,8 +973,8 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
                 if (gid < r->n_prims) slot[gid] = i;
             }
             LBVH_CHECK(cudaMemcpyAsync(r->tris, t_new.data(), (size_t)r->n_tris * sizeof(BvhTri), cudaMemcpyHostToDevice, st));
-            LBVH_CHECK(cudaMemcpyAsync(r->tri_slot, slot.data(), (size_t)r->n_prims * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-            LBVH_CHECK(cudaMemcpyAsync(r->nodes, out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
+            LBVH_CHECK(cudaMemcpyAsync(r->tri_slot.get(), slot.data(), (size_t)r->n_prims * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+            LBVH_CHECK(cudaMemcpyAsync(r->nodes.get(), out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
             LBVH_CHECK(cudaStreamSynchronize(st));
             r->root = 0; r->max_depth = depth;
             if (sah) { sah[0] = c_old[0]; sah[1] = c_new; }
@@ -990,20 +990,10 @@ int lbvh_refine_sah(LbvhResult *r, cudaStream_t st, double sah[2], int mode) {
     if (n == 0) return 0;
     if (sah) { sah[0] = cst[0]; sah[1] = cst[1] < cst[0] ? cst[1] : cst[0]; }
     if (!(cst[1] < cst[0]) || !depth_ok(depth)) return 0;                      // never trade the tree for a costlier one
-    LBVH_CHECK(cudaMemcpyAsync(r->nodes, out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
+    LBVH_CHECK(cudaMemcpyAsync(r->nodes.get(), out.data(), (size_t)n * sizeof(BvhNode), cudaMemcpyHostToDevice, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     r->root = 0; r->max_depth = depth;
     return 0;
-}
-
-void lbvh_refit_free(LbvhRefit *s) {
-    if (s->slot_jk) cudaFree(s->slot_jk);
-    if (s->slot_box) cudaFree(s->slot_box);
-    if (s->node_box) cudaFree(s->node_box);
-    if (s->bounds) cudaFree(s->bounds);
-    if (s->order) cudaFree(s->order);
-    if (s->src4) cudaFree(s->src4);
-    *s = LbvhRefit{};
 }
 
 // What the refit needs of the tree, derived once at the first update (set_scene pays nothing for it): the slots' (j, k), the reachable BVH2
@@ -1016,7 +1006,7 @@ static int lbvh_refit_prepare(const LbvhResult *r, LbvhRefit *s, cudaStream_t st
     std::vector<BvhTri> ht(n);
     LBVH_CHECK(cudaMemcpyAsync(ht.data(), r->tris, (size_t)n * sizeof(BvhTri), cudaMemcpyDeviceToHost, st));
     std::vector<BvhNode> h2(r->root >= 0 ? r->n_nodes : 0);
-    if (!h2.empty()) LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes, (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
+    if (!h2.empty()) LBVH_CHECK(cudaMemcpyAsync(h2.data(), r->nodes.get(), (size_t)r->n_nodes * sizeof(BvhNode), cudaMemcpyDeviceToHost, st));
     LBVH_CHECK(cudaStreamSynchronize(st));
     std::vector<uint32_t> gid(n), jk(n);
     for (uint32_t i = 0; i < n; i++) { memcpy(&gid[i], &ht[i].a.w, 4); if (gid[i] >= np) gid[i] = 0u; }
@@ -1064,21 +1054,21 @@ static int lbvh_refit_prepare(const LbvhResult *r, LbvhRefit *s, cudaStream_t st
             for (uint32_t j = 0; j < k; j++) jk[b[j]] = (j << 16) | k;
         }
     }
-    LBVH_CHECK(cudaMalloc(&s->slot_jk, (size_t)n * 4));
-    LBVH_CHECK(cudaMalloc(&s->slot_box, (size_t)n * 6 * sizeof(float)));
-    LBVH_CHECK(cudaMalloc(&s->bounds, 6 * sizeof(float)));
-    LBVH_CHECK(cudaMemcpyAsync(s->slot_jk, jk.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    LBVH_CHECK(alloc(s->slot_jk, (size_t)n * 4));
+    LBVH_CHECK(alloc(s->slot_box, (size_t)n * 6 * sizeof(float)));
+    LBVH_CHECK(alloc(s->bounds, 6 * sizeof(float)));
+    LBVH_CHECK(cudaMemcpyAsync(s->slot_jk.get(), jk.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     if (!h2.empty()) {
-        LBVH_CHECK(cudaMalloc(&s->order, order.size() * 4));
-        LBVH_CHECK(cudaMalloc(&s->node_box, (size_t)r->n_nodes * 6 * sizeof(float)));
-        LBVH_CHECK(cudaMemcpyAsync(s->order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
+        LBVH_CHECK(alloc(s->order, order.size() * 4));
+        LBVH_CHECK(alloc(s->node_box, (size_t)r->n_nodes * 6 * sizeof(float)));
+        LBVH_CHECK(cudaMemcpyAsync(s->order.get(), order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
         if (r->nodes4) {                                                     // the collapse is deterministic: re-run on the unchanged BVH2 it was built from
             std::vector<Bvh4Node> h4(r->n_nodes); std::vector<int32_t> src((size_t)r->n_nodes * 4);
             int d4 = 0;
             const uint32_t n4 = bvh4_collapse_src(h2.data(), r->n_nodes, r->root, h4.data(), &d4, src.data());
             if (n4 != r->n_nodes4) return (int)cudaErrorInvalidValue;
-            LBVH_CHECK(cudaMalloc(&s->src4, (size_t)n4 * 4 * 4));
-            LBVH_CHECK(cudaMemcpyAsync(s->src4, src.data(), (size_t)n4 * 4 * 4, cudaMemcpyHostToDevice, st));
+            LBVH_CHECK(alloc(s->src4, (size_t)n4 * 4 * 4));
+            LBVH_CHECK(cudaMemcpyAsync(s->src4.get(), src.data(), (size_t)n4 * 4 * 4, cudaMemcpyHostToDevice, st));
             s->n4 = n4;
         }
     }
@@ -1087,22 +1077,23 @@ static int lbvh_refit_prepare(const LbvhResult *r, LbvhRefit *s, cudaStream_t st
     return 0;
 }
 
-int lbvh_refit(LbvhResult *r, LbvhRefit *s, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
+int lbvh_refit(LbvhResult *r, const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
                uint32_t n_instances, cudaStream_t st) {
     if (!r->tris || r->n_tris == 0 || n_instances == 0) return (int)cudaErrorInvalidValue;
+    LbvhRefit *s = &r->refit;
     if (!s->ready) {
         const int e = lbvh_refit_prepare(r, s, st);
-        if (e != 0) { lbvh_refit_free(s); return e; }
+        if (e != 0) { r->refit = LbvhRefit{}; return e; }
     }
     const uint32_t n = r->n_tris;
     const float binit[6] = { 3.0e38f, 3.0e38f, 3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f };
-    LBVH_CHECK(cudaMemcpyAsync(s->bounds, binit, sizeof(binit), cudaMemcpyHostToDevice, st));
-    k_refit_slots<<<(n + 255) / 256, 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, n_instances, s->slot_jk, n, r->tris, s->slot_box, s->bounds);
+    LBVH_CHECK(cudaMemcpyAsync(s->bounds.get(), binit, sizeof(binit), cudaMemcpyHostToDevice, st));
+    k_refit_slots<<<(n + 255) / 256, 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, n_instances, s->slot_jk.get(), n, r->tris, s->slot_box.get(), s->bounds.get());
     for (size_t l = s->level_off.size(); l-- > 1;) {                         // deepest level first
         const uint32_t first = s->level_off[l - 1], count = s->level_off[l] - first;
-        k_refit_level<<<(count + 255) / 256, 256, 0, st>>>(s->order, first, count, s->slot_box, s->bounds, r->nodes, s->node_box);
+        k_refit_level<<<(count + 255) / 256, 256, 0, st>>>(s->order.get(), first, count, s->slot_box.get(), s->bounds.get(), r->nodes.get(), s->node_box.get());
     }
-    if (s->n4) k_refit_wide<<<(s->n4 * 4 + 255) / 256, 256, 0, st>>>(s->src4, s->n4, r->nodes, r->nodes4);
+    if (s->n4) k_refit_wide<<<(s->n4 * 4 + 255) / 256, 256, 0, st>>>(s->src4.get(), s->n4, r->nodes.get(), r->nodes4.get());
     LBVH_CHECK(cudaGetLastError());
     LBVH_CHECK(cudaStreamSynchronize(st));
     return 0;
@@ -1118,7 +1109,7 @@ int lbvh_refresh_shade(LbvhResult *r, const b200pt_vertex *d_verts, const uint32
     for (uint32_t i = 0; i < m; i++) { total += h_meshes[h_instances[insts[i]].mesh].tri_count; if (total > 0xFFFFFFFFull) return (int)cudaErrorInvalidValue; list.push_back((uint32_t)total); }
     if (total == 0) return 0;
     LBVH_CHECK(cudaMemcpyAsync(d_list, list.data(), list.size() * 4, cudaMemcpyHostToDevice, st));
-    k_refresh_shade<<<(uint32_t)((total + 255) / 256), 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, d_list, m, r->shade);
+    k_refresh_shade<<<(uint32_t)((total + 255) / 256), 256, 0, st>>>(d_verts, d_indices, d_meshes, d_instances, d_list, m, r->shade.get());
     LBVH_CHECK(cudaGetLastError());
     LBVH_CHECK(cudaStreamSynchronize(st));
     return 0;
@@ -1134,25 +1125,11 @@ int any_nonfinite(const float *d_v, size_t n, uint32_t *d_flag, uint32_t *h_smal
     return 0;
 }
 
-void lbvh_free(LbvhResult *r) {
-    if (r->nodes4) cudaFree(r->nodes4);
-    r->nodes4 = nullptr; r->n_nodes4 = 0; r->depth4 = 0;
-    if (r->nodes) cudaFree(r->nodes);
-    if (r->shade) cudaFree(r->shade);
-    if (r->tri_slot) cudaFree(r->tri_slot);
-    r->shade = nullptr; r->tri_slot = nullptr;
-    if (r->h_ref_box) free(r->h_ref_box);
-    r->h_ref_box = nullptr; r->n_prims = 0;
-    r->nodes = nullptr; r->tris = nullptr; r->n_nodes = r->n_tris = 0; r->bytes = 0;
-}
-
 int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const DevMesh *d_meshes, const DevInstance *d_instances,
-               const DevInstance *, const DevMesh *, uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, bool keep_ref_boxes,
-               DevPtr<float> *dev_ref_box) {
+               uint32_t n_instances, uint32_t n_tris, LbvhResult *out, cudaStream_t st, std::vector<float> *host_ref_box, DevPtr<float> *dev_ref_box) {
+    if (host_ref_box) host_ref_box->clear();
     if (dev_ref_box) dev_ref_box->reset();
-    out->shade = nullptr; out->tri_slot = nullptr; out->h_ref_box = nullptr; out->n_prims = n_tris;
-    out->nodes = nullptr; out->tris = nullptr; out->n_nodes = 0; out->n_tris = n_tris; out->root = 0; out->max_depth = 1; out->bytes = 0;
-    out->nodes4 = nullptr; out->n_nodes4 = 0; out->depth4 = 0;
+    *out = LbvhResult{};
     if (n_tris == 0 || n_instances == 0) return (int)cudaErrorInvalidValue;
     const uint32_t nt = n_tris, ntblocks = (nt + 255) / 256;
 
@@ -1178,11 +1155,10 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
     // ---- per-reference stage
     const uint32_t n = (uint32_t)total, n_int = n > 1 ? n - 1 : 0, n_nodes_alloc = n_int ? n_int : 1;
     const size_t node_bytes = (size_t)n_nodes_alloc * sizeof(BvhNode), tri_bytes = (size_t)n * sizeof(BvhTri);
-    DevPtr<unsigned char> blob;
-    LBVH_CHECK(alloc(blob, node_bytes + tri_bytes));
-    LBVH_CHECK(cudaMemsetAsync(blob.get(), 0, node_bytes, st));
-    BvhNode *nodes = reinterpret_cast<BvhNode *>(blob.get());
-    BvhTri *tris = reinterpret_cast<BvhTri *>(blob.get() + node_bytes);
+    DevPtr<BvhNode> nodes;                                                  // [nodes | tris]
+    LBVH_CHECK(alloc(nodes, node_bytes + tri_bytes));
+    LBVH_CHECK(cudaMemsetAsync(nodes.get(), 0, node_bytes, st));
+    BvhTri *tris = reinterpret_cast<BvhTri *>(nodes.get() + n_nodes_alloc);
     DevPtr<float> ref_box, leaf_box, node_box; DevPtr<uint32_t> ref_tri, vals, vals2, hist; DevPtr<unsigned long long> keys, keys2;
     DevPtr<int> left, right, parent_int, parent_leaf; DevPtr<unsigned int> flags; DevPtr<int2> range;
     const uint32_t nblocks = (n + 255) / 256;
@@ -1211,7 +1187,7 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
     if (n_int) {
         k_karras<<<(n_int + 255) / 256, 256, 0, st>>>(keys.get(), (int)n, left.get(), right.get(), parent_int.get(), parent_leaf.get(), range.get());
         k_refit<<<nblocks, 256, 0, st>>>((int)n, left.get(), right.get(), parent_int.get(), parent_leaf.get(), leaf_box.get(), node_box.get(), flags.get());
-        k_emit<<<(n_int + 255) / 256, 256, 0, st>>>((int)n_int, left.get(), right.get(), range.get(), leaf_box.get(), node_box.get(), bounds.get(), nodes);
+        k_emit<<<(n_int + 255) / 256, 256, 0, st>>>((int)n_int, left.get(), right.get(), range.get(), leaf_box.get(), node_box.get(), bounds.get(), nodes.get());
     }
     LBVH_CHECK(cudaStreamSynchronize(st));
     LBVH_CHECK(cudaGetLastError());
@@ -1235,14 +1211,15 @@ int lbvh_build(const b200pt_vertex *d_verts, const uint32_t *d_indices, const De
             }
         }
     }
-    if (keep_ref_boxes && n_int) {                                          // opt-in SAH build (lbvh_refine_sah mode 2) works from these
-        out->h_ref_box = static_cast<float *>(malloc((size_t)n * 6 * sizeof(float)));
-        if (out->h_ref_box) LBVH_CHECK(cudaMemcpy(out->h_ref_box, leaf_box.get(), (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
+    if (host_ref_box && n_int) {                                            // the host SAH build (lbvh_refine_sah mode 2) works from these
+        host_ref_box->resize((size_t)n * 6);
+        LBVH_CHECK(cudaMemcpy(host_ref_box->data(), leaf_box.get(), (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost));
     }
     if (dev_ref_box && n_int) *dev_ref_box = std::move(leaf_box);           // the GPU builder (lbvh_ploc_rebuild) works from these, on the device
 
-    out->shade = shade.release(); out->tri_slot = tri_slot.release();
-    out->nodes = reinterpret_cast<BvhNode *>(blob.release()); out->tris = tris; out->n_nodes = n_nodes_alloc; out->n_tris = n;   // n_tris = BvhTri slots (references)
+    out->shade = std::move(shade); out->tri_slot = std::move(tri_slot);
+    out->nodes = std::move(nodes); out->tris = tris; out->n_nodes = n_nodes_alloc; out->n_tris = n;   // n_tris = BvhTri slots (references)
+    out->n_prims = nt;
     out->root = root_ref;
     out->max_depth = max_depth;
     out->bytes = node_bytes + tri_bytes;

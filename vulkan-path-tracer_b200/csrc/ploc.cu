@@ -176,9 +176,9 @@ int lbvh_ploc_rebuild(LbvhResult *r, DevPtr<float> ref_box, uint32_t *h_small, c
     if (n_out == 0 || !depth_ok) return 0;
     PLOC_CHECK(alloc(tris, (size_t)n * sizeof(BvhTri)));
     PLOC_CHECK(cudaMemcpyAsync(tris.get(), r->tris, (size_t)n * sizeof(BvhTri), cudaMemcpyDeviceToDevice, st));
-    PLOC_CHECK(cudaMemsetAsync(r->tri_slot, 0, (size_t)r->n_prims * 4, st));
-    k_permute_tris<<<(n + 255) / 256, 256, 0, st>>>(tris.get(), perm.get(), n, r->tris, r->tri_slot);
-    PLOC_CHECK(cudaMemcpyAsync(r->nodes, nodes.get(), (size_t)n_out * sizeof(BvhNode), cudaMemcpyDeviceToDevice, st));
+    PLOC_CHECK(cudaMemsetAsync(r->tri_slot.get(), 0, (size_t)r->n_prims * 4, st));
+    k_permute_tris<<<(n + 255) / 256, 256, 0, st>>>(tris.get(), perm.get(), n, r->tris, r->tri_slot.get());
+    PLOC_CHECK(cudaMemcpyAsync(r->nodes.get(), nodes.get(), (size_t)n_out * sizeof(BvhNode), cudaMemcpyDeviceToDevice, st));
     PLOC_CHECK(cudaGetLastError());
     PLOC_CHECK(cudaStreamSynchronize(st));
     r->root = 0; r->max_depth = depth;
@@ -278,12 +278,12 @@ int lbvh_build_wide_device(LbvhResult *r, uint32_t *h_small, cudaStream_t st) {
     DevPtr<Bvh4Node> scratch, out;                                         // collapsed into room for n_nodes, kept at the exact size
     uint32_t n4 = 0; int d4 = 0;
     PLOC_CHECK(alloc(scratch, (size_t)r->n_nodes * sizeof(Bvh4Node)));
-    const int e = bvh4_collapse_device(r->nodes, r->n_nodes, r->root, scratch.get(), &n4, &d4, h_small, st);
+    const int e = bvh4_collapse_device(r->nodes.get(), r->n_nodes, r->root, scratch.get(), &n4, &d4, h_small, st);
     if (e != 0 || n4 == 0) return e;
     PLOC_CHECK(alloc(out, (size_t)n4 * sizeof(Bvh4Node)));
     PLOC_CHECK(cudaMemcpyAsync(out.get(), scratch.get(), (size_t)n4 * sizeof(Bvh4Node), cudaMemcpyDeviceToDevice, st));
     PLOC_CHECK(cudaStreamSynchronize(st));
-    r->nodes4 = out.release(); r->n_nodes4 = n4; r->depth4 = d4;
+    r->nodes4 = std::move(out); r->n_nodes4 = n4; r->depth4 = d4;
     return 0;
 }
 
