@@ -8,21 +8,31 @@
 //     fails; a failing call leaves nothing live, a successful call exactly its outputs;
 //   * the first lbvh_refit of a tree, with and without a BVH4: the k-th cudaMalloc of the refit state fails; a failing call leaves the
 //     tree and no refit state, the next call succeeds, and a successful call leaves exactly the tree and its refit state;
-//   * lbvh_build of a scene whose split counts add up to 2^28 references returns an error and leaves nothing live.
-// The trees handed to the functions under test are blocks of the shim too, so the LbvhResult that owns them releases them.
+//   * lbvh_build of a scene whose split counts add up to 2^28 references returns an error and leaves nothing live;
+//   * Engine::set_env_map, set_luts and set_material (its emissive rebuild) on an engine with a scene, a map and tables: the k-th creation
+//     fails; every non-null pointer of the device view (Engine::dev_scene) lies in a live block and has_env / has_luts agree with it.  A
+//     failed set_env_map / set_luts leaves no map / no tables, and every launch that reads them refuses with B200PT_ERR_NO_SCENE; a failed
+//     emissive rebuild leaves the previous tables; a successful call leaves exactly its new blocks, and the view holds them.
+// The trees handed to the functions under test are blocks of the shim too, so the LbvhResult that owns them releases them.  query_launch_cfg's
+// device queries (set_scene) are shims as well.
 // Built and run by tests/test_resource_ownership.py: nvcc --cudart shared ... tests/native/alloc_faults.cpp <every object of build/> -lz
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <set>
 #include <vector>
 #include <cuda_runtime.h>
 #include "kernels.h"
+#include "engine.h"
 #include "b200pt.h"
 using namespace b200pt;
 
 static long g_fail_at = 0, g_created = 0;      // creations since the last arm(); the g_fail_at-th fails (0: none)
 static std::set<void *> g_live;
+struct Block { size_t bytes; long serial; };
+static std::map<const char *, Block> g_blocks;  // every live block, with its size and its creation's number
+static long g_serial = 0;
 static uint32_t g_readback = 0;
 
 static void arm(long k, uint32_t readback) { g_fail_at = k; g_created = 0; g_readback = readback; }
@@ -32,14 +42,23 @@ static cudaError_t create(void **p, size_t bytes) {
     *p = nullptr;
     if (++g_created == g_fail_at) return cudaErrorMemoryAllocation;
     *p = calloc(1, bytes ? bytes : 1);
-    g_live.insert(*p);
+    g_live.insert(*p); g_blocks[static_cast<const char *>(*p)] = { bytes ? bytes : 1, ++g_serial };
     return cudaSuccess;
 }
 static cudaError_t release(void *p) {
     if (!p) return cudaSuccess;
     if (!g_live.erase(p)) { printf("FAIL: release of a handle that is not live\n"); exit(1); }
+    g_blocks.erase(static_cast<const char *>(p));
     free(p);
     return cudaSuccess;
+}
+// p points into a live block
+static bool live(const void *p) {
+    const char *c = static_cast<const char *>(p);
+    auto it = g_blocks.upper_bound(c);
+    if (it == g_blocks.begin()) return false;
+    --it;
+    return c < it->first + it->second.bytes;
 }
 static cudaError_t copy(void *dst, const void *src, size_t n, cudaMemcpyKind kind) {
     if (kind == cudaMemcpyDeviceToHost) for (size_t i = 0; i + 4 <= n; i += 4) memcpy(static_cast<char *>(dst) + i, &g_readback, 4);
@@ -66,6 +85,12 @@ cudaError_t cudaMemsetAsync(void *p, int v, size_t n, cudaStream_t) { memset(p, 
 cudaError_t cudaMemcpy(void *d, const void *s, size_t n, cudaMemcpyKind k) { return copy(d, s, n, k); }
 cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind k, cudaStream_t) { return copy(d, s, n, k); }
 cudaError_t cudaLaunchKernel(const void *, dim3, dim3, void **, size_t, cudaStream_t) { return cudaSuccess; }
+// what query_launch_cfg asks of the device when set_scene builds a tree: one CTA of every kernel per SM on 132 SMs
+cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
+cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { memset(p, 0, sizeof *p); p->multiProcessorCount = 132; return cudaSuccess; }
+cudaError_t cudaFuncGetAttributes(cudaFuncAttributes *a, const void *) { memset(a, 0, sizeof *a); return cudaSuccess; }
+cudaError_t cudaFuncSetAttribute(const void *, cudaFuncAttribute, int) { return cudaSuccess; }
+cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 1; return cudaSuccess; }
 }
 
 static int failures = 0;
@@ -192,6 +217,97 @@ int main() {
     };
     each_k("lbvh_refit", 0xFFFFFFFFu, true, [&](std::vector<void *> *) { return refit(false); });
     each_k("lbvh_refit (BVH4)", 0xFFFFFFFFu, true, [&](std::vector<void *> *) { return refit(true); });
+
+    // The device view of an engine (Engine::dev_scene) across failed updates: a one-quad scene, an environment map and the lookup tables,
+    // then set_env_map, set_luts and set_material's emissive rebuild with their k-th allocation failing.  After every call each non-null
+    // pointer of the view lies in a live block and the readiness checks agree with the view.
+    {
+        const std::set<void *> before_engine = g_live;
+        setenv("B200PT_BVH_SAH", "0", 1);                          // the plain LBVH: the host tree passes need real boxes
+        {
+            Engine e(0);
+            auto view_ok = [&](const char *what, long k) {
+                const DevScene sc = e.dev_scene();
+                const void *ptrs[] = { sc.verts, sc.indices, sc.meshes, sc.instances, sc.materials, sc.textures, sc.emissive, sc.env, sc.alias, sc.env_row_cos,
+                                       sc.lut_reflect, sc.lut_refract_out, sc.lut_refract_in, sc.tri_slot, sc.tri_class, sc.nodes, sc.nodes4, sc.tris, sc.shade_tris,
+                                       sc.em_tris, sc.em_tri_base, sc.volumes, sc.grids };
+                bool ok = e.has_env() == (sc.env && sc.alias && sc.env_row_cos) && e.has_luts() == (sc.lut_reflect && sc.lut_refract_out && sc.lut_refract_in);
+                for (const void *p : ptrs) ok = ok && (!p || live(p));
+                expect(ok, what, k);
+            };
+            auto code = [](auto f) { try { f(); } catch (const CudaError &err) { return err.code; } return (int)B200PT_OK; };
+            // call() with its k-th creation failing, for k = 1, 2, ... until it succeeds; check(k, ok, prev, created): the view before the
+            // call and the blocks the call left behind
+            auto each_failure = [&](const char *name, auto call, auto check) {
+                const int failures0 = failures;
+                for (long k = 1;; k++) {
+                    const DevScene prev = e.dev_scene();
+                    const long serial0 = g_serial;
+                    arm(k, 0);
+                    const bool ok = code(call) == B200PT_OK;
+                    const bool injected = g_created >= k;
+                    arm(0, 0);
+                    std::set<const void *> created;
+                    for (const auto &b : g_blocks) if (b.second.serial > serial0) created.insert(b.first);
+                    expect(ok != injected, name, k);
+                    view_ok(name, k);
+                    check(k, ok, prev, created);
+                    if (!injected) { printf("%s: %ld creations, %d failed\n", name, k - 1, failures - failures0); return; }
+                }
+            };
+
+            HostScene s;                                           // one quad, one instance, one material that emits nothing
+            HostMesh quad;
+            quad.vertices.resize(4);
+            for (int v = 0; v < 4; v++) { quad.vertices[v].Position[0] = (float)(v & 1); quad.vertices[v].Position[1] = (float)(v >> 1); }
+            quad.indices = { 0, 1, 2, 2, 1, 3 };
+            s.meshes.push_back(quad);
+            b200pt_material m{}; m.BaseColor[0] = m.BaseColor[1] = m.BaseColor[2] = 0.5f;
+            m.BaseColorTextureIndex = m.NormalTextureIndex = m.RoughnessTextureIndex = m.MetallicTextureIndex = m.EmissiveTextureIndex = 0;
+            s.materials.push_back(m);
+            HostTexture white; white.width = white.height = 1; white.channels = 4; white.data = { 255, 255, 255, 255 };
+            s.textures.push_back(white);
+            b200pt_instance in{}; for (int i = 0; i < 4; i++) in.Transform[i * 5] = 1.0f;
+            s.instances.push_back(in);
+            for (int i = 0; i < 16; i++) s.camera_view[i] = (i % 5 == 0) ? 1.0f : 0.0f;
+            s.camera_aspect = 1.0f;
+            std::vector<float> rgba(4 * 2 * 4, 1.0f);
+            const size_t lut_n[3] = { 64 * 64 * 32, 128 * 128 * 32, 128 * 128 * 32 };
+            std::vector<float> lut[3] = { std::vector<float>(lut_n[0], 0.5f), std::vector<float>(lut_n[1], 0.5f), std::vector<float>(lut_n[2], 0.5f) };
+            arm(0, 1u);                                            // lbvh_build: every triangle one reference
+            int r = code([&] { e.set_scene(std::move(s)); e.set_env_map(2, 2, rgba.data()); e.set_luts(lut[0].data(), lut[1].data(), lut[2].data()); });
+            expect(r == B200PT_OK && e.has_scene() && e.has_env() && e.has_luts(), "engine set up", 0);
+            view_ok("engine set up", 0);
+            auto refuses = [&](long k, bool env) {                 // every launch that reads the map (env) or the tables refuses
+                float out[64] = {}; const float dir[3] = { 0.0f, 0.0f, 1.0f }, pdf = 1.0f; const uint32_t depth = 1, u0 = 0; uint32_t survivors = 0;
+                expect(code([&] { e.path_trace(1, 0); }) == B200PT_ERR_NO_SCENE && (!env || code([&] { e.miss_query(1, dir, &depth, &pdf, out); }) == B200PT_ERR_NO_SCENE) &&
+                       code([&] { e.shade_query(false, 1, &u0, &u0, out, dir, dir, &pdf, &u0, nullptr, out); }) == B200PT_ERR_NO_SCENE &&
+                       code([&] { e.bounce_query(1, out, 0, out, &survivors); }) == B200PT_ERR_NO_SCENE, "refused without the map or the tables", k);
+            };
+
+            each_failure("set_env_map", [&] { e.set_env_map(4, 2, rgba.data()); }, [&](long k, bool ok, const DevScene &, const std::set<const void *> &created) {
+                const DevScene sc = e.dev_scene();
+                if (ok) expect(e.has_env() && created == std::set<const void *>{ sc.env, sc.alias, sc.env_row_cos } && sc.envW == 4 && sc.envH == 2,
+                               "set_env_map: the view holds the new map", k);
+                else { expect(!e.has_env() && created.empty(), "failed set_env_map: no map, nothing of the call live", k); refuses(k, true); }
+            });
+            each_failure("set_luts", [&] { e.set_luts(lut[0].data(), lut[1].data(), lut[2].data()); }, [&](long k, bool ok, const DevScene &, const std::set<const void *> &created) {
+                const DevScene sc = e.dev_scene();
+                if (ok) expect(e.has_luts() && created == std::set<const void *>{ sc.lut_reflect, sc.lut_refract_out, sc.lut_refract_in }, "set_luts: the view holds the new tables", k);
+                else { expect(!e.has_luts() && created.empty(), "failed set_luts: no tables, nothing of the call live", k); refuses(k, false); }
+            });
+            m.EmissiveColor[0] = 1.0f;                             // the quad becomes an emitter: two EmTri
+            each_failure("set_material", [&] { e.set_material(0, m); }, [&](long k, bool ok, const DevScene &prev, const std::set<const void *> &created) {
+                const DevScene sc = e.dev_scene();
+                if (ok) expect(sc.n_emissive == 1 && created == std::set<const void *>{ sc.em_tris, sc.em_tri_base } && g_blocks.at((const char *)sc.em_tris).bytes == 2 * sizeof(EmTri),
+                               "set_material: the view holds the new emissive tables", k);
+                else expect(sc.n_emissive == 0 && sc.em_tris == prev.em_tris && sc.em_tri_base == prev.em_tri_base && created.empty(),
+                            "failed set_material: the previous emissive tables", k);
+            });
+        }
+        unsetenv("B200PT_BVH_SAH");
+        expect(g_live == before_engine, "engine destroyed: nothing live", 0);
+    }
     if (failures) { printf("%d failures\n", failures); return 1; }
     puts("ok");
     return 0;

@@ -1,5 +1,6 @@
-"""CPU-side checks that the host runtime releases every CUDA resource it creates, on error paths too: tests/native/alloc_faults.cpp links the
-built objects against shims of the CUDA runtime that fail the k-th creation and track every live block, event and stream (no GPU needed)."""
+"""CPU-side checks that the host runtime releases every CUDA resource it creates, on error paths too, and that the device view of the scene
+holds only live blocks after a failed update: tests/native/alloc_faults.cpp links the built objects against shims of the CUDA runtime that
+fail the k-th creation and track every live block, event and stream (no GPU needed)."""
 import glob
 import os
 import re
@@ -56,3 +57,14 @@ def test_lbvh_build_rejects_2_28_references_and_releases_every_block(alloc_fault
     allocated before the check is released."""
     n, failed = _case(alloc_faults, "lbvh_build (2^28 references)")
     assert n == 7 and failed == 0
+
+
+@pytest.mark.parametrize("name", ["set_env_map", "set_luts", "set_material"])
+def test_failed_scene_updates_leave_a_device_view_of_live_blocks(alloc_faults, name):
+    """An engine with a one-quad scene, an environment map and the lookup tables; the k-th allocation of set_env_map, set_luts or
+    set_material's emissive rebuild fails, for every k.  After each call every non-null pointer of Engine::dev_scene lies in a live block
+    and has_env / has_luts agree with the view.  A failed set_env_map / set_luts leaves no map / no tables, and path_trace and the
+    shade, miss and bounce queries refuse with B200PT_ERR_NO_SCENE; a failed emissive rebuild keeps the previous tables; a successful call
+    leaves exactly its new blocks, in the view."""
+    n, failed = _case(alloc_faults, name)
+    assert n == (2 if name == "set_material" else 3) and failed == 0

@@ -87,7 +87,7 @@ void Engine::free_scene() {
     d_verts_.reset(); d_indices_.reset(); d_meshes_.reset(); d_instances_.reset(); d_materials_.reset(); d_textures_.reset(); d_emissive_.reset();
     d_em_tris_.reset(); d_em_tri_base_.reset(); d_tri_class_.reset();
     d_texdata_.clear();
-    bvh_ = {};
+    tree_ = {};
     free_pose_data();
     has_scene_ = false;
 }
@@ -136,6 +136,7 @@ void Engine::upload_scene() {
     }
     CK(alloc(d_emissive_, std::max<size_t>(1, scene_.instances.size()) * sizeof(DevEmissive)));
     rebuild_emissive();
+    upload_instances();
     // textures
     std::vector<DevTexture> dt(scene_.textures.size());
     d_texdata_.resize(scene_.textures.size());
@@ -146,12 +147,14 @@ void Engine::upload_scene() {
         dt[i] = { d_texdata_[i].get(), t.width, t.height, t.channels, 0 };
     }
     CK(alloc(d_textures_, dt.size() * sizeof(DevTexture))); CK(cudaMemcpy(d_textures_.get(), dt.data(), dt.size() * sizeof(DevTexture), cudaMemcpyHostToDevice));
-    ds_.verts = d_verts_.get(); ds_.indices = d_indices_.get(); ds_.meshes = d_meshes_.get(); ds_.instances = d_instances_.get(); ds_.materials = d_materials_.get();
     CK(alloc(d_tri_class_, std::max<size_t>(1, n_tris_)));
     rebuild_tri_class();
-    ds_.textures = d_textures_.get(); ds_.emissive = d_emissive_.get();
-    build_bvh(&bvh_, &ds_, &lc_);
+    tree_ = build_bvh();
     upload_pose_data();
+}
+
+void Engine::upload_instances() {
+    CK(cudaMemcpy(d_instances_.get(), h_instances_.data(), h_instances_.size() * sizeof(DevInstance), cudaMemcpyHostToDevice));
 }
 
 // DevInstance of every instance from scene_.instances (o2w = rows 0-2 of the column-major Transform, w2o its inverse); emissive_tri_count is
@@ -170,10 +173,11 @@ void Engine::fill_instances() {
     n_tris_ = tri_base;
 }
 
-// The acceleration structure of the instances in d_instances_, built into *out: the BVH fields of *ds and the launch configuration *lc are set
-// from it (moving *out keeps them valid).  set_scene and update_instance_transforms(rebuild) both use it.
-// gpu_builder: the tree is built on the device (PLOC over the LBVH's references, ploc.cu) instead of by the host tree-quality passes.
-void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_builder) {
+// The acceleration structure of the instances in d_instances_ and its launch configuration.  set_scene and update_instance_transforms(rebuild)
+// both use it.  gpu_builder: the tree is built on the device (PLOC over the LBVH's references, ploc.cu) instead of by the host tree-quality passes.
+Engine::SceneTree Engine::build_bvh(bool gpu_builder) {
+    SceneTree tree;
+    LbvhResult *const out = &tree.bvh;
     // acceleration structure: GPU LBVH over the flattened instances
     // tree-quality pass over the GPU LBVH: same hits, fewer node visits / triangle tests.  Level 3 (full binned-SAH build + insertion-based
     // refinement) is the default;
@@ -195,22 +199,28 @@ void Engine::build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_bu
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refine_sah failed: ") + cudaGetErrorString((cudaError_t)r) };
         if (getenv("B200PT_DEBUG")) fprintf(stderr, "[b200pt] SAH pass (mode %d): cost %.3f -> %.3f, depth %d\n", sah_mode, sah[0], sah[1], out->max_depth);
     }
-    ds->nodes = out->nodes.get(); ds->tris = out->tris; ds->shade_tris = out->shade.get(); ds->tri_slot = out->tri_slot.get();
-    ds->n_tris = out->n_tris; ds->n_nodes = out->n_nodes; ds->root = out->root; ds->bvh_bytes = out->bytes <= 0xFFFFFFFFull ? (uint32_t)out->bytes : 0;
-    ds->nodes4 = nullptr; ds->n_nodes4 = 0;
     if (out->bytes > 64u * 1024u) {                                         // scenes that traverse out of L2/HBM get the BVH4 (host collapse of the GPU-built BVH2)
         r = gpu_builder ? lbvh_build_wide_device(out, h_small_.get(), stream_) : lbvh_build_wide(out, stream_);
         if (r != 0) throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_build_wide failed: ") + cudaGetErrorString((cudaError_t)r) };
-        ds->nodes4 = out->nodes4.get(); ds->n_nodes4 = out->n_nodes4;
     }
     // A handful of triangle slots (the 12-triangle Cornell box): shared-memory traversals test them in order, no hierarchy (bvh_traverse.cuh).
     {
         uint32_t flat_max = 16;
         if (const char *e = getenv("B200PT_FLAT_MAX")) { const int v = atoi(e); if (v >= 0 && v <= 64) flat_max = (uint32_t)v; }
-        ds->n_flat = (out->n_tris <= flat_max) ? out->n_tris : 0u;
+        tree.n_flat = (out->n_tris <= flat_max) ? out->n_tris : 0u;
     }
-    int q = query_launch_cfg(*ds, out->max_depth, out->depth4, lc);
+    DevScene sc{};
+    tree.view(sc);
+    int q = query_launch_cfg(sc, out->max_depth, out->depth4, &tree.lc);
     if (q != 0) throw CudaError{ B200PT_ERR_CUDA, "query_launch_cfg failed" };
+    return tree;
+}
+
+void Engine::SceneTree::view(DevScene &sc) const {
+    sc.nodes = bvh.nodes.get(); sc.tris = bvh.tris; sc.shade_tris = bvh.shade.get(); sc.tri_slot = bvh.tri_slot.get();
+    sc.n_tris = bvh.n_tris; sc.n_nodes = bvh.n_nodes; sc.root = bvh.root; sc.bvh_bytes = bvh.bytes <= 0xFFFFFFFFull ? (uint32_t)bvh.bytes : 0;
+    sc.nodes4 = bvh.nodes4.get(); sc.n_nodes4 = bvh.n_nodes4;
+    sc.n_flat = n_flat;
 }
 
 // TLAS::Update (VulkanHelper/Source/Vulkan/TLASImpl.cpp:192-293): every instance transform replaced, the tree refit in place (rebuild == 0),
@@ -291,7 +301,8 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         }
         if (instances) { scene_.instances = old_instances; fill_instances(); }
         CK(cudaStreamSynchronize(stream_));
-        rebuild_emissive();                                     // DevEmissive::xf, the world-space EmTri, and d_instances_ (o2w / w2o)
+        rebuild_emissive();                                     // DevEmissive::xf, the world-space EmTri
+        upload_instances();
     };
     try {
         for (const VertexSource &s : src) {
@@ -309,7 +320,8 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         }
         if (instances) { scene_.instances = *instances; fill_instances(); }
         CK(cudaStreamSynchronize(stream_));
-        rebuild_emissive();                                     // the world-space EmTri, from the mirror; d_instances_
+        rebuild_emissive();                                     // the world-space EmTri, from the mirror
+        upload_instances();
     } catch (...) {
         try { restore(); } catch (...) { has_scene_ = false; }
         throw;
@@ -319,9 +331,9 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
         for (size_t a = 0; a < h_instances_.size(); a++) if (listed[h_instances_[a].mesh]) changed.push_back((uint32_t)a);
         uint32_t *const d_list = src.empty() ? nullptr : static_cast<uint32_t *>(scratch((2 * changed.size() + 1) * sizeof(uint32_t)));
         auto refit = [&]() {
-            int r = lbvh_refit(&bvh_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), stream_);
+            int r = lbvh_refit(&tree_.bvh, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), (uint32_t)h_instances_.size(), stream_);
             if (r == 0 && !src.empty())
-                r = lbvh_refresh_shade(&bvh_, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), changed.data(),
+                r = lbvh_refresh_shade(&tree_.bvh, d_verts_.get(), d_indices_.get(), d_meshes_.get(), d_instances_.get(), h_instances_.data(), h_meshes_.data(), changed.data(),
                                        (uint32_t)changed.size(), d_list, stream_);
             return r;
         };
@@ -331,10 +343,10 @@ void Engine::commit(const std::vector<VertexSource> &src, const std::vector<b200
             throw CudaError{ B200PT_ERR_CUDA, std::string("lbvh_refit failed: ") + cudaGetErrorString((cudaError_t)r) };
         }
     } else {
-        LbvhResult fresh{}; DevScene ds = ds_; LaunchCfg lc = lc_;
-        try { build_bvh(&fresh, &ds, &lc, rebuild == B200PT_REBUILD_GPU); }
+        SceneTree fresh;
+        try { fresh = build_bvh(rebuild == B200PT_REBUILD_GPU); }
         catch (...) { try { restore(); } catch (...) { has_scene_ = false; } throw; }
-        bvh_ = std::move(fresh); ds_ = ds; lc_ = lc;
+        tree_ = std::move(fresh);
     }
     reset();
 }
@@ -475,28 +487,23 @@ void Engine::rebuild_tri_class() {
         if (cnt) { class_mask_ |= 1u << c; std::fill(tc.begin() + first, tc.begin() + first + cnt, c); }
     }
     CK(cudaMemcpy(d_tri_class_.get(), tc.data(), tc.size(), cudaMemcpyHostToDevice));
-    ds_.tri_class = d_tri_class_.get();
-    ds_.uniform_class = 0xFFu;
-    for (uint32_t c = 0; c < MC_COUNT; c++) if (class_mask_ == (1u << c)) ds_.uniform_class = c;
 }
 
-// emissive-mesh list: PathTracer.cpp:458-469 (+ SetMaterial maintenance :712-810); keyed on constant EmissiveColor != 0 (Q16)
+// emissive-mesh list: PathTracer.cpp:458-469 (+ SetMaterial maintenance :712-810); keyed on constant EmissiveColor != 0 (Q16).
+// The emissive records, tables and counts change together, after every upload has succeeded; d_instances_ (which carries the counts) is the
+// caller's to upload.
 void Engine::rebuild_emissive() {
     std::vector<DevEmissive> em;
     for (size_t i = 0; i < scene_.instances.size(); i++) {
         const b200pt_instance &in = scene_.instances[i];
         const b200pt_material &m = scene_.materials[in.MaterialIndex];
-        h_instances_[i].emissive_tri_count = 0;
         if (m.EmissiveColor[0] != 0.0f || m.EmissiveColor[1] != 0.0f || m.EmissiveColor[2] != 0.0f) {
             DevEmissive e; e.mesh = in.MeshIndex; e.material = in.MaterialIndex; e.tri_count = h_meshes_[in.MeshIndex].tri_count; e.instance = (uint32_t)i;
             memcpy(e.xf, in.Transform, sizeof e.xf);
             em.push_back(e);
-            h_instances_[i].emissive_tri_count = e.tri_count;
         }
     }
     if (em.size() >= 10000) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "too many emissive meshes (MAX_EMISSIVE_MESHES)" };
-    n_emissive_ = (uint32_t)em.size();
-    if (!em.empty()) CK(cudaMemcpy(d_emissive_.get(), em.data(), em.size() * sizeof(DevEmissive), cudaMemcpyHostToDevice));
     // world-space emissive triangles (SH/Sampler.slang:376-391: vertices fetched and transformed per sample in the reference)
     std::vector<EmTri> et; std::vector<uint32_t> base;
     for (const DevEmissive &e : em) {
@@ -517,13 +524,15 @@ void Engine::rebuild_emissive() {
             et.push_back(r);
         }
     }
-    d_em_tris_.reset(); d_em_tri_base_.reset();
-    CK(alloc(d_em_tris_, std::max<size_t>(1, et.size()) * sizeof(EmTri))); CK(alloc(d_em_tri_base_, std::max<size_t>(1, base.size()) * sizeof(uint32_t)));
-    if (!et.empty()) CK(cudaMemcpy(d_em_tris_.get(), et.data(), et.size() * sizeof(EmTri), cudaMemcpyHostToDevice));
-    if (!base.empty()) CK(cudaMemcpy(d_em_tri_base_.get(), base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    ds_.em_tris = d_em_tris_.get(); ds_.em_tri_base = d_em_tri_base_.get();
-    CK(cudaMemcpy(d_instances_.get(), h_instances_.data(), h_instances_.size() * sizeof(DevInstance), cudaMemcpyHostToDevice));
-    ds_.n_emissive = n_emissive_;
+    DevPtr<EmTri> em_tris; DevPtr<uint32_t> em_tri_base;
+    CK(alloc(em_tris, std::max<size_t>(1, et.size()) * sizeof(EmTri))); CK(alloc(em_tri_base, std::max<size_t>(1, base.size()) * sizeof(uint32_t)));
+    if (!et.empty()) CK(cudaMemcpy(em_tris.get(), et.data(), et.size() * sizeof(EmTri), cudaMemcpyHostToDevice));
+    if (!base.empty()) CK(cudaMemcpy(em_tri_base.get(), base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (!em.empty()) CK(cudaMemcpy(d_emissive_.get(), em.data(), em.size() * sizeof(DevEmissive), cudaMemcpyHostToDevice));
+    d_em_tris_ = std::move(em_tris); d_em_tri_base_ = std::move(em_tri_base);
+    n_emissive_ = (uint32_t)em.size();
+    for (DevInstance &d : h_instances_) d.emissive_tri_count = 0;
+    for (const DevEmissive &e : em) h_instances_[e.instance].emissive_tri_count = e.tri_count;
 }
 
 void Engine::set_material(uint32_t idx, const b200pt_material &m) {
@@ -536,6 +545,7 @@ void Engine::set_material(uint32_t idx, const b200pt_material &m) {
     scene_.materials[idx] = m;
     { const DevMaterial dm = make_dev_material(m); CK(cudaMemcpy(d_materials_.get() + idx, &dm, sizeof dm, cudaMemcpyHostToDevice)); launch_prepare_materials(d_materials_.get(), idx, 1, stream_); CK(cudaStreamSynchronize(stream_)); }
     rebuild_emissive();
+    upload_instances();
     rebuild_tri_class();
     reset();
 }
@@ -575,8 +585,6 @@ void Engine::upload_volumes() {
     }
     if (!dv.empty()) CK(cudaMemcpy(d_volumes_.get(), dv.data(), dv.size() * sizeof(DevVolume), cudaMemcpyHostToDevice));
     if (!dg.empty()) CK(cudaMemcpy(d_grids_.get(), dg.data(), dg.size() * sizeof(DevGrid), cudaMemcpyHostToDevice));
-    ds_.volumes = d_volumes_.get(); ds_.n_volumes = (uint32_t)dv.size(); ds_.phase_function = phase_function_;
-    ds_.grids = d_grids_.get(); ds_.n_grids = (uint32_t)dg.size();
     reset();
 }
 // the three READ-ONLY members of b200pt_volume follow the density data attached to the index, whatever the caller's struct says
@@ -633,7 +641,7 @@ void Engine::remove_density_data(uint32_t idx) {                                
 }
 void Engine::set_phase_function(uint32_t pf) {
     if (pf > 2u) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "phase function: 0 HG, 1 Draine, 2 HG + Draine" };
-    phase_function_ = pf; ds_.phase_function = pf; reset();
+    phase_function_ = pf; reset();
 }
 
 // PathTracer::LoadEnvironmentMap (PathTracer.cpp:1137-1332)
@@ -644,17 +652,17 @@ void Engine::set_env_map(uint32_t w, uint32_t h, const float *rgba) {
     std::vector<float> px(rgba, rgba + (size_t)w * h * 4);
     std::vector<uint2> alias((size_t)w * h);
     build_env_alias(px.data(), w, h, alias.data());
+    // The previous map is released first; the new one is filled in local owners and moved in once every upload has succeeded.
     d_env_.reset(); d_alias_.reset(); d_env_row_cos_.reset();
+    DevPtr<float4> d_env; DevPtr<uint2> d_alias; DevPtr<float2> d_row_cos;
     {   // SH/Sampler.slang:329-331: stepTheta = M_PI / height; theta0 = py * stepTheta; cos(theta0), cos(theta0 + stepTheta)
         std::vector<float2> rc(h); const float stepTheta = 3.1415926535897F / (float)h;
         for (uint32_t y = 0; y < h; y++) { const float t0 = (float)y * stepTheta; rc[y] = make_float2(cosf(t0), cosf(t0 + stepTheta)); }
-        CK(alloc(d_env_row_cos_, rc.size() * sizeof(float2))); CK(cudaMemcpy(d_env_row_cos_.get(), rc.data(), rc.size() * sizeof(float2), cudaMemcpyHostToDevice));
-        ds_.env_row_cos = d_env_row_cos_.get();
+        CK(alloc(d_row_cos, rc.size() * sizeof(float2))); CK(cudaMemcpy(d_row_cos.get(), rc.data(), rc.size() * sizeof(float2), cudaMemcpyHostToDevice));
     }
-    CK(alloc(d_env_, px.size() * 4)); CK(cudaMemcpy(d_env_.get(), px.data(), px.size() * 4, cudaMemcpyHostToDevice));
-    CK(alloc(d_alias_, alias.size() * sizeof(uint2))); CK(cudaMemcpy(d_alias_.get(), alias.data(), alias.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    ds_.env = d_env_.get(); ds_.alias = d_alias_.get(); ds_.envW = w; ds_.envH = h;
-    has_env_ = true;
+    CK(alloc(d_env, px.size() * 4)); CK(cudaMemcpy(d_env.get(), px.data(), px.size() * 4, cudaMemcpyHostToDevice));
+    CK(alloc(d_alias, alias.size() * sizeof(uint2))); CK(cudaMemcpy(d_alias.get(), alias.data(), alias.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    d_env_ = std::move(d_env); d_alias_ = std::move(d_alias); d_env_row_cos_ = std::move(d_row_cos); env_w_ = w; env_h_ = h;
     reset();
 }
 
@@ -663,9 +671,10 @@ void Engine::set_luts(const float *refl, const float *rout, const float *rin) {
     if (!refl || !rout || !rin) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "null LUT" };
     sync_all();
     const size_t n[3] = { 64 * 64 * 32, 128 * 128 * 32, 128 * 128 * 32 }; const float *src[3] = { refl, rout, rin };
-    for (int i = 0; i < 3; i++) { CK(alloc(d_luts_[i], n[i] * 4)); CK(cudaMemcpy(d_luts_[i].get(), src[i], n[i] * 4, cudaMemcpyHostToDevice)); }
-    ds_.lut_reflect = d_luts_[0].get(); ds_.lut_refract_out = d_luts_[1].get(); ds_.lut_refract_in = d_luts_[2].get();
-    has_luts_ = true;
+    // Each previous table is released before its replacement is allocated; the new ones are moved in once every upload has succeeded.
+    DevPtr<float> luts[3];
+    for (int i = 0; i < 3; i++) { d_luts_[i].reset(); CK(alloc(luts[i], n[i] * 4)); CK(cudaMemcpy(luts[i].get(), src[i], n[i] * 4, cudaMemcpyHostToDevice)); }
+    for (int i = 0; i < 3; i++) d_luts_[i] = std::move(luts[i]);
     reset();
 }
 
@@ -808,6 +817,24 @@ void Engine::ensure_wave(size_t cap, int contexts) {
     wave_cap_ = cap;
 }
 
+DevScene Engine::dev_scene() const {
+    DevScene sc{};
+    sc.verts = d_verts_.get(); sc.indices = d_indices_.get(); sc.meshes = d_meshes_.get(); sc.instances = d_instances_.get();
+    sc.materials = d_materials_.get(); sc.textures = d_textures_.get(); sc.tri_class = d_tri_class_.get();
+    sc.uniform_class = 0xFFu;
+    for (uint32_t c = 0; c < MC_COUNT; c++) if (class_mask_ == (1u << c)) sc.uniform_class = c;
+    sc.emissive = d_emissive_.get(); sc.em_tris = d_em_tris_.get(); sc.em_tri_base = d_em_tri_base_.get(); sc.n_emissive = n_emissive_;
+    tree_.view(sc);
+    sc.env = d_env_.get(); sc.alias = d_alias_.get(); sc.env_row_cos = d_env_row_cos_.get(); sc.envW = env_w_; sc.envH = env_h_;
+    sc.lut_reflect = d_luts_[0].get(); sc.lut_refract_out = d_luts_[1].get(); sc.lut_refract_in = d_luts_[2].get();
+    if (d_volumes_ && d_grids_) {                       // both allocated by the first upload_volumes
+        sc.volumes = d_volumes_.get(); sc.n_volumes = (uint32_t)volumes_.size();
+        sc.grids = d_grids_.get(); sc.n_grids = (uint32_t)std::count_if(grids_.begin(), grids_.end(), [](const auto &g) { return g != nullptr; });
+    }
+    sc.phase_function = phase_function_;
+    return sc;
+}
+
 DevConfig Engine::make_dev_config() const {
     DevConfig d; memset(&d, 0, sizeof d);
     memcpy(d.VI, view_inv_, sizeof d.VI); memcpy(d.PI, proj_inv_, sizeof d.PI);
@@ -838,15 +865,15 @@ bool Engine::scene_has_media() const {
 }
 
 // One bounce of path_trace's loop; bounce_query runs the same sequence on caller-given paths.
-uint64_t Engine::bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
+uint64_t Engine::bounce(const CallPlan &cp, const DevScene &sc, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
                         const std::function<void(int)> &mark) {
     const uint32_t par = k & 1u;
     const Queues q{ B.q_miss, B.q_hit, (uint32_t)wave_cap_ };
     uint64_t launches = 0;
-    if (cp.pre) launches += launch_volume_decide(lc_, ds_, dc, pst[cur], B.so, B.counts.get(), par, B.sample_buf, B.rng_carry, st);
-    if (!(cp.camera && k == 0)) launches += launch_extend(lc_, cp, ds_, pst[cur], B.so.hit, B.counts.get(), par, q, d_ctr_.get(), k == 0, st); mark(1);
-    launches += launch_shade(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(2);
-    if (!cp.fuse) launches += launch_connect(lc_, cp, ds_, dc, pst[cur], pst[cur ^ 1], B.so, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(3);
+    if (cp.pre) launches += launch_volume_decide(tree_.lc, sc, dc, pst[cur], B.so, B.counts.get(), par, B.sample_buf, B.rng_carry, st);
+    if (!(cp.camera && k == 0)) launches += launch_extend(tree_.lc, cp, sc, pst[cur], B.so.hit, B.counts.get(), par, q, d_ctr_.get(), k == 0, st); mark(1);
+    launches += launch_shade(tree_.lc, cp, sc, dc, pst[cur], pst[cur ^ 1], B.so, B.so.hit, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(2);
+    if (!cp.fuse) launches += launch_connect(tree_.lc, cp, sc, dc, pst[cur], pst[cur ^ 1], B.so, B.counts.get(), par, q, B.sample_buf, B.rng_carry, d_ctr_.get(), flags, st); mark(3);
     return launches;
 }
 
@@ -854,8 +881,8 @@ uint64_t Engine::bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, con
 bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "PathTrace before SetScene" };
-    if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "no environment map (PathTracer always loads one, PathTracer.cpp:202)" };
-    if (!has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "no energy-compensation lookup tables (PathTracer.cpp:199-201)" };
+    if (!has_env()) throw CudaError{ B200PT_ERR_NO_SCENE, "no environment map (PathTracer always loads one, PathTracer.cpp:202)" };
+    if (!has_luts()) throw CudaError{ B200PT_ERR_NO_SCENE, "no energy-compensation lookup tables (PathTracer.cpp:199-201)" };
     const uint32_t S = cfg_.ScreenChunkCount, S2 = S * S;
     const bool adaptive = adaptive_.Enable != 0u;              // S == 1 (set_config / set_adaptive / set_track_variance)
     const bool tracked = records();                           // statistics without adaptive sampling: the records over the identity list, no decisions
@@ -907,8 +934,9 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
     auto pcg = [](uint32_t in) { uint32_t st = in * 747796405u + 2891336453u; uint32_t w = ((st >> ((st >> 28u) + 4u)) ^ st) * 277803737u; return (w >> 22u) ^ w; };
 
     const bool medium = scene_has_media();
-    const CallPlan cp = plan_call(lc_, ds_, dc, medium, class_mask_);
-    ds_.pre_pass = cp.pre ? 1u : 0u;
+    DevScene sc = dev_scene();
+    const CallPlan cp = plan_call(tree_.lc, sc, dc, medium, class_mask_);
+    sc.pre_pass = cp.pre ? 1u : 0u;
     const uint32_t implied_flag = cp.implied ? WAVE_IMPLIED : 0u;   // per-launch flags: kernels.h
     const uint32_t qcap = (uint32_t)wave_cap_;
 
@@ -947,15 +975,15 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
             CK(cudaMemcpyAsync(B.d_disp.get(), B.h_disp.get(), nd * sizeof(DevDispatch), cudaMemcpyHostToDevice, st));
             CK(cudaEventRecord(B.disp_ev.get(), st));
             PathState pst[2] = { B.ps[0], B.ps[1] };              // payload.VolumeDepth travels only while the scene has volumes
-            if (!ds_.n_volumes) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
+            if (!sc.n_volumes) { pst[0].vol_depth = nullptr; pst[1].vol_depth = nullptr; }
             const Queues q{ B.q_miss, B.q_hit, qcap };
             for (uint32_t s = 0; s < cfg_.SamplesPerFrame; s++) {
                 const uint32_t wflags = (s == 0 && cp.store ? WAVE_STORE : 0u) | (s + 1 < cfg_.SamplesPerFrame ? WAVE_CARRY : 0u);
                 if (cp.camera) {
                     CK(cudaMemsetAsync(B.counts.get(), 0, CTRL_WORDS * sizeof(uint32_t), st));   // before any CTA appends to the parity-0 queues
-                    launches += launch_camera(lc_, cp, ds_, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
+                    launches += launch_camera(tree_.lc, cp, sc, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags | implied_flag, B.rng_carry, pst[0], B.sample_buf, B.so.hit,
                                               B.counts.get(), q, d_ctr_.get(), st, act);
-                } else launches += launch_raygen(lc_, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts.get(), d_ctr_.get(), st, act);
+                } else launches += launch_raygen(tree_.lc, dc, B.d_disp.get(), nd, Pw, s == 0 ? 1u : 0u, wflags, B.rng_carry, pst[0], B.sample_buf, B.counts.get(), d_ctr_.get(), st, act);
                 mark(0);
                 int cur = 0; uint32_t k = 0;
                 for (;;) {
@@ -963,7 +991,7 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                     if (!medium && cfg_.MaxDepth - std::min(cfg_.MaxDepth, k) < chunk) chunk = cfg_.MaxDepth - std::min(cfg_.MaxDepth, k);
                     if (chunk == 0) break;
                     for (uint32_t b = 0; b < chunk; b++, k++) {
-                        launches += bounce(cp, dc, B, pst, cur, k, wflags | (k == 0 ? implied_flag : 0u), st, mark);
+                        launches += bounce(cp, sc, dc, B, pst, cur, k, wflags | (k == 0 ? implied_flag : 0u), st, mark);
                         cur ^= 1;
                     }
                     if (!medium && k >= cfg_.MaxDepth) break;    // every surviving path has Depth >= MaxDepth: provably empty
@@ -980,8 +1008,8 @@ bool Engine::path_trace(uint32_t dispatches, uint32_t base_seed) {
                 if (wave_seq_ > 0) CK(cudaStreamWaitEvent(st, resolved_ev_[ctx ^ 1].get(), 0));
                 CK(cudaStreamWaitEvent(st, image_free_ev_.get(), 0));
             }
-            if (tracked) launch_resolve_adaptive(lc_, dc, nd, Pw, d_active_.get(), B.sample_buf, d_image_.get(), d_px_state_.get(), st);
-            else launch_resolve(lc_, dc, B.d_disp.get(), nd, P, B.sample_buf, d_image_.get(), st);
+            if (tracked) launch_resolve_adaptive(tree_.lc, dc, nd, Pw, d_active_.get(), B.sample_buf, d_image_.get(), d_px_state_.get(), st);
+            else launch_resolve(tree_.lc, dc, B.d_disp.get(), nd, P, B.sample_buf, d_image_.get(), st);
             CK(cudaEventRecord(resolved_ev_[ctx].get(), st));
             wave_seq_++;
             launches++; waves++; mark(4);
@@ -1124,7 +1152,7 @@ void Engine::accumulate_rows(const float4 *d_frame, uint32_t frame_index, uint32
     CK(cudaSetDevice(device_));
     if (!d_image_ || !d_frame || y0 >= y1 || y1 > H_ || world_ != 1) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "accumulate_rows: no image / bad rows / partitioned image" };
     join_waves();
-    launch_accumulate(d_frame, d_image_.get(), y0 * W_, (y1 - y0) * W_, frame_index, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);
+    launch_accumulate(d_frame, d_image_.get(), y0 * W_, (y1 - y0) * W_, frame_index, tree_.lc.grid_light > 0 ? tree_.lc.grid_light : 1184, stream_);
     CK(cudaGetLastError());
 }
 // HDR rows read by post_process_rows(y0, y1): the final kernel's rows y0-1 .. y1-1 and the first down pass's taps 2y-2 .. 2y+1 over D[1]
@@ -1195,7 +1223,7 @@ void Engine::post_chain(const float4 *src, uint32_t y0, uint32_t y1) {
         launch_bloom_final(src, d_mips_[1].get(), mip_wh_[2], mip_wh_[3], d_ldr_.get(), (keep_bloom_ && whole) ? d_mips_[0].get() : nullptr, W_, H_, p, stream_, whole ? nullptr : r);   // last up pass + :238-245
         bloom_valid_ = keep_bloom_ && whole;
     } else {
-        launch_bloom_threshold(src, d_mips_[0].get(), W_ * H_, p, lc_.grid_light > 0 ? lc_.grid_light : 1184, stream_);            // :200-226, i == 0
+        launch_bloom_threshold(src, d_mips_[0].get(), W_ * H_, p, tree_.lc.grid_light > 0 ? tree_.lc.grid_light : 1184, stream_);            // :200-226, i == 0
         for (uint32_t i = 1; i < mips; i++) launch_bloom_down(d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], p, stream_);
         for (uint32_t i = mips - 1; i > 0; i--) launch_bloom_up(d_mips_[i].get(), mip_wh_[2 * i], mip_wh_[2 * i + 1], d_mips_[i - 1].get(), mip_wh_[2 * (i - 1)], mip_wh_[2 * (i - 1) + 1], p, stream_);   // :229-235
         launch_tonemap(src, d_mips_[0].get(), d_ldr_.get(), W_, H_, p, stream_);                           // :238-245
@@ -1232,7 +1260,7 @@ void Engine::volume_walks(uint32_t n, const float *org, const float *dir, const 
     sync_all();
     DeviceBlocks a(stream_);
     float *d_T = a.out<float>(n), *d_s = a.out<float>(n); int32_t *d_v = a.out<int32_t>(n); uint32_t *d_r = a.out<uint32_t>(2 * (size_t)n);
-    launch_volume_walks(ds_, n, a.in(org, 3 * (size_t)n), a.in(dir, 3 * (size_t)n), a.in(seeds, n), ray_depth, d_T, d_s, d_v, d_r, stream_);
+    launch_volume_walks(dev_scene(), n, a.in(org, 3 * (size_t)n), a.in(dir, 3 * (size_t)n), a.in(seeds, n), ray_depth, d_T, d_s, d_v, d_r, stream_);
     a.get(T, d_T, n); a.get(scatter, d_s, n); a.get(vol, d_v, n); a.get(rng2, d_r, 2 * (size_t)n);
     a.sync();
 }
@@ -1241,7 +1269,7 @@ void Engine::volume_walks(uint32_t n, const float *org, const float *dir, const 
 void Engine::trace_closest(uint32_t n, const float *org, const float *dir, float tmin, float tmax, float *t, uint32_t *prim, uint32_t *inst, float *uv, uint32_t *stats) {
     const std::vector<float> lo(n, tmin), hi(n, tmax);
     std::vector<uint32_t> st3(stats ? 3 * (size_t)n : 0);
-    const int shape = lc_.bvh_in_smem ? (ds_.n_flat ? TQ_FLAT : TQ_SHARED) : TQ_GLOBAL;
+    const int shape = tree_.lc.bvh_in_smem ? (tree_.n_flat ? TQ_FLAT : TQ_SHARED) : TQ_GLOBAL;
     trace_query(shape, TQ_CLOSEST, false, n, org, dir, lo.data(), hi.data(), nullptr, nullptr, t, prim, inst, uv, nullptr, stats ? st3.data() : nullptr);
     if (stats) for (size_t i = 0; i < n; i++) { stats[2 * i] = st3[3 * i]; stats[2 * i + 1] = st3[3 * i + 1]; }
 }
@@ -1259,7 +1287,7 @@ void Engine::trace_query(int shape, int kind, bool fma, uint32_t n, const float 
     if (any) q.occluded = a.out<uint32_t>(n);
     else { q.t = a.out<float>(n); q.prim = a.out<uint32_t>(n); q.inst = a.out<uint32_t>(n); q.uv = a.out<float>(2 * (size_t)n); }
     if (stats) q.stats = a.out<uint32_t>(3 * (size_t)n);
-    const int r = launch_trace_query(lc_, ds_, bvh_.depth4, shape, kind, fma, q, stream_);
+    const int r = launch_trace_query(tree_.lc, dev_scene(), tree_.bvh.depth4, shape, kind, fma, q, stream_);
     if (r == TQ_UNSUPPORTED) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "trace_query: the scene has no such traversal shape" };
     CK((cudaError_t)r);
     if (any) a.get(occluded, q.occluded, n);
@@ -1271,9 +1299,10 @@ void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, c
                          const float *pay_pdf, const uint32_t *rng, const float *L, float *out) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
-    if (!has_env_ || !has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "shade_query: no environment map or no lookup tables" };
+    if (!has_env() || !has_luts()) throw CudaError{ B200PT_ERR_NO_SCENE, "shade_query: no environment map or no lookup tables" };
     if (!n) return;
-    if (ds_.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: scenes with volumes or the atmosphere are not supported" };
+    const DevScene sc = dev_scene();
+    if (sc.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "shade_query: scenes with volumes or the atmosphere are not supported" };
     std::vector<uint32_t> gid(n);
     for (uint32_t i = 0; i < n; i++) {                                      // (instance, primitive) -> global triangle id, as k_world_tris numbers them
         if (inst[i] >= h_instances_.size() || prim[i] >= h_meshes_[h_instances_[inst[i]].mesh].tri_count)
@@ -1289,14 +1318,14 @@ void Engine::shade_query(bool force_general, uint32_t n, const uint32_t *inst, c
     if (L) q.L = a.in(L, 3 * (size_t)n);
     const size_t out_count = (size_t)n * B200PT_SQ_STRIDE;
     q.out = a.out<float>(out_count);
-    CK((cudaError_t)launch_shade_query(ds_, make_dev_config(), q, stream_));
+    CK((cudaError_t)launch_shade_query(sc, make_dev_config(), q, stream_));
     a.get(out, q.out, out_count);
     a.sync();
 }
 void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, const float *pay_pdf, float *out) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
-    if (!has_env_) throw CudaError{ B200PT_ERR_NO_SCENE, "miss_query: no environment map" };
+    if (!has_env()) throw CudaError{ B200PT_ERR_NO_SCENE, "miss_query: no environment map" };
     if (!n) return;
     DeviceBlocks a(stream_);
     MissQuery q{};
@@ -1304,15 +1333,16 @@ void Engine::miss_query(uint32_t n, const float *dir, const uint32_t *depth, con
     q.dir = a.in(dir, 3 * (size_t)n); q.depth = a.in(depth, n); q.pay_pdf = a.in(pay_pdf, n);
     const size_t out_count = (size_t)n * B200PT_MQ_STRIDE;
     q.out = a.out<float>(out_count);
-    CK((cudaError_t)launch_miss_query(ds_, make_dev_config(), q, stream_));
+    CK((cudaError_t)launch_miss_query(dev_scene(), make_dev_config(), q, stream_));
     a.get(out, q.out, out_count);
     a.sync();
 }
 void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *out, uint32_t *survivors) {
     CK(cudaSetDevice(device_));
     if (!has_scene_) throw CudaError{ B200PT_ERR_NO_SCENE, "no scene" };
-    if (!has_env_ || !has_luts_) throw CudaError{ B200PT_ERR_NO_SCENE, "bounce_query: no environment map or no lookup tables" };
-    if (ds_.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: scenes with volumes or the atmosphere are not supported" };
+    if (!has_env() || !has_luts()) throw CudaError{ B200PT_ERR_NO_SCENE, "bounce_query: no environment map or no lookup tables" };
+    DevScene sc = dev_scene();
+    if (sc.n_volumes != 0u || atmosphere_.Enable) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: scenes with volumes or the atmosphere are not supported" };
     static_assert(B200PT_BQ_STORE == WAVE_STORE && B200PT_BQ_CARRY == WAVE_CARRY, "bounce_query flags are the wave flags");
     if (flags & ~(uint32_t)(B200PT_BQ_STORE | B200PT_BQ_CARRY)) throw CudaError{ B200PT_ERR_WRONG_ARGUMENTS, "bounce_query: unknown flag bits" };
     *survivors = 0;
@@ -1357,9 +1387,9 @@ void Engine::bounce_query(uint32_t n, const float *in, uint32_t flags, float *ou
     CK(cudaStreamSynchronize(stream_));                       // (the pageable sources above are copied by now)
 
     const DevConfig dc = make_dev_config();
-    const CallPlan cp = plan_call(lc_, ds_, dc, scene_has_media(), class_mask_);
-    ds_.pre_pass = 0u;
-    last_.kernel_launches += bounce(cp, dc, B, pst, cur, k, flags, stream_, [](int) {});
+    const CallPlan cp = plan_call(tree_.lc, sc, dc, scene_has_media(), class_mask_);
+    sc.pre_pass = 0u;
+    last_.kernel_launches += bounce(cp, sc, dc, B, pst, cur, k, flags, stream_, [](int) {});
 
     std::vector<float4> hit(n), nx_op(n), nx_dr(n), nx_td(n), nx_rs(n), nx_med(n);
     std::vector<float> nx_g(n);
@@ -1465,7 +1495,7 @@ void Engine::run_features(const b200pt_denoise_params &p) {
     for (int k = 0; k < 3; k++) d[k] = (VI[k] * t[0] + VI[4 + k] * t[1] + VI[8 + k] * t[2]) / tl;
     const double dl = std::sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
     const float3 fwd = make_float3((float)(d[0] / dl), (float)(d[1] / dl), (float)(d[2] / dl));
-    CK((cudaError_t)launch_features(lc_, ds_, make_dev_config(), fwd, p.FeatureSamples, pcg_host(0x46454154u), d_dn_.get(), d_dn_.get() + n, stream_));
+    CK((cudaError_t)launch_features(tree_.lc, dev_scene(), make_dev_config(), fwd, p.FeatureSamples, pcg_host(0x46454154u), d_dn_.get(), d_dn_.get() + n, stream_));
     launch_record_variance(d_px_state_.get(), (uint32_t)n, reinterpret_cast<float *>(d_dn_.get() + 6 * n), stream_);
     CK(cudaGetLastError());
 }
@@ -1541,7 +1571,7 @@ void Engine::post_process_denoised() {
     post_denoised_ = true;
 }
 void Engine::scene_stats(uint32_t *tris, uint32_t *nodes, uint32_t *emissive, uint32_t *textures) const {
-    if (tris) *tris = n_tris_; if (nodes) *nodes = bvh_.n_nodes; if (emissive) *emissive = n_emissive_; if (textures) *textures = (uint32_t)scene_.textures.size();
+    if (tris) *tris = n_tris_; if (nodes) *nodes = tree_.bvh.n_nodes; if (emissive) *emissive = n_emissive_; if (textures) *textures = (uint32_t)scene_.textures.size();
 }
 
 // The launchers update_instance_transforms(B200PT_REBUILD_GPU) runs, on the caller's boxes in the given order (no scene needed).  Rejects what

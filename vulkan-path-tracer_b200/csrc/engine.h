@@ -43,6 +43,11 @@ public:
     const b200pt_atmosphere &atmosphere() const { return atmosphere_; }
     const HostScene &scene() const { return scene_; }
     bool has_scene() const { return has_scene_; }
+    bool has_env() const { return d_env_ && d_alias_ && d_env_row_cos_; }       // set_env_map has succeeded
+    bool has_luts() const { return d_luts_[0] && d_luts_[1] && d_luts_[2]; }    // set_luts has succeeded
+    // The device view of the scene that every launch reads, each field taken from the owner of its data or the host fact it depends on.
+    // pre_pass is 0: path_trace sets it on its own copy.
+    DevScene dev_scene() const;
     void set_camera(const float vi[16], const float pi[16]);
     void get_camera(float vi[16], float pi[16]) const;
     void resize(uint32_t w, uint32_t h);
@@ -117,10 +122,16 @@ public:
     std::string last_error;
 
 private:
+    // The acceleration structure and what is decided when it is built: the launch configuration and the flat walk (B200PT_FLAT_MAX).
+    struct SceneTree {
+        LbvhResult bvh{}; LaunchCfg lc{}; uint32_t n_flat = 0;
+        void view(DevScene &sc) const;              // the tree's fields of a DevScene
+    };
     void free_scene();
     void upload_scene();
     void fill_instances();                          // h_instances_ and n_tris_ from scene_.instances
-    void build_bvh(LbvhResult *out, DevScene *ds, LaunchCfg *lc, bool gpu_builder = false);   // the BVH half of upload_scene
+    void upload_instances();                        // d_instances_ from h_instances_ (o2w / w2o, emissive_tri_count)
+    SceneTree build_bvh(bool gpu_builder = false);  // the BVH half of upload_scene
     void rebuild_emissive();
     void rebuild_tri_class();                       // per-triangle shading class (MaterialClass) + the set of classes present in the scene
     void upload_volumes();
@@ -142,26 +153,25 @@ private:
     bool timed_ = false;                            // ev_ have been recorded (by a path_trace call that launched work)
 
     HostScene scene_;
-    bool has_scene_ = false, has_env_ = false, has_luts_ = false;
+    bool has_scene_ = false;
     b200pt_config cfg_;
     float view_inv_[16], proj_inv_[16];
     uint32_t W_ = 0, H_ = 0, rank_ = 0, world_ = 1, band_ = 16, local_rows_ = 0;
     uint64_t dispatch_count_ = 0;
     uint32_t frame_count_ = 0, samples_accumulated_ = 0;
 
-    // device scene
-    DevScene ds_{};
+    // device scene (dev_scene() is its view)
     DevPtr<b200pt_vertex> d_verts_; DevPtr<uint32_t> d_indices_; DevPtr<DevMesh> d_meshes_; DevPtr<DevInstance> d_instances_;
     DevPtr<DevMaterial> d_materials_; DevPtr<DevTexture> d_textures_; DevPtr<DevEmissive> d_emissive_; DevPtr<EmTri> d_em_tris_; DevPtr<uint32_t> d_em_tri_base_;
     std::vector<DevPtr<uint8_t>> d_texdata_;
     std::vector<DevInstance> h_instances_; std::vector<DevMesh> h_meshes_;
-    DevPtr<float4> d_env_; DevPtr<uint2> d_alias_; DevPtr<float2> d_env_row_cos_; DevPtr<float> d_luts_[3];
+    DevPtr<float4> d_env_; DevPtr<uint2> d_alias_; DevPtr<float2> d_env_row_cos_; uint32_t env_w_ = 0, env_h_ = 0; DevPtr<float> d_luts_[3];
     std::vector<b200pt_volume> volumes_; uint32_t phase_function_ = 0; DevPtr<DevVolume> d_volumes_;
     struct GridData { PreparedGrid host; DevPtr<float> d_values, d_max_densities; };
     std::vector<std::shared_ptr<GridData>> grids_;      // parallel to volumes_: density data of the heterogeneous ones (nullptr: homogeneous)
     DevPtr<DevGrid> d_grids_; int density_data_counter_ = 0;   // PathTracer.cpp:1508-1513: slots are handed out round-robin
     b200pt_atmosphere atmosphere_{};
-    LbvhResult bvh_{};
+    SceneTree tree_{};
     PinnedPtr<uint32_t> h_small_;                   // pinned 4-word readback buffer of the GPU tree builder (ploc.cu)
     DevPtr<uint8_t> d_scratch_; size_t scratch_bytes_ = 0;   // scratch(): the staging buffer and shading-refresh list of update_mesh_vertices and pose
     void *scratch(size_t bytes);
@@ -177,7 +187,6 @@ private:
     std::vector<PoseMesh> pose_meshes_;             // HostAnimation::deformable order
     uint32_t pose_grid_ = 0, pose_max_joints_ = 0, pose_vertices_ = 0, pose_palette_floats_ = 0, pose_morph_floats_ = 0;
     bool pose_gen_normals_ = false;
-    LaunchCfg lc_{};
     uint32_t n_tris_ = 0, n_emissive_ = 0;
     DevPtr<uint8_t> d_tri_class_; uint32_t class_mask_ = 0;   // bit c: some triangle's material is of MaterialClass c
 
@@ -209,7 +218,7 @@ private:
     bool scene_has_media() const;                   // can a path random-walk inside a mesh without gaining Depth?
     // bounce k of a sub-wave in context B: the paths of pst[cur] (control word k & 1) are traced and shaded, the survivors written to
     // pst[cur ^ 1].  mark(kind) follows each launch group (profiling).  Returns the number of kernels enqueued on st.
-    uint64_t bounce(const CallPlan &cp, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
+    uint64_t bounce(const CallPlan &cp, const DevScene &sc, const DevConfig &dc, WaveBuf &B, const PathState pst[2], int cur, uint32_t k, uint32_t flags, cudaStream_t st,
                     const std::function<void(int)> &mark);
 
     // adaptive sampling: allocated only while enabled.  The state is rebuilt lazily (prepare_adaptive) after every reset.
